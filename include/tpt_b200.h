@@ -95,7 +95,12 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * bench.py's end-to-end leg, so that every step carries its host -> device copy),
  * "mitsuba_compare" (default 0; DO_MITSUBA_COMPARE of Config.h:25 as a runtime switch, applied by the NEXT
  * tpt_set_scene: constant sky (0.15, 0.21, 0.3) (Test.cpp:226-227) and zero Metal roughness (Test.cpp:143-145); the
- * switch's third effect, zero aperture (Test.cpp:312-313), is camera data: the Test.h shim's UpdateTest applies it). */
+ * switch's third effect, zero aperture (Test.cpp:312-313), is camera data: the Test.h shim's UpdateTest applies it),
+ * "light_sampling" (default 1; 0 = DO_LIGHT_SAMPLING 0 of Config.h:24 as a runtime switch, applied by the NEXT
+ * tpt_set_scene: no explicit light sampling at Lambert vertices (no light draws, no shadow rays, Test.cpp:95-133) and
+ * every hit adds its emission (the doMaterialE suppression of Test.cpp:209-215 is off). Exact and reference-GPU strict
+ * modes stay bit-identical to the reference built that way. The flag is part of the scene: toggling it re-uploads the
+ * scene and invalidates the exact_lookahead cache). */
 int tpt_set_option(tpt_context* ctx, const char* key, int value);
 
 /* Replaces DrawTest() (Test.cpp:344-367) for frames [frameCount, frameCount+numFrames) — numFrames*spp samples

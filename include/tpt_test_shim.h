@@ -30,6 +30,11 @@ void tpt_shim_set_mode(int mode);
  * DO_MITSUBA_COMPARE (Config.h:25; constant sky, zero Metal roughness, zero aperture). Rebuilds the scene tables; takes
  * effect with the next UpdateTest(). Environment: TPT_BIG_SCENE=0|1, TPT_MITSUBA=0|1. */
 void tpt_shim_set_variant(int bigScene, int mitsubaCompare);
+/* The reference's third compile-time switch, DO_LIGHT_SAMPLING (Config.h:24), at run time: on (default) = explicit light
+ * sampling with shadow rays; off = a plain path tracer that adds every hit's emission (Test.cpp:95-133 and :209-215
+ * compiled out). UpdateTest() passes it to tpt_set_option("light_sampling") before every tpt_set_scene(); takes effect
+ * with the next UpdateTest(). Environment: TPT_LIGHT_SAMPLING=0|1. */
+void tpt_shim_set_light_sampling(int on);
 /* Restores the un-animated scene (the reference keeps animated positions in its static arrays, Test.cpp:304-308). */
 void tpt_shim_reset_scene(void);
 /* The C-ABI context behind the shim (NULL before InitializeTest()), for tpt_set_option() etc. */

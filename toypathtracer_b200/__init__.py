@@ -345,6 +345,13 @@ def set_variant(big_scene: bool = True, mitsuba_compare: bool = False):
     _load_shim().tpt_shim_set_variant(1 if big_scene else 0, 1 if mitsuba_compare else 0)
 
 
+def set_light_sampling(on: bool = True):
+    """The reference's compile-time switch DO_LIGHT_SAMPLING (Config.h:24) at run time for the Test.h API: False renders
+    without explicit light sampling (no shadow rays; every hit adds its emission). Takes effect with the next
+    UpdateTest()."""
+    _load_shim().tpt_shim_set_light_sampling(1 if on else 0)
+
+
 def set_mode(mode: int):
     """Mode used by DrawTest(): MODE_EXACT (default, bit-identical to the reference) or MODE_FAST."""
     _load_shim().tpt_shim_set_mode(mode)

@@ -6,10 +6,11 @@
 //
 // Extra C entry points (not in Test.h) select the mode/device: tpt_shim_set_mode(), tpt_shim_context(), and the
 // reference's two compile-time scene switches as runtime ones: tpt_shim_set_variant(bigScene, mitsubaCompare)
-// (DO_BIG_SCENE Test.cpp:10-11, DO_MITSUBA_COMPARE Config.h:25).
+// (DO_BIG_SCENE Test.cpp:10-11, DO_MITSUBA_COMPARE Config.h:25), and the third one, DO_LIGHT_SAMPLING (Config.h:24),
+// as tpt_shim_set_light_sampling(on).
 // Environment: TPT_MODE=exact|fast|refgpu|refgpu_fast (default exact: results bit-identical to the reference),
 // TPT_DEVICE=<n>, TPT_PIN_BACKBUFFER=1 (cudaHostRegister the caller's backbuffer once), TPT_BIG_SCENE=0|1,
-// TPT_MITSUBA=0|1.
+// TPT_MITSUBA=0|1, TPT_LIGHT_SAMPLING=0|1.
 #include "../../include/tpt_b200.h"   // (include/tpt_test_shim.h documents this file's exports)
 #include <math.h>
 #include <stdint.h>
@@ -38,6 +39,7 @@ enum { Lambert = 0, Metal = 1, Dielectric = 2 };
 const int kMaxSphereCount = 46;
 int kSphereCount = 46;             // 46 spheres (2 emissive) with DO_BIG_SCENE, 9 spheres (1 emissive) without (Test.cpp:10)
 bool s_Mitsuba = false;            // DO_MITSUBA_COMPARE (Config.h:25)
+bool s_LightSampling = true;       // DO_LIGHT_SAMPLING (Config.h:24)
 Sphere s_Spheres[kMaxSphereCount];
 Material s_SphereMats[kMaxSphereCount];
 int s_EmissiveSpheres[kMaxSphereCount];
@@ -145,6 +147,8 @@ extern "C" void tpt_shim_set_variant(int bigScene, int mitsubaCompare)
     s_Mitsuba = mitsubaCompare != 0;
     buildScene();
 }
+// DO_LIGHT_SAMPLING at run time (on by default, like the reference's Config.h). Takes effect with the next UpdateTest().
+extern "C" void tpt_shim_set_light_sampling(int on) { s_LightSampling = on != 0; }
 extern "C" tpt_context* tpt_shim_context() { return s_Ctx; }
 
 // Test.cpp:240-246
@@ -160,6 +164,8 @@ void InitializeTest()
     const char* big = getenv("TPT_BIG_SCENE");
     const char* mit = getenv("TPT_MITSUBA");
     if (big || mit) tpt_shim_set_variant(big ? atoi(big) : (kSphereCount == 46), mit ? atoi(mit) : (int)s_Mitsuba);
+    const char* ls = getenv("TPT_LIGHT_SAMPLING");
+    if (ls) tpt_shim_set_light_sampling(atoi(ls));
     const char* d = getenv("TPT_DEVICE");
     int rc = tpt_create(d ? atoi(d) : 0, &s_Ctx);
     if (rc) die("tpt_create", rc);
@@ -205,6 +211,7 @@ void UpdateTest(float time, int frameCount, int screenWidth, int screenHeight, u
     if (s_Ctx)
     {
         tpt_set_option(s_Ctx, "mitsuba_compare", s_Mitsuba ? 1 : 0);
+        tpt_set_option(s_Ctx, "light_sampling", s_LightSampling ? 1 : 0);
         int rc = tpt_set_scene(s_Ctx, s_Spheres, s_SphereMats, kSphereCount, &s_Cam, s_EmissiveSpheres, s_EmissiveSphereCount);
         if (rc) die("tpt_set_scene", rc);
     }

@@ -313,7 +313,7 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
     ctx->scene.blob = ctx->dBlobs[ctx->curBlob];
     ctx->scene.layout = L;
     ctx->scene.count = count;
-    ctx->scene.nLights = nLights;
+    ctx->scene.nLights = sampled_lights(L.flags, nLights);   // 0 with light sampling off: every light loop is empty
     // small scenes: stage everything (spheres + materials); large ones: geometry only, materials from L2
     ctx->scene.stagedBytes = L.totalBytes <= 64 * 1024 ? L.totalBytes : L.geomBytes;
     // Expanded-form sweep gate (FastHitterK, tpt_fast.cu). With u = 2^-24 the expanded form evaluates
@@ -361,6 +361,7 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     if (!strcmp(key, "fast_alpha_zero")) { ctx->fastAlphaZero = value ? 1 : 0; return 0; }
     if (!strcmp(key, "scene_upload_always")) { ctx->sceneUploadAlways = value ? 1 : 0; return 0; }
     if (!strcmp(key, "mitsuba_compare")) { ctx->sceneFlags = value ? (ctx->sceneFlags | kSceneMitsuba) : (ctx->sceneFlags & ~(uint32_t)kSceneMitsuba); return 0; }
+    if (!strcmp(key, "light_sampling")) { ctx->sceneFlags = value ? (ctx->sceneFlags & ~(uint32_t)kSceneNoLightSampling) : (ctx->sceneFlags | kSceneNoLightSampling); return 0; }
     if (!strcmp(key, "host_progress")) { ctx->hostProgress = value ? 1 : 0; return 0; }
     if (!strcmp(key, "host_zero_copy")) { ctx->hostZeroCopy = value ? 1 : 0; return 0; }
     if (!strcmp(key, "progress_bands")) { if (value < 1 || value > 16) return fail_msg(ctx, "progress_bands: 1..16"); ctx->progressBands = value; return 0; }

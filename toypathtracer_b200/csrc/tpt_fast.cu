@@ -335,7 +335,7 @@ k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlo
                     st.d = st.nextDir;
                     st.thr = st.thrAlb;
                     st.kind = 0;
-                    st.doMaterialE = false;
+                    st.doMaterialE = emission_after_lambert(sc);
                     ++st.depth;
                 }
             }
@@ -729,9 +729,16 @@ __device__ __forceinline__ void build_sph_pairs(const SceneView& sc, const float
     }
 }
 
+// Light-sampling mode of path_step, fixed at compile time per kernel instance:
+//   kLsOn       explicit light sampling (DO_LIGHT_SAMPLING 1); the scene flag is not looked at
+//   kLsOff      DO_LIGHT_SAMPLING 0: a Lambert vertex bounces at once and adds its emission; no shadow rays, so the
+//               light-sampling block and the QPath fields it keeps (nextDir, thrAlb, nl, pend, albedo) are dead code
+//   kLsRuntime  either, from the scene flag (warp-uniform): the kernels that have no kLsOff twin
+enum { kLsOn = 0, kLsOff = 1, kLsRuntime = 2 };
+
 // One iteration of the per-lane path state machine shared by the queue kernels: intersect the lane's current ray
 // (path or shadow) against all spheres, then shade. Returns true when the lane's path has ended (st.col is final).
-template <class Hitter>
+template <int LS, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
@@ -745,7 +752,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
     bool finished = false;
     if (st.active)
     {
-        if (st.kind == 0)
+        if (LS == kLsOff || st.kind == 0)
         {
             if (id < 0) { st.col = st.col + st.thr * sky(st.d, sc); finished = true; }
             else
@@ -759,6 +766,14 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 // long-latency steps in front of every shading branch); keeping the second test opaque keeps it two branches
                 int mtype = mat.type;
                 if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
+                else if (LS == kLsOff && mtype == kLambert)
+                {
+                    // Test.cpp:86-92 without the light loop; the emission is always added (Test.cpp:209-215 compiled out)
+                    st.col = st.col + st.thr * mat.emissive;
+                    V3 target = normal + RandomUnitVector<false>(st.rng);
+                    st.thr = st.thr * mat.albedo;
+                    st.o = pos; st.d = M<false>::normalize(target); ++st.depth;
+                }
                 else if (mtype == kLambert)
                 {
                     if (st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
@@ -780,7 +795,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     V3 outDir = M<false>::normalize(refl);
                     if (dot(outDir, normal) > 0.0f)
                     {
-                        if (st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
+                        if (LS == kLsOff || st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
                         st.doMaterialE = true;
                         st.thr = st.thr * mat.albedo;
                         st.o = pos; st.d = outDir; ++st.depth;
@@ -794,7 +809,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     if (!ok) { st.col = st.col + st.thr * mat.emissive; finished = true; }
                     else
                     {
-                        if (st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
+                        if (LS == kLsOff || st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
                         st.doMaterialE = true;
                         st.thr = st.thr * att;
                         st.o = pos; st.d = outDir; ++st.depth;
@@ -809,7 +824,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             wantLight = true; lightFrom = j + 1;
         }
     }
-    if (wantLight)
+    if (LS != kLsOff && wantLight)
     {
         int j = lightFrom;
         while (j < sc.nLights && sc.lights[j].id == st.mid) ++j;
@@ -848,7 +863,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             st.d = st.nextDir;
             st.thr = st.thrAlb;
             st.kind = 0;
-            st.doMaterialE = false;
+            st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
             ++st.depth;
         }
     }
@@ -870,11 +885,12 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // conservative + reference-form pass 2 (FastHitterK2C: any scene). THREADS: 128 (6 CTAs/SM) for scenes whose staged
 // geometry is small; one big CTA per SM when the sphere arrays fill most of an SM's shared memory.
 // Dynamic shared memory: [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
-template <int THREADS, int MINB, int KFORM>
-__global__ void __launch_bounds__(THREADS, MINB)
-k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
-             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-             uint32_t raysOffset)
+// The body is shared by k_fast_queue (light sampling) and k_fast_queue_nolight (DO_LIGHT_SAMPLING 0) below.
+template <int THREADS, int KFORM, int LS>
+__device__ __forceinline__ void
+fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+                uint32_t raysOffset)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
@@ -988,7 +1004,7 @@ k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
         if (exhausted) { if (!trDry) trDry = gtimer(); ++trDryTrips; trDryLanes += (unsigned)__popc(__ballot_sync(0xffffffffu, st.active)); }
 #endif
 
-        const bool finished = KFORM == 3 ? path_step(sc, st, rc, hitK2C) : KFORM == 2 ? path_step(sc, st, rc, hitK2) : (KFORM == 1 ? path_step(sc, st, rc, hitK) : path_step(sc, st, rc, hitS));
+        const bool finished = KFORM == 3 ? path_step<LS>(sc, st, rc, hitK2C) : KFORM == 2 ? path_step<LS>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<LS>(sc, st, rc, hitK) : path_step<LS>(sc, st, rc, hitS));
         if (finished)
         {
             red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x * st.weight, st.col.y * st.weight, st.col.z * st.weight);
@@ -1015,6 +1031,26 @@ k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
         t[0] = trEntry; t[1] = trReady; t[2] = trDry; t[3] = gtimer(); t[4] = trTrips; t[5] = trDryTrips; t[6] = trDryLanes; t[7] = smid;
     }
 #endif
+}
+
+template <int THREADS, int MINB, int KFORM>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+             uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOn>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+}
+
+// DO_LIGHT_SAMPLING 0 (scene flag kSceneNoLightSampling): the same kernel without the light-sampling half of the state
+// machine. Same launch shapes and instances as k_fast_queue (launch_queue_t picks one or the other).
+template <int THREADS, int MINB, int KFORM>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+                     uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOff>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
 }
 
 // ---- variant 8 ------------------------------------------------------------------------------------------------
@@ -1051,10 +1087,11 @@ __device__ __forceinline__ void generate_group_rays(const DrawParams& p, float4 
     }
 }
 
-template <int MINB, int KFORM, bool ALLS>
-__global__ void __launch_bounds__(kQueueThreads, MINB)
-k_fast_group(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
-             uint32_t stagedBytes, uint32_t numGroups, uint32_t S, float wPrev)
+// The body is shared by k_fast_group (light sampling) and k_fast_group_nolight (DO_LIGHT_SAMPLING 0) below.
+template <int KFORM, bool ALLS, int LS>
+__device__ __forceinline__ void
+fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                uint32_t stagedBytes, uint32_t numGroups, uint32_t S, float wPrev)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
@@ -1138,7 +1175,7 @@ k_fast_group(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
         }
         if (!__any_sync(0xffffffffu, st.active)) break;
 
-        const bool finished = KFORM == 2 ? path_step(sc, st, rc, hitK2) : (KFORM == 1 ? path_step(sc, st, rc, hitK) : path_step(sc, st, rc, hitS));
+        const bool finished = KFORM == 2 ? path_step<LS>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<LS>(sc, st, rc, hitK) : path_step<LS>(sc, st, rc, hitS));
         bool lastOfGroup = false;
         if (finished)
         {
@@ -1175,7 +1212,24 @@ k_fast_group(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
     if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
 }
 
-// ---- variant 5 ------------------------------------------------------------------------------------------------
+template <int MINB, int KFORM, bool ALLS>
+__global__ void __launch_bounds__(kQueueThreads, MINB)
+k_fast_group(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+             uint32_t stagedBytes, uint32_t numGroups, uint32_t S, float wPrev)
+{
+    fast_group_body<KFORM, ALLS, kLsOn>(p, blob, L, count, nLights, stagedBytes, numGroups, S, wPrev);
+}
+
+// DO_LIGHT_SAMPLING 0 twin of k_fast_group (see k_fast_queue_nolight).
+template <int MINB, int KFORM, bool ALLS>
+__global__ void __launch_bounds__(kQueueThreads, MINB)
+k_fast_group_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                     uint32_t stagedBytes, uint32_t numGroups, uint32_t S, float wPrev)
+{
+    fast_group_body<KFORM, ALLS, kLsOff>(p, blob, L, count, nLights, stagedBytes, numGroups, S, wPrev);
+}
+
+// ---- variant 5------------------------------------------------------------------------------------------------
 // "tile queue": the warp-level slab dealing and path state machine of variant 3, but a CTA owns a tile of kTileQPix
 // pixels for ALL its samples: radiance is accumulated in shared memory and the finished tile is written ONCE with
 // coalesced 128-bit stores (st.global.L1::no_allocate.v4, + 128-bit loads of `prev` when it has weight). The store
@@ -1277,7 +1331,7 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
                 need = __ballot_sync(0xffffffffu, !st.active);
             }
             if (!__any_sync(0xffffffffu, st.active)) break;
-            if (KFORM == 2 ? path_step(sc, st, rc, hitK2) : (KFORM == 1 ? path_step(sc, st, rc, hitK) : path_step(sc, st, rc, hitS)))
+            if (KFORM == 2 ? path_step<kLsRuntime>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<kLsRuntime>(sc, st, rc, hitK) : path_step<kLsRuntime>(sc, st, rc, hitS)))
             {
                 atomicAdd(&sAcc[st.pixOff * 3 + 0], st.col.x * st.weight);
                 atomicAdd(&sAcc[st.pixOff * 3 + 1], st.col.y * st.weight);
@@ -1605,7 +1659,8 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                         const float4 fnx = WFLD(WF_NEXT, slot);
                         float4 fthr = WFLD(WF_THR, slot);
                         const int depth = ((m2 >> 8) & 0xff) + 1;
-                        m2 = 0 | (depth << 8) | (0 << 16);       // doMaterialE = false after a Lambert vertex (Test.cpp:214)
+                        // doMaterialE = false after a Lambert vertex (Test.cpp:214), unless light sampling is off
+                        m2 = 0 | (depth << 8) | ((emission_after_lambert(sc) ? 1 : 0) << 16);
                         WFLD(WF_D, slot) = make_float4(fnx.x, fnx.y, fnx.z, __int_as_float(m2));
                         WFLD(WF_THR, slot) = make_float4(fta.x, fta.y, fta.z, fthr.w);
                     }
@@ -1654,7 +1709,7 @@ template <int THREADS, int MINB, int KFORM>
 static cudaError_t launch_queue_t(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream,
                                   unsigned int* bandDone, int numBands, unsigned int* bandExpected)
 {
-    auto kern = k_fast_queue<THREADS, MINB, KFORM>;
+    auto kern = (sc.layout.flags & kSceneNoLightSampling) ? k_fast_queue_nolight<THREADS, MINB, KFORM> : k_fast_queue<THREADS, MINB, KFORM>;
     const int simd = (sc.count + 3) / 4 * 4;
     const size_t stagedAl = ((size_t)sc.stagedBytes + 127u) & ~(size_t)127u;
     const size_t raysOffset = stagedAl + (KFORM >= 2 ? (((size_t)simd * 16 + 127u) & ~(size_t)127u) : 0);
@@ -1842,6 +1897,9 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         const bool alls = sc.stagedBytes == sc.layout.totalBytes;
         auto kern = alls ? (kform == 2 ? k_fast_group<TPT_QUEUE_MINB, 2, true> : kform == 1 ? k_fast_group<TPT_QUEUE_MINB, 1, true> : k_fast_group<TPT_QUEUE_MINB, 0, true>)
                          : (kform == 2 ? k_fast_group<TPT_QUEUE_MINB, 2, false> : kform == 1 ? k_fast_group<TPT_QUEUE_MINB, 1, false> : k_fast_group<TPT_QUEUE_MINB, 0, false>);
+        if (sc.layout.flags & kSceneNoLightSampling)
+            kern = alls ? (kform == 2 ? k_fast_group_nolight<TPT_QUEUE_MINB, 2, true> : kform == 1 ? k_fast_group_nolight<TPT_QUEUE_MINB, 1, true> : k_fast_group_nolight<TPT_QUEUE_MINB, 0, true>)
+                        : (kform == 2 ? k_fast_group_nolight<TPT_QUEUE_MINB, 2, false> : kform == 1 ? k_fast_group_nolight<TPT_QUEUE_MINB, 1, false> : k_fast_group_nolight<TPT_QUEUE_MINB, 0, false>);
         const size_t dyn8 = kform == 2 ? ((sc.stagedBytes + 127u) & ~127u) + (size_t)simd * 16 : sc.stagedBytes;
         e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn8);
         if (e != cudaSuccess) return e;

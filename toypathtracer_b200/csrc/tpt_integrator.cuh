@@ -492,6 +492,11 @@ TPT_HD V3 sky(V3 dir, const SceneView& sc)
     return ((1.0f - t) * v3(1.0f, 1.0f, 1.0f) + t * v3(0.5f, 0.7f, 1.0f)) * 0.3f;
 }
 
+// doMaterialE after a Lambert vertex (Test.cpp:209-215): with light sampling the next hit's emission was already counted
+// by the shadow rays and is suppressed; with DO_LIGHT_SAMPLING 0 that block is compiled out and every hit adds its
+// emission. The light loops need no test of their own: with light sampling off the kernels get nLights = 0.
+TPT_HD bool emission_after_lambert(const SceneView& sc) { return (sc.flags & kSceneNoLightSampling) != 0; }
+
 // Test.cpp:195-234 (+ Scatter's Lambert branch, Test.cpp:86-136) for ONE camera ray, reference order.
 // The recursion `matE + lightE + attenuation * Trace(...)` (Test.cpp:216) is unrolled with an explicit stack and
 // folded back to front so the rounding sequence is the reference's.
@@ -543,7 +548,7 @@ TPT_HD V3 trace_exact(const SceneView& sc, Ray r, uint32_t& state, unsigned& ray
             break;
         }
         if (!doMaterialE) matE = v3(0, 0, 0);   // Test.cpp:210
-        doMaterialE = (mat.type != kLambert);  // Test.cpp:214
+        doMaterialE = (mat.type != kLambert) || emission_after_lambert(sc);  // Test.cpp:214
         e[n] = matE + lightE;
         a[n] = attenuation;
         ++n;
@@ -590,7 +595,7 @@ TPT_HD V3 trace_fast(const SceneView& sc, Ray r, uint32_t& state, unsigned& rayC
                 int hid = hitter.hit(sc, pos, l, TPT_MIN_T, TPT_MAX_T, ts);
                 if (hid == L.id) col = col + thr * contrib;
             }
-            doMaterialE = false;
+            doMaterialE = emission_after_lambert(sc);
         }
         else
         {
@@ -743,7 +748,7 @@ TPT_HD bool xchain_step(const SceneView& sc, const Camera88& cam, XChain& c, int
         {
             V3 matE = c.matE;
             if (!c.doMaterialE) matE = v3(0, 0, 0);             // Test.cpp:210
-            c.doMaterialE = false;                              // Test.cpp:214 (Lambert)
+            c.doMaterialE = emission_after_lambert(sc);         // Test.cpp:214 (Lambert)
             c.e[c.n] = matE + c.lightE;
             c.a[c.n] = c.albedo;
             ++c.n;
@@ -856,7 +861,7 @@ TPT_D bool xshade_event(const SceneView& sc, XShade& sh, int type, int mid, V3 a
             }
             else attenuation = mat.type == kMetal ? mat.albedo : v3(1, 1, 1);   // Test.cpp:149 / :158
             if (!sh.doMaterialE) matE = v3(0, 0, 0);      // Test.cpp:210
-            sh.doMaterialE = (type != XE_LAMBERT);        // Test.cpp:214
+            sh.doMaterialE = (type != XE_LAMBERT) || emission_after_lambert(sc);   // Test.cpp:214
             sh.e[sh.n] = matE + lightE;
             sh.a[sh.n] = attenuation;
             ++sh.n;

@@ -241,7 +241,7 @@ __device__ __forceinline__ bool rg_step(const DrawParams& p, const SceneView& sc
         {
             V3 matE = st.matE;
             if (!st.doMaterialE) matE = v3(0, 0, 0);
-            st.doMaterialE = false;                                               // Lambert
+            st.doMaterialE = emission_after_lambert(sc);                          // Lambert (DO_LIGHT_SAMPLING 0: kept on)
             st.col = st.col + st.atten * (matE + st.lightE);                      // ComputeShader.hlsl:318-319
             st.atten = st.atten * st.albedo;
             st.o = st.pos; st.d = st.nextDir; st.kind = 0;

@@ -95,7 +95,7 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.matRi = (const float*)(base + L.offMatRi);
     v.count = count;
     v.simdCount = (count + 3) / 4 * 4;
-    v.nLights = nLights;
+    v.nLights = sampled_lights(L.flags, nLights);
     v.flags = L.flags;
     v.sphShared = 0;
     return v;

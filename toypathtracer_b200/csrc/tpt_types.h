@@ -62,7 +62,15 @@ struct SceneBlobLayout
 // DO_MITSUBA_COMPARE (Config.h:25) as a runtime switch: constant sky (Test.cpp:226-227) and zero Metal roughness
 // (Test.cpp:143-145; applied when the scene is packed). Its third effect, zero aperture (Test.cpp:312-313), is camera
 // data and therefore the caller's (the Test.h shim's UpdateTest builds the camera).
-enum SceneFlags : uint32_t { kSceneMitsuba = 1u };
+// DO_LIGHT_SAMPLING (Config.h:24) switched OFF at run time: no explicit light sampling at Lambert vertices (no light
+// draws, no shadow rays, Test.cpp:95-133) and the emission of every hit is added (the doMaterialE suppression of
+// Test.cpp:209-215 is compiled out there). The kernels see it as a light count of 0 (sampled_lights()) plus the
+// emission rule (emission_after_lambert()).
+enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u };
+
+// Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
+// keeps the light table either way, so toggling the switch uploads the same bytes.
+inline int sampled_lights(uint32_t sceneFlags, int nLights) { return (sceneFlags & kSceneNoLightSampling) ? 0 : nLights; }
 
 struct DrawParams
 {
