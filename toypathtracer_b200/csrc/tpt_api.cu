@@ -450,10 +450,8 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         // Host-buffer draw whose `prev` has zero weight, into page-locked memory the GPU can address: the trace kernel's
         // coalesced 128-bit pixel stores go straight into the caller's buffer over PCIe while the other pixels are still
         // being traced — no staging image, no device-to-host copy after the kernel.
-        float wPrev = 1.0f;
-        for (int f = 0; f < numFrames; ++f) wPrev *= lerp_fac(frameCount + f, testFlags);
         cudaPointerAttributes attr;
-        if (wPrev == 0.0f && numFrames <= 256 && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
+        if (prev_weight(frameCount, numFrames, testFlags) == 0.0f && numFrames <= 256 && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
             attr.type == cudaMemoryTypeHost && attr.devicePointer)
         {
             dImage = (float*)attr.devicePointer;
@@ -472,14 +470,8 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         // untouched alpha are part of bit parity). Fast mode uploads it only when prev has a non-zero weight;
         // otherwise the kernel writes alpha = 0, which is what every reference shell's zero-initialised buffer
         // holds (TestWin.cpp:73-74, Renderer.mm:148-149, Emscripten/main.cpp:50-51).
-        needPrev = mode == TPT_MODE_EXACT;
-        if (!needPrev)
-        {
-            // (REFGPU writes alpha = 1 and lerp(col, prev, 0) does not read prev: same rule as the fast mode)
-            float wPrev = 1.0f;
-            for (int f = 0; f < numFrames; ++f) wPrev *= lerp_fac(frameCount + f, testFlags);
-            needPrev = wPrev != 0.0f;
-        }
+        // (REFGPU writes alpha = 1 and lerp(col, prev, 0) does not read prev: same rule as the fast mode)
+        needPrev = mode == TPT_MODE_EXACT || prev_weight(frameCount, numFrames, testFlags) != 0.0f;
         if (needPrev)
         {
             cudaError_t e = copy_rows(dImage, backbuffer, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream);

@@ -104,6 +104,13 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     return v;
 }
 
+// Adds the warp's ray counts to *counter with one atomic per warp; all 32 lanes must call it.
+__device__ __forceinline__ void flush_ray_count(unsigned long long* counter, unsigned rc, int lane)
+{
+    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
+    if (lane == 0 && rc) atomicAdd(counter, (unsigned long long)rc);
+}
+
 __device__ __forceinline__ float4 ld_stream_f4(const float* p)
 {
     float4 r;

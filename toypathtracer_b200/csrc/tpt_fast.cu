@@ -11,8 +11,10 @@
 //            path ends (ray regeneration), so the ray-vs-all-spheres sweep — 85 % of the instructions — always
 //            runs with full warps. Radiance is accumulated per pixel in shared memory; finished tiles are
 //            written with coalesced 128-bit stores (and 128-bit loads of `prev` when accumulating).
+#include <climits>
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
 #include <vector>
 #include "tpt_integrator.cuh"
 #include "tpt_device_utils.cuh"
@@ -149,9 +151,7 @@ k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
         st_stream_f4(px, blend_prev(p, px, sWPrev, acc.x, acc.y, acc.z));
     }
-    // one atomic per warp
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 // ---- variant 1 ------------------------------------------------------------------------------------------------
@@ -361,8 +361,7 @@ k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlo
             sAcc[i * 3 + 0] = 0.0f; sAcc[i * 3 + 1] = 0.0f; sAcc[i * 3 + 2] = 0.0f;
         }
     }
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 
@@ -729,6 +728,66 @@ __device__ __forceinline__ void build_sph_pairs(const SceneView& sc, const float
     }
 }
 
+// Dynamic shared memory of the fast kernels: [staged blob | pad to 128 B | pair array (KFORM 2/3) | per-warp buffers].
+// A launch with nothing behind the blob requests the blob itself, unpadded. roundPairs pads the pair array to 128 B
+// before the buffers: the slab queue does, variants 5 and 8 (no buffers) and the fit rules of fast_queue_kform and the
+// queue's CTA size do not. The difference is deliberate and kept: it sets how much shared memory those launches
+// request, and with it their occupancy and grid.
+struct FastSmem
+{
+    uint32_t pairs;     // offset of the pair array
+    uint32_t buffers;   // offset of the per-warp buffers (queue: camera rays; wavefront: the path pool)
+    uint32_t bytes;     // dynamic shared memory of the launch
+};
+__host__ __device__ inline FastSmem fast_smem(uint32_t stagedBytes, uint32_t pairBytes = 0, uint32_t bufferBytes = 0,
+                                              bool roundPairs = false)
+{
+    FastSmem s;
+    s.pairs = (stagedBytes + 127u) & ~127u;
+    s.buffers = s.pairs + (roundPairs ? (pairBytes + 127u) & ~127u : pairBytes);
+    s.bytes = pairBytes + bufferBytes != 0 ? s.buffers + bufferBytes : stagedBytes;
+    return s;
+}
+
+// Sweep setup of the kernels that pick a sweep form KFORM, run after stage_blob/make_view; returns that form's hitter.
+//   0  reference form on the staged {s, r^2} array (SerialHitter)
+//   1  expanded form: {s, r^2} rewritten to {s, K} in place (FastHitterK)
+//   2  expanded form on the pair array, built from {s, K} (FastHitterK2)
+//   3  conservative pair array built from {s, r^2}, which stays for the reference-form pass 2 (FastHitterK2C)
+// The sweep's loads are plain (schedulable) asm: their addresses are made opaque AFTER the barrier so that none of them
+// can be hoisted above the rewrite of the sphere array or the construction of the pair array.
+template <int KFORM>
+__device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char* smem, const SceneBlobLayout& L, uint32_t stagedBytes)
+{
+    float4* sph = reinterpret_cast<float4*>(smem + L.offSph);
+    float4* pairs = reinterpret_cast<float4*>(smem + fast_smem(stagedBytes).pairs);
+    if constexpr (KFORM == 1 || KFORM == 2) build_sphK(sc, sph);
+    __syncthreads();
+    if constexpr (KFORM == 0) return SerialHitter<false>();
+    else if constexpr (KFORM == 1)
+    {
+        FastHitterK h; h.sphK = sc.sphShared; h.simdCount = sc.simdCount;
+        asm volatile("" : "+r"(h.sphK));
+        return h;
+    }
+    else if constexpr (KFORM == 2)
+    {
+        build_sph_pairs(sc, sph, pairs);
+        __syncthreads();
+        FastHitterK2 h; h.sphK = sc.sphShared; h.sphP = smem_u32(pairs); h.simdCount = sc.simdCount;
+        asm volatile("" : "+r"(h.sphK), "+r"(h.sphP));
+        return h;
+    }
+    else
+    {
+        build_sph_pairs_from_r2(sc, sph, pairs);
+        __syncthreads();
+        FastHitterK2C h; h.sph = sc.sphShared; h.sphP = smem_u32(pairs); h.simdCount = sc.simdCount;
+        asm volatile("" : "+r"(h.sph), "+r"(h.sphP));
+        return h;
+    }
+}
+
 // Light-sampling mode of path_step, fixed at compile time per kernel instance:
 //   kLsOn       explicit light sampling (DO_LIGHT_SAMPLING 1); the scene flag is not looked at
 //   kLsOff      DO_LIGHT_SAMPLING 0: a Lambert vertex bounces at once and adds its emission; no shadow rays, so the
@@ -881,10 +940,9 @@ __device__ unsigned long long* g_warpTrace = nullptr;
 __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t)); return t; }
 #endif
 
-// KFORM 0: reference-form sweep, 1: expanded form, 2: expanded form on the pair array, 3: pair-array pass 1 made
-// conservative + reference-form pass 2 (FastHitterK2C: any scene). THREADS: 128 (6 CTAs/SM) for scenes whose staged
-// geometry is small; one big CTA per SM when the sphere arrays fill most of an SM's shared memory.
-// Dynamic shared memory: [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
+// KFORM: the sweep form (prepare_sweep). THREADS: 128 (6 CTAs/SM) for scenes whose staged geometry is small; one big CTA
+// per SM when the sphere arrays fill most of an SM's shared memory.
+// Dynamic shared memory (FastSmem): [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
 // The body is shared by k_fast_queue (light sampling) and k_fast_queue_nolight (DO_LIGHT_SAMPLING 0) below.
 template <int THREADS, int KFORM, int LS>
 __device__ __forceinline__ void
@@ -908,19 +966,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     // the 128-thread instances are only launched for scenes whose whole blob is staged (launch_fast): their view points into
     // shared memory for every section, so materials, lights and 1/r load with LDS instead of generic LD
     SceneView sc = make_view<THREADS == 128>(smem, blob, L, stagedBytes, count, nLights);
-    float4* sphK = reinterpret_cast<float4*>(smem + L.offSph);
-    if (KFORM == 1 || KFORM == 2) build_sphK(sc, sphK);
-    __syncthreads();
-    float4* pairs = reinterpret_cast<float4*>(smem + ((stagedBytes + 127u) & ~127u));     // KFORM 2/3: behind the staged blob
-    if (KFORM == 2) { build_sph_pairs(sc, sphK, pairs); __syncthreads(); }
-    if (KFORM == 3) { build_sph_pairs_from_r2(sc, sphK, pairs); __syncthreads(); }
-    FastHitterK hitK; hitK.sphK = sc.sphShared; hitK.simdCount = sc.simdCount;
-    FastHitterK2 hitK2; hitK2.sphK = sc.sphShared; hitK2.sphP = smem_u32(pairs); hitK2.simdCount = sc.simdCount;
-    FastHitterK2C hitK2C; hitK2C.sph = sc.sphShared; hitK2C.sphP = smem_u32(pairs); hitK2C.simdCount = sc.simdCount;
-    // the sweep's loads are plain (schedulable) asm: make their address opaque AFTER the barrier so that none of them can
-    // be hoisted above the in-place {s, r^2} -> {s, K} rewrite / the construction of the pair array
-    asm volatile("" : "+r"(hitK.sphK), "+r"(hitK2.sphK), "+r"(hitK2.sphP), "+r"(hitK2C.sph), "+r"(hitK2C.sphP));
-    SerialHitter<false> hitS;
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
     const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
@@ -1004,8 +1050,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if (exhausted) { if (!trDry) trDry = gtimer(); ++trDryTrips; trDryLanes += (unsigned)__popc(__ballot_sync(0xffffffffu, st.active)); }
 #endif
 
-        const bool finished = KFORM == 3 ? path_step<LS>(sc, st, rc, hitK2C) : KFORM == 2 ? path_step<LS>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<LS>(sc, st, rc, hitK) : path_step<LS>(sc, st, rc, hitS));
-        if (finished)
+        if (path_step<LS>(sc, st, rc, hitter))
         {
             red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x * st.weight, st.col.y * st.weight, st.col.z * st.weight);
             st.active = false;
@@ -1021,8 +1066,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         }
     }
     if (bandDone && doneCnt) { __threadfence(); atomicAdd(bandDone + curBand, doneCnt); }
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 #if TPT_TRACE_WARPS
     if (lane == 0 && g_warpTrace)
     {
@@ -1105,15 +1149,7 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     for (int i = threadIdx.x; i < (kQueueThreads / 32) * kGroupOpen * kGroupPix; i += kQueueThreads) (&sAcc[0][0][0])[i] = make_float4(0, 0, 0, 0);
     if (threadIdx.x < (kQueueThreads / 32) * kGroupOpen) (&sRemain[0][0])[threadIdx.x] = 0;
     SceneView sc = make_view<ALLS>(smem, blob, L, stagedBytes, count, nLights);     // ALLS: whole blob staged -> LDS for every section
-    float4* sphK = reinterpret_cast<float4*>(smem + L.offSph);
-    if (KFORM) build_sphK(sc, sphK);
-    __syncthreads();
-    float4* pairs = reinterpret_cast<float4*>(smem + ((stagedBytes + 127u) & ~127u));
-    if (KFORM == 2) { build_sph_pairs(sc, sphK, pairs); __syncthreads(); }
-    FastHitterK hitK; hitK.sphK = sc.sphShared; hitK.simdCount = sc.simdCount;
-    FastHitterK2 hitK2; hitK2.sphK = sc.sphShared; hitK2.sphP = smem_u32(pairs); hitK2.simdCount = sc.simdCount;
-    asm volatile("" : "+r"(hitK.sphK), "+r"(hitK2.sphK), "+r"(hitK2.sphP));     // see k_fast_queue
-    SerialHitter<false> hitS;
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
@@ -1175,9 +1211,8 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         }
         if (!__any_sync(0xffffffffu, st.active)) break;
 
-        const bool finished = KFORM == 2 ? path_step<LS>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<LS>(sc, st, rc, hitK) : path_step<LS>(sc, st, rc, hitS));
         bool lastOfGroup = false;
-        if (finished)
+        if (path_step<LS>(sc, st, rc, hitter))
         {
             float* a = reinterpret_cast<float*>(&sAcc[warp][st.pixOff >> 4][st.pixOff & 15u]);
             atomicAdd(a + 0, st.col.x * st.weight);
@@ -1208,8 +1243,7 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             __syncwarp();
         }
     }
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 template <int MINB, int KFORM, bool ALLS>
@@ -1253,15 +1287,7 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
     if (threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); }
     for (int i = threadIdx.x; i < kTileQPix * 3; i += kQueueThreads) sAcc[i] = 0.0f;
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    float4* sphK = reinterpret_cast<float4*>(smem + L.offSph);
-    if (KFORM) build_sphK(sc, sphK);
-    __syncthreads();
-    float4* pairs = reinterpret_cast<float4*>(smem + ((stagedBytes + 127u) & ~127u));
-    if (KFORM == 2) { build_sph_pairs(sc, sphK, pairs); __syncthreads(); }
-    FastHitterK hitK; hitK.sphK = sc.sphShared; hitK.simdCount = sc.simdCount;
-    FastHitterK2 hitK2; hitK2.sphK = sc.sphShared; hitK2.sphP = smem_u32(pairs); hitK2.simdCount = sc.simdCount;
-    asm volatile("" : "+r"(hitK.sphK), "+r"(hitK2.sphK), "+r"(hitK2.sphP));     // see k_fast_queue
-    SerialHitter<false> hitS;
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
     const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
@@ -1331,7 +1357,7 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
                 need = __ballot_sync(0xffffffffu, !st.active);
             }
             if (!__any_sync(0xffffffffu, st.active)) break;
-            if (KFORM == 2 ? path_step<kLsRuntime>(sc, st, rc, hitK2) : (KFORM == 1 ? path_step<kLsRuntime>(sc, st, rc, hitK) : path_step<kLsRuntime>(sc, st, rc, hitS)))
+            if (path_step<kLsRuntime>(sc, st, rc, hitter))
             {
                 atomicAdd(&sAcc[st.pixOff * 3 + 0], st.col.x * st.weight);
                 atomicAdd(&sAcc[st.pixOff * 3 + 1], st.col.y * st.weight);
@@ -1352,8 +1378,7 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
             sAcc[i * 3 + 0] = 0.0f; sAcc[i * 3 + 1] = 0.0f; sAcc[i * 3 + 2] = 0.0f;
         }
     }
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 // ---- variant 6 ------------------------------------------------------------------------------------------------
@@ -1670,69 +1695,100 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         __syncthreads();
     }
 #undef WFLD
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 } // namespace tpt
 #include "tpt_refgpu.cuh"
 namespace tpt {
 
+// ---- sweep form (KFORM, see prepare_sweep) per kernel family -------------------------------------------------------
+// Inputs: sc.kformMode, the fast_kform option (0 reference form, 1 expanded form, 2 pair array where it fits), and
+// sc.kformOk, the scene passes the expanded form's accuracy gate (tpt_set_scene; never with fast_kform 0).
+// The families differ on purpose:
+//   slab queue (variants 3/4/9, and tpt_draw's automatic variant): the pair array where the blob, the pairs and 24
+//     camera-ray buffers fit in 200 KB, else form 1. A scene that fails the gate runs the conservative form 3 when
+//     fast_kform is 2 and the pairs fit, else form 0.
+//   group and tile queue (variants 8 and 5): the pair array up to 1024 spheres, else form 1. No form 3: a scene that
+//     fails the gate runs form 0.
+//   reference-GPU native instance: form 2 under the group rule but only when fast_kform is 2, else its own
+//     reference-form setup (RgSetupPlain); never form 1 or 3.
+static uint32_t simd_count(const SceneDev& sc) { return (uint32_t)((sc.count + 3) / 4 * 4); }
+
+int fast_queue_kform(const SceneDev& sc)
+{
+    const bool pairsFit = fast_smem(sc.stagedBytes, simd_count(sc) * 16, 24 * 2048).bytes <= 200 * 1024;
+    if (sc.kformMode == 0) return 0;
+    if (sc.kformOk) return (sc.kformMode == 1 || !pairsFit) ? 1 : 2;
+    return (sc.kformMode == 2 && pairsFit) ? 3 : 0;
+}
+static int fast_group_kform(const SceneDev& sc)
+{
+    return !sc.kformOk ? 0 : (sc.kformMode == 1 || simd_count(sc) > 1024 ? 1 : 2);
+}
+static int refgpu_fast_kform(const SceneDev& sc)
+{
+    return sc.kformOk && sc.kformMode == 2 && simd_count(sc) <= 1024 ? 2 : 0;
+}
+
+// Runtime sweep form -> kernel instance: f(std::integral_constant<int, kform>) for kform in [1, KMAX], f(<0>) otherwise.
+template <int KMAX, class F>
+static auto for_kform(int kform, F f)
+{
+    if constexpr (KMAX == 0) return f(std::integral_constant<int, 0>());
+    else return kform == KMAX ? f(std::integral_constant<int, KMAX>()) : for_kform<KMAX - 1>(kform, f);
+}
+// the light-sampling instance, or its DO_LIGHT_SAMPLING 0 twin where the scene turns light sampling off
+template <class Kernel>
+static Kernel light_twin(const SceneDev& sc, Kernel on, Kernel off) { return (sc.layout.flags & kSceneNoLightSampling) ? off : on; }
+
 // The reference-GPU-compatible mode's native instance sweeps like the fast mode: expanded form on the pair array.
 struct RgSetupK2
 {
     using Hitter = FastHitterK2;
     static constexpr int kMinBlocks = 6;
-    static size_t extra_smem(const SceneDev& sc) { return (((size_t)sc.stagedBytes + 127u) & ~(size_t)127u) - sc.stagedBytes + (size_t)((sc.count + 3) / 4 * 4) * 16; }
+    static size_t dyn_smem(const SceneDev& sc) { return fast_smem(sc.stagedBytes, simd_count(sc) * 16).bytes; }
     static __device__ __forceinline__ Hitter prepare(SceneView& sc, unsigned char* smem, const SceneBlobLayout& L, uint32_t stagedBytes)
     {
-        float4* sphK = reinterpret_cast<float4*>(smem + L.offSph);
-        build_sphK(sc, sphK);                       // padded spheres get K = 1e30: never candidates (ComputeShader.hlsl:134)
-        __syncthreads();
-        float4* pairs = reinterpret_cast<float4*>(smem + ((stagedBytes + 127u) & ~127u));
-        build_sph_pairs(sc, sphK, pairs);
-        __syncthreads();
-        Hitter h; h.sphK = sc.sphShared; h.sphP = smem_u32(pairs); h.simdCount = sc.simdCount;
-        asm volatile("" : "+r"(h.sphK), "+r"(h.sphP));
-        return h;
+        return prepare_sweep<2>(sc, smem, L, stagedBytes);   // padded spheres get K = 1e30: never candidates (ComputeShader.hlsl:134)
     }
 };
 
 cudaError_t launch_refgpu_fast(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
 {
-    const int simd = (sc.count + 3) / 4 * 4;
-    if (sc.kformOk && sc.kformMode == 2 && simd <= 1024) return launch_refgpu_t<false, RgSetupK2>(p, sc, numSMs, stream);
+    if (refgpu_fast_kform(sc) == 2) return launch_refgpu_t<false, RgSetupK2>(p, sc, numSMs, stream);
     return launch_refgpu_t<false>(p, sc, numSMs, stream);
 }
 
-template <int THREADS, int MINB, int KFORM>
-static cudaError_t launch_queue_t(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream,
-                                  unsigned int* bandDone, int numBands, unsigned int* bandExpected)
+float prev_weight(int frame0, int numFrames, unsigned flags)
 {
-    auto kern = (sc.layout.flags & kSceneNoLightSampling) ? k_fast_queue_nolight<THREADS, MINB, KFORM> : k_fast_queue<THREADS, MINB, KFORM>;
-    const int simd = (sc.count + 3) / 4 * 4;
-    const size_t stagedAl = ((size_t)sc.stagedBytes + 127u) & ~(size_t)127u;
-    const size_t raysOffset = stagedAl + (KFORM >= 2 ? (((size_t)simd * 16 + 127u) & ~(size_t)127u) : 0);
-    const size_t dyn3 = raysOffset + (size_t)(THREADS / 32) * kSlabPix * 32;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn3);
-    if (e != cudaSuccess) return e;
-    int perSM = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, THREADS, dyn3);
-    if (e != cudaSuccess) return e;
-    if (perSM < 1) perSM = 1;
-    float wPrev = 1.0f;
-    for (int f = 0; f < p.numFrames; ++f) wPrev *= lerp_fac(p.frame0 + f, p.flags);
+    float w = 1.0f;
+    for (int f = 0; f < numFrames; ++f) w *= lerp_fac(frame0 + f, flags);
+    return w;
+}
+
+using QueueKernel = decltype(&k_fast_queue<128, TPT_QUEUE_MINB, 0>);
+template <int THREADS, int MINB>
+static QueueKernel queue_kernel(const SceneDev& sc, int kform)
+{
+    return for_kform<3>(kform, [&](auto K) {
+        return light_twin(sc, k_fast_queue<THREADS, MINB, decltype(K)::value>, k_fast_queue_nolight<THREADS, MINB, decltype(K)::value>);
+    });
+}
+
+static cudaError_t launch_queue(QueueKernel kern, int threads, int kform, const DrawParams& p, const SceneDev& sc, int numSMs,
+                                cudaStream_t stream, unsigned int* bandDone, int numBands, unsigned int* bandExpected)
+{
+    const FastSmem lay = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0, (uint32_t)(threads / 32) * kSlabPix * 32, true);
     const long long regionPix = (long long)p.numRows * p.width;
-    k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, wPrev);
-    e = cudaGetLastError();
-    if (e != cudaSuccess) return e;
     const uint32_t S = (uint32_t)(p.spp * p.numFrames);
     const long long slabs = ((regionPix + kSlabPix - 1) / kSlabPix) * S;
     if (slabs > 0x7fffffffLL) return cudaErrorInvalidValue;
-    long long grid = (long long)numSMs * perSM;
-    const long long ctasNeeded = (slabs + THREADS / 32 - 1) / (THREADS / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded;
-    e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+    long long grid = 0;
+    cudaError_t e = persistent_grid(kern, threads, lay.bytes, numSMs, (slabs + threads / 32 - 1) / (threads / 32), p, stream, grid);
+    if (e != cudaSuccess) return e;
+    k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
+    e = cudaGetLastError();
     if (e != cudaSuccess) return e;
     // optional progress bands (host-buffer draws): band b = macro-tiles [b*mpb, (b+1)*mpb)
     const uint32_t mtiles = (uint32_t)((regionPix + kSlabPix - 1) / kSlabPix);
@@ -1749,15 +1805,15 @@ static cudaError_t launch_queue_t(const DrawParams& p, const SceneDev& sc, int n
     }
 #if TPT_TRACE_WARPS
     static unsigned long long* dTrace = nullptr;
-    const size_t traceWords = (size_t)grid * (THREADS / 32) * 8;
+    const size_t traceWords = (size_t)grid * (threads / 32) * 8;
     if (getenv("TPT_TRACE_FILE"))
     {
         if (!dTrace) { cudaMalloc(&dTrace, (size_t)132 * 16 * 32 * 8 * 8); cudaMemcpyToSymbol(g_warpTrace, &dTrace, sizeof(dTrace)); }
         cudaMemsetAsync(dTrace, 0, traceWords * 8, stream);
     }
 #endif
-    kern<<<(unsigned)grid, THREADS, dyn3, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                      (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, (uint32_t)raysOffset);
+    kern<<<(unsigned)grid, threads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                                                          (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers);
 #if TPT_TRACE_WARPS
     if (const char* tf = getenv("TPT_TRACE_FILE"))
     {
@@ -1781,37 +1837,21 @@ k_debug_hit(const unsigned char* __restrict__ blob, SceneBlobLayout L, int count
     __shared__ uint64_t bar;
     stage_blob(smem, blob, stagedBytes, &bar);
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    float4* sphK = reinterpret_cast<float4*>(smem + L.offSph);
-    if (KFORM == 1 || KFORM == 2) build_sphK(sc, sphK);
-    __syncthreads();
-    float4* pairs = reinterpret_cast<float4*>(smem + ((stagedBytes + 127u) & ~127u));
-    if (KFORM == 2) { build_sph_pairs(sc, sphK, pairs); __syncthreads(); }
-    if (KFORM == 3) { build_sph_pairs_from_r2(sc, sphK, pairs); __syncthreads(); }
-    FastHitterK hitK; hitK.sphK = sc.sphShared; hitK.simdCount = sc.simdCount;
-    FastHitterK2 hitK2; hitK2.sphK = sc.sphShared; hitK2.sphP = smem_u32(pairs); hitK2.simdCount = sc.simdCount;
-    FastHitterK2C hitK2C; hitK2C.sph = sc.sphShared; hitK2C.sphP = smem_u32(pairs); hitK2C.simdCount = sc.simdCount;
-    asm volatile("" : "+r"(hitK.sphK), "+r"(hitK2.sphK), "+r"(hitK2.sphP), "+r"(hitK2C.sph), "+r"(hitK2C.sphP));
-    SerialHitter<false> hitS;
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     {
         const V3 o{rays[6 * i], rays[6 * i + 1], rays[6 * i + 2]}, d{rays[6 * i + 3], rays[6 * i + 4], rays[6 * i + 5]};
         float t = TPT_MAX_T;
-        int id;
-        if (KFORM == 3) id = hitK2C.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
-        else if (KFORM == 2) id = hitK2.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
-        else if (KFORM == 1) id = hitK.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
-        else id = hitS.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
-        outId[i] = id;
+        outId[i] = hitter.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
         outT[i] = t;
     }
 }
 
 cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, int* dId, float* dT, long long n, int numSMs, cudaStream_t stream)
 {
-    auto kern = kform == 3 ? k_debug_hit<3> : kform == 2 ? k_debug_hit<2> : kform == 1 ? k_debug_hit<1> : k_debug_hit<0>;
-    const int simd = (sc.count + 3) / 4 * 4;
-    const size_t stagedAl = ((size_t)sc.stagedBytes + 127u) & ~(size_t)127u;
-    const size_t dyn = stagedAl + (kform >= 2 ? (size_t)simd * 16 : 0);
+    auto kern = for_kform<3>(kform, [](auto K) { return k_debug_hit<decltype(K)::value>; });
+    // the blob padded to 128 B even without a pair array: the end of the (possibly empty) pair array
+    const size_t dyn = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0).buffers;
     if (dyn > 200 * 1024) return cudaErrorInvalidValue;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
     if (e != cudaSuccess) return e;
@@ -1819,28 +1859,18 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
     return cudaGetLastError();
 }
 
-// Sweep form the slab-queue kernel (variants 3/4) runs for this scene and option set: see k_fast_queue.
-int fast_queue_kform(const SceneDev& sc)
-{
-    const int simd = (sc.count + 3) / 4 * 4;
-    const size_t pairBytes = (size_t)simd * 16, stagedAl = ((size_t)sc.stagedBytes + 127u) & ~(size_t)127u;
-    const bool pairsFit = stagedAl + pairBytes + 24 * 2048 <= 200 * 1024;
-    if (sc.kformMode == 0) return 0;
-    if (sc.kformOk) return (sc.kformMode == 1 || !pairsFit) ? 1 : 2;
-    return (sc.kformMode == 2 && pairsFit) ? 3 : 0;
-}
-
 int fast_slab_pixels() { return kSlabPix; }
 
 int fast_kernel_launches(const DrawParams&, int variant) { return (variant == 3 || variant == 4 || variant == 9 || variant == 6 || variant == 7) ? 2 : 1; }
 bool fast_variant_writes_final_pixels(int variant) { return variant == 8; }
 
-
-
 cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, int numSMs, cudaStream_t stream,
                         unsigned int* bandDone, int numBands, unsigned int* bandExpected)
 {
     if (p.numFrames > kMaxFramesPerDraw) return cudaErrorInvalidValue;
+    const long long regionPix = (long long)p.numRows * p.width;
+    const uint32_t S = (uint32_t)(p.spp * p.numFrames);
+    long long grid = 0;
     cudaError_t e;
     if (variant == 0)
     {
@@ -1853,135 +1883,85 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
     if (variant == 1 || variant == 2)
     {
         auto kern = variant == 1 ? k_fast_persistent<2> : k_fast_persistent<3>;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
-        if (e != cudaSuccess) return e;
-        int perSM = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, kFastThreads, sc.stagedBytes);
-        if (e != cudaSuccess) return e;
-        if (perSM < 1) perSM = 1;
-        const long long regionPix = (long long)p.numRows * p.width;
         const int numTiles = (int)((regionPix + kTilePix - 1) / kTilePix);
-        int grid = numSMs * perSM;
-        if (grid > numTiles) grid = numTiles;
-        e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+        e = persistent_grid(kern, kFastThreads, sc.stagedBytes, numSMs, numTiles, p, stream, grid);
         if (e != cudaSuccess) return e;
-        kern<<<grid, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, numTiles);
+        kern<<<(unsigned)grid, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, numTiles);
         return cudaGetLastError();
     }
     if (variant == 3 || variant == 4 || variant == 9)
     {
-        // sweep form: 2 = expanded form on the pair array (the pair array costs 16 B per sphere of extra shared memory) where
-        // the scene passes the accuracy gate, 3 = the conservative packed form + reference-form pass 2 where it does not,
-        // 1 / 0 = scalar expanded / reference form (comparison, or scenes too large for the pair array)
-        const int simd = (sc.count + 3) / 4 * 4;
-        const size_t pairBytes = (size_t)simd * 16, stagedAl = ((size_t)sc.stagedBytes + 127u) & ~(size_t)127u;
         const int kform = fast_queue_kform(sc);
-        // small scenes: 128-thread CTAs, 6 (variant 4: 7) per SM; scenes whose arrays fill most of an SM's shared memory: ONE
-        // 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs x 4 warps with a copy each)
-        const bool big = stagedAl + ((kform >= 2) ? pairBytes : 0) + 4 * 2048 > 36 * 1024 || sc.stagedBytes != sc.layout.totalBytes;
-#define TPT_LAUNCH_QUEUE(T, M, K) return launch_queue_t<T, M, K>(p, sc, numSMs, stream, bandDone, numBands, bandExpected)
-        if (big) { switch (kform) { case 3: TPT_LAUNCH_QUEUE(TPT_BIG_THREADS, 1, 3); case 2: TPT_LAUNCH_QUEUE(TPT_BIG_THREADS, 1, 2); case 1: TPT_LAUNCH_QUEUE(TPT_BIG_THREADS, 1, 1); default: TPT_LAUNCH_QUEUE(TPT_BIG_THREADS, 1, 0); } }
+        // small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays fill most of an SM's
+        // shared memory: ONE 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs x 4 warps
+        // with a copy each)
+        const bool big = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0, 4 * 2048).bytes > 36 * 1024 ||
+                         sc.stagedBytes != sc.layout.totalBytes;
         // long draws (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80; short ones keep 6, where a
         // warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant 9 forces the 8-CTA
         // instance (A/B runs).
-        const long long slabsPerWarp = (((long long)p.numRows * p.width + kSlabPix - 1) / kSlabPix) * p.spp * p.numFrames / ((long long)numSMs * 32);
-        if (kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) TPT_LAUNCH_QUEUE(128, 8, 2);
-        if (variant == 3 || variant == 9) { switch (kform) { case 3: TPT_LAUNCH_QUEUE(128, TPT_QUEUE_MINB, 3); case 2: TPT_LAUNCH_QUEUE(128, TPT_QUEUE_MINB, 2); case 1: TPT_LAUNCH_QUEUE(128, TPT_QUEUE_MINB, 1); default: TPT_LAUNCH_QUEUE(128, TPT_QUEUE_MINB, 0); } }
-        switch (kform) { case 3: TPT_LAUNCH_QUEUE(128, 7, 3); case 2: TPT_LAUNCH_QUEUE(128, 7, 2); case 1: TPT_LAUNCH_QUEUE(128, 7, 1); default: TPT_LAUNCH_QUEUE(128, 7, 0); }   // variant 4: 72 registers
-#undef TPT_LAUNCH_QUEUE
+        const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * p.spp * p.numFrames / ((long long)numSMs * 32);
+        QueueKernel kern = variant == 4 ? queue_kernel<128, 7>(sc, kform) : queue_kernel<128, TPT_QUEUE_MINB>(sc, kform);
+        int threads = 128;
+        if (big) { kern = queue_kernel<TPT_BIG_THREADS, 1>(sc, kform); threads = TPT_BIG_THREADS; }
+        else if (kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48)))
+            kern = light_twin(sc, k_fast_queue<128, 8, 2>, k_fast_queue_nolight<128, 8, 2>);
+        return launch_queue(kern, threads, kform, p, sc, numSMs, stream, bandDone, numBands, bandExpected);
     }
     if (variant == 8)
     {
-        const int simd = (sc.count + 3) / 4 * 4;
-        const int kform = !sc.kformOk ? 0 : (sc.kformMode == 1 || simd > 1024 ? 1 : 2);
+        const int kform = fast_group_kform(sc);
         const bool alls = sc.stagedBytes == sc.layout.totalBytes;
-        auto kern = alls ? (kform == 2 ? k_fast_group<TPT_QUEUE_MINB, 2, true> : kform == 1 ? k_fast_group<TPT_QUEUE_MINB, 1, true> : k_fast_group<TPT_QUEUE_MINB, 0, true>)
-                         : (kform == 2 ? k_fast_group<TPT_QUEUE_MINB, 2, false> : kform == 1 ? k_fast_group<TPT_QUEUE_MINB, 1, false> : k_fast_group<TPT_QUEUE_MINB, 0, false>);
-        if (sc.layout.flags & kSceneNoLightSampling)
-            kern = alls ? (kform == 2 ? k_fast_group_nolight<TPT_QUEUE_MINB, 2, true> : kform == 1 ? k_fast_group_nolight<TPT_QUEUE_MINB, 1, true> : k_fast_group_nolight<TPT_QUEUE_MINB, 0, true>)
-                        : (kform == 2 ? k_fast_group_nolight<TPT_QUEUE_MINB, 2, false> : kform == 1 ? k_fast_group_nolight<TPT_QUEUE_MINB, 1, false> : k_fast_group_nolight<TPT_QUEUE_MINB, 0, false>);
-        const size_t dyn8 = kform == 2 ? ((sc.stagedBytes + 127u) & ~127u) + (size_t)simd * 16 : sc.stagedBytes;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn8);
-        if (e != cudaSuccess) return e;
-        int perSM = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, kQueueThreads, dyn8);
-        if (e != cudaSuccess) return e;
-        if (perSM < 1) perSM = 1;
-        float wPrev = 1.0f;
-        for (int f = 0; f < p.numFrames; ++f) wPrev *= lerp_fac(p.frame0 + f, p.flags);
-        const long long regionPix = (long long)p.numRows * p.width;
-        const uint32_t S = (uint32_t)(p.spp * p.numFrames);
+        auto kern = for_kform<2>(kform, [&](auto K) {
+            constexpr int k = decltype(K)::value;
+            return alls ? light_twin(sc, k_fast_group<TPT_QUEUE_MINB, k, true>, k_fast_group_nolight<TPT_QUEUE_MINB, k, true>)
+                        : light_twin(sc, k_fast_group<TPT_QUEUE_MINB, k, false>, k_fast_group_nolight<TPT_QUEUE_MINB, k, false>);
+        });
+        const size_t dyn = fast_smem(sc.stagedBytes, kform == 2 ? simd_count(sc) * 16 : 0).bytes;
         const long long groups = (regionPix + kGroupPix - 1) / kGroupPix;
         if (groups > 0x7fffffffLL) return cudaErrorInvalidValue;
-        long long grid = (long long)numSMs * perSM;
-        const long long ctasNeeded = (groups + kQueueThreads / 32 - 1) / (kQueueThreads / 32);
-        if (grid > ctasNeeded) grid = ctasNeeded;
-        e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+        e = persistent_grid(kern, kQueueThreads, dyn, numSMs, (groups + kQueueThreads / 32 - 1) / (kQueueThreads / 32), p, stream, grid);
         if (e != cudaSuccess) return e;
-        kern<<<(unsigned)grid, kQueueThreads, dyn8, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                                (uint32_t)groups, S, wPrev);
+        kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                                                               (uint32_t)groups, S, prev_weight(p.frame0, p.numFrames, p.flags));
         return cudaGetLastError();
     }
     if (variant == 6 || variant == 7)
     {
         auto kern = variant == 6 ? k_fast_wave<3> : k_fast_wave<4>;
-        const uint32_t poolOffset = (sc.stagedBytes + 127u) & ~127u;
-        const size_t dyn = (size_t)poolOffset + (size_t)kWaveFields * kWaveSlots * 16;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+        const FastSmem lay = fast_smem(sc.stagedBytes, 0, kWaveFields * kWaveSlots * 16);
+        const long long total = ((regionPix + 127) / 128) * 128 * S;      // whole 128-pixel slabs; tail pixels are skipped
+        if (total > 0x7fffffffLL) return cudaErrorInvalidValue;
+        e = persistent_grid(kern, kWaveThreads, lay.bytes, numSMs, (total + kWaveChunk - 1) / kWaveChunk, p, stream, grid);
         if (e != cudaSuccess) return e;
-        int perSM = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, kWaveThreads, dyn);
-        if (e != cudaSuccess) return e;
-        if (perSM < 1) perSM = 1;
-        float wPrev = 1.0f;
-        for (int f = 0; f < p.numFrames; ++f) wPrev *= lerp_fac(p.frame0 + f, p.flags);
-        const long long regionPix = (long long)p.numRows * p.width;
-        k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, wPrev);
+        k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;
         WaveArgs wa;
-        wa.S = (uint32_t)(p.spp * p.numFrames);
-        const long long total = ((regionPix + 127) / 128) * 128 * wa.S;      // whole 128-pixel slabs; tail pixels are skipped
-        if (total > 0x7fffffffLL) return cudaErrorInvalidValue;
+        wa.S = S;
         wa.totalPaths = (uint32_t)total;
         wa.divS = make_fastdiv(wa.S); wa.divW = make_fastdiv((uint32_t)p.width); wa.divSpp = make_fastdiv((uint32_t)p.spp);
-        long long grid = (long long)numSMs * perSM;
-        const long long need = (total + kWaveChunk - 1) / kWaveChunk;
-        if (grid > need) grid = need;
-        e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
-        if (e != cudaSuccess) return e;
-        kern<<<(unsigned)grid, kWaveThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, poolOffset, wa);
+        kern<<<(unsigned)grid, kWaveThreads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, lay.buffers, wa);
         return cudaGetLastError();
     }
     if (variant == 5)
     {
-        const int simd = (sc.count + 3) / 4 * 4;
-        const int kform = !sc.kformOk ? 0 : (sc.kformMode == 1 || simd > 1024 ? 1 : 2);
-        auto kern = kform == 2 ? k_fast_tileq<6, 2> : kform == 1 ? k_fast_tileq<6, 1> : k_fast_tileq<6, 0>;
-        const size_t dyn5 = kform == 2 ? ((sc.stagedBytes + 127u) & ~127u) + (size_t)simd * 16 : sc.stagedBytes;
-        e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn5);
+        const int kform = fast_group_kform(sc);
+        auto kern = for_kform<2>(kform, [](auto K) { return k_fast_tileq<6, decltype(K)::value>; });
+        const size_t dyn = fast_smem(sc.stagedBytes, kform == 2 ? simd_count(sc) * 16 : 0).bytes;
+        // the tile size follows from the resident grid, which is clamped to the tiles afterwards
+        e = persistent_grid(kern, kQueueThreads, dyn, numSMs, LLONG_MAX, p, stream, grid);
         if (e != cudaSuccess) return e;
-        int perSM = 0;
-        e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, kQueueThreads, dyn5);
-        if (e != cudaSuccess) return e;
-        if (perSM < 1) perSM = 1;
-        float wPrev = 1.0f;
-        for (int f = 0; f < p.numFrames; ++f) wPrev *= lerp_fac(p.frame0 + f, p.flags);
-        const long long regionPix = (long long)p.numRows * p.width;
         // tile size: >= ~8192 paths per tile keeps the per-tile barrier tail < 1-2 %; then shrink (down to one slab)
         // until there are >= 8 tiles per CTA so the end-of-kernel quantisation stays small on sharded images
-        const uint32_t S = (uint32_t)(p.spp * p.numFrames);
-        long long grid = (long long)numSMs * perSM;
         uint32_t tileQPix = (8192 / S + kSlabPix - 1) / kSlabPix * kSlabPix;
         if (tileQPix < (uint32_t)kSlabPix) tileQPix = kSlabPix;
         if (tileQPix > (uint32_t)kTileQPix) tileQPix = kTileQPix;
         while (tileQPix > (uint32_t)kSlabPix && (regionPix + tileQPix - 1) / tileQPix < 8 * grid && tileQPix * S > 2048) tileQPix -= kSlabPix;
         const long long tiles = (regionPix + tileQPix - 1) / tileQPix;
         if (grid > tiles) grid = tiles;
-        e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
-        if (e != cudaSuccess) return e;
-        kern<<<(unsigned)grid, kQueueThreads, dyn5, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                                (uint32_t)tiles, S, wPrev, tileQPix);
+        kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                                                               (uint32_t)tiles, S, prev_weight(p.frame0, p.numFrames, p.flags), tileQPix);
         return cudaGetLastError();
     }
     return cudaErrorInvalidValue;

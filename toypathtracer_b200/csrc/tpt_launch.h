@@ -38,5 +38,23 @@ cudaError_t launch_refgpu_fast(const DrawParams& p, const SceneDev& sc, int numS
 int fast_slab_pixels();
 int fast_kernel_launches(const DrawParams& p, int variant);
 bool fast_variant_writes_final_pixels(int variant);   // the trace kernel stores finished pixels itself (no L2 reductions)
+// weight of `prev` when frames [frame0, frame0 + numFrames) are blended into it: the product of their lerp_fac
+float prev_weight(int frame0, int numFrames, unsigned flags);
+
+// Launch set-up of a persistent kernel: allows `dyn` bytes of dynamic shared memory, sizes the grid to the CTAs that stay
+// resident on numSMs SMs (at least one per SM) but no more than `ctasNeeded`, and zeroes the work counter.
+template <class Kernel>
+cudaError_t persistent_grid(Kernel kern, int threads, size_t dyn, int numSMs, long long ctasNeeded, const DrawParams& p,
+                            cudaStream_t stream, long long& grid)
+{
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+    if (e != cudaSuccess) return e;
+    int perSM = 0;
+    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, threads, dyn);
+    if (e != cudaSuccess) return e;
+    grid = (long long)numSMs * (perSM < 1 ? 1 : perSM);
+    if (grid > ctasNeeded) grid = ctasNeeded;
+    return cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+}
 
 } // namespace tpt

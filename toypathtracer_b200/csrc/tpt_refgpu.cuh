@@ -271,7 +271,7 @@ template <bool EXACT> struct RgSetupPlain
 {
     using Hitter = SerialHitter<EXACT, false>;
     static constexpr int kMinBlocks = 1;
-    static size_t extra_smem(const SceneDev&) { return 0; }
+    static size_t dyn_smem(const SceneDev& sc) { return sc.stagedBytes; }
     static __device__ __forceinline__ Hitter prepare(SceneView& sc, unsigned char* smem, const SceneBlobLayout& L, uint32_t)
     {
         // the shader loops over sphereCount spheres only (ComputeShader.hlsl:134): the SIMD padding of the CPU path's SoA
@@ -338,28 +338,19 @@ k_refgpu(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L
         if (!__any_sync(0xffffffffu, st.active)) break;
         if (st.active && rg_step<EXACT>(p, sc, st, rc, hitter)) st.active = false;
     }
-    for (int off = 16; off > 0; off >>= 1) rc += __shfl_xor_sync(0xffffffffu, rc, off);
-    if (lane == 0 && rc) atomicAdd(p.rayCounter, (unsigned long long)rc);
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 template <bool EXACT, class Setup = RgSetupPlain<EXACT>>
 static cudaError_t launch_refgpu_t(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
 {
     auto kern = k_refgpu<EXACT, Setup>;
-    const size_t dyn = sc.stagedBytes + Setup::extra_smem(sc);
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
-    if (e != cudaSuccess) return e;
-    int perSM = 0;
-    e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&perSM, kern, kRgThreads, dyn);
-    if (e != cudaSuccess) return e;
-    if (perSM < 1) perSM = 1;
+    const size_t dyn = Setup::dyn_smem(sc);
     const long long regionPix = (long long)p.numRows * p.width;
     const long long slabs = (regionPix + kRgSlabPix - 1) / kRgSlabPix;
     if (slabs > 0x7fffffffLL) return cudaErrorInvalidValue;
-    long long grid = (long long)numSMs * perSM;
-    const long long ctasNeeded = (slabs + kRgThreads / 32 - 1) / (kRgThreads / 32);
-    if (grid > ctasNeeded) grid = ctasNeeded;
-    e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+    long long grid = 0;
+    cudaError_t e = persistent_grid(kern, kRgThreads, dyn, numSMs, (slabs + kRgThreads / 32 - 1) / (kRgThreads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
     kern<<<(unsigned)grid, kRgThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, (uint32_t)slabs);
     return cudaGetLastError();
