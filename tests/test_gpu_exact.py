@@ -35,7 +35,7 @@ def test_golden_vectors(gpu_ctx):
     g = np.load(os.path.join(GOLD, "ref_192x108_f0-3.npz"))
     sph, mats, cam, em = golden_scene()
     gpu_ctx.set_scene(sph, mats, cam, em)
-    for lanes in (32, 8, 9, 1, 2, 64, 65, 70, 0):
+    for lanes in (32, 8, 9, 1, 2, 64, 65, 66, 67, 70, 71, 0):
         gpu_ctx.set_option("exact_lanes", lanes)
         # frame by frame (numFrames = 1: blend fused into the trace kernel)
         buf = np.zeros((108, 192, 4), np.float32)

@@ -25,7 +25,7 @@ def kernel_counts(lib):
             if cur: rows.append((demangle(cur), n, cnt))
             cur, cnt, n = m.group(1), collections.Counter(), 0
             continue
-        if cur and re.match(r"\s+/\*[0-9a-f]{4}\*/", line):
+        if cur and re.match(r"\s+/\*[0-9a-f]{4,}\*/", line):
             n += 1
             for name, rx in COLS:
                 if re.search(rx, line): cnt[name] += 1

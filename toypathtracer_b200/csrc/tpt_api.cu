@@ -612,7 +612,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
                 CK(cudaMemsetAsync(ctx->dLookRays, 0, L * sizeof(unsigned long long), stream), "zero lookahead counters");
                 DrawParams pl = p;
                 pl.frame0 = frameCount; pl.numFrames = (int)L; pl.scratch = ctx->dLook; pl.rayCounter = ctx->dLookRays;
-                e = launch_exact(pl, scene, ctx->exactLanes, stream, /*resolve*/ L == 1);
+                e = launch_exact(pl, scene, ctx->exactLanes, ctx->numSMs, stream, /*resolve*/ L == 1);
                 if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
                 ctx->lastLaunches += 1;
                 k.frame0 = frameCount; k.n = (int)L;
@@ -637,7 +637,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
                 if (r) return r;
                 p.scratch = ctx->dScratch;
             }
-            e = launch_exact(p, scene, ctx->exactLanes, stream);
+            e = launch_exact(p, scene, ctx->exactLanes, ctx->numSMs, stream);
             ctx->lastLaunches += nf > 1 ? 2 : 1;
         }
         else if (refgpu)

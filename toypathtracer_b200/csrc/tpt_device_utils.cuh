@@ -36,19 +36,24 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity)
 // Producer/consumer waits of warps that share an SM with working warps: try_wait with a suspend-time hint, and a
 // nanosleep between attempts, so that a waiting warp issues a handful of instructions per microsecond instead of spinning
 // (measured in the split exact kernel: the plain try_wait loop was 23 % of all issued instructions).
+// CLUSTER: the barrier is arrived at from another CTA of the cluster, so the wait acquires at cluster scope.
+template <bool CLUSTER = false>
 __device__ __forceinline__ void mbar_wait_sleep(uint64_t* bar, uint32_t parity)
 {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n"
-        "@p bra DONE_S;\n"
-        "WAIT_LOOP_S:\n"
-        "nanosleep.u32 128;\n"          // 32 .. 1024 ns measured: no difference in frame time
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1, %2;\n"
-        "@!p bra WAIT_LOOP_S;\n"
-        "DONE_S:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity), "r"(100000u) : "memory");
+#define TPT_WAIT_SLEEP(TRY_WAIT)                                                                                              \
+    asm volatile(                                                                                                             \
+        "{\n"                                                                                                                 \
+        ".reg .pred p;\n" TRY_WAIT " p, [%0], %1, %2;\n"                                                                      \
+        "@p bra DONE_S;\n"                                                                                                    \
+        "WAIT_LOOP_S:\n"                                                                                                      \
+        "nanosleep.u32 128;\n" /* 32 .. 1024 ns measured: no difference in frame time */                                     \
+        TRY_WAIT " p, [%0], %1, %2;\n"                                                                                        \
+        "@!p bra WAIT_LOOP_S;\n"                                                                                              \
+        "DONE_S:\n"                                                                                                           \
+        "}\n" ::"r"(smem_u32(bar)), "r"(parity), "r"(100000u) : "memory")
+    if constexpr (CLUSTER) TPT_WAIT_SLEEP("mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64");
+    else TPT_WAIT_SLEEP("mbarrier.try_wait.parity.shared::cta.b64");
+#undef TPT_WAIT_SLEEP
 }
 // 1-D bulk copy global -> shared through the TMA unit; bytes % 16 == 0, both addresses 16 B aligned.
 __device__ __forceinline__ void tma_bulk_g2s(void* dstSmem, const void* srcGlobal, uint32_t bytes, uint64_t* bar)

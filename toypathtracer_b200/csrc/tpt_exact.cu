@@ -15,6 +15,64 @@
 
 namespace tpt {
 
+// The (frame, row) of a chain. Consecutive chains = the same row in consecutive frames: neighbouring lanes trace the same
+// pixels with different RNG streams (coherent geometry, similar path lengths), and the expensive bottom rows are
+// scheduled first. Every kernel uses this order.
+struct Chain
+{
+    int ri, fi;          // row index within the draw, frame index within the draw
+    int y, frame;        // image row, frame number (seeds the row's RNG stream)
+    size_t imgRow;       // first pixel of the row in p.image
+};
+template <class Index>
+__device__ __forceinline__ Chain decode_chain(const DrawParams& p, Index chain)
+{
+    Chain c;
+    c.ri = (int)(chain / (Index)p.numFrames);
+    c.fi = (int)(chain % (Index)p.numFrames);
+    c.y = p.row0 + c.ri * p.rowStep;
+    c.frame = p.frame0 + c.fi;
+    c.imgRow = (size_t)(p.packed ? c.ri : c.y) * p.width;
+    return c;
+}
+
+// LANES consecutive lanes of the warp share one ray (LANES = 1, 8, 16 or 32).
+template <int EXACT, int LANES>
+__device__ __forceinline__ GroupHitter<EXACT, LANES> group_hitter(int lane)
+{
+    GroupHitter<EXACT, LANES> h;
+    h.sub = lane % LANES;
+    h.mask = LANES == 32 ? 0xffffffffu : (((1u << (LANES & 31)) - 1u) << (lane - h.sub));
+    return h;
+}
+
+// Test.cpp:293-295: prev*lerpFac + col*(1-lerpFac) per component; alpha is never written by the CPU path
+__device__ __forceinline__ void blend(float4& prev, V3 col, float lerpFac)
+{
+    const float oneMinus = 1.0f - lerpFac;
+    prev.x = prev.x * lerpFac + col.x * oneMinus;
+    prev.y = prev.y * lerpFac + col.y * oneMinus;
+    prev.z = prev.z * lerpFac + col.z * oneMinus;
+}
+
+// A finished pixel of chain c: blended into p.image when the draw has one frame, else stored in p.scratch for
+// k_resolve_exact, which blends the frames in order.
+__device__ __forceinline__ void store_pixel(const DrawParams& p, const Chain& c, int x, V3 col, float lerpFac)
+{
+    if (p.numFrames == 1)
+    {
+        float4* px = reinterpret_cast<float4*>(p.image + (c.imgRow + x) * 4);
+        float4 prev = *px;
+        blend(prev, col, lerpFac);
+        *px = prev;
+    }
+    else
+    {
+        float4* px = reinterpret_cast<float4*>(p.scratch) + ((size_t)c.fi * p.numRows + c.ri) * p.width + x;
+        *px = make_float4(col.x, col.y, col.z, 0.0f);
+    }
+}
+
 template <int LANES>
 __global__ void k_trace_exact(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L,
                               int count, int nLights, uint32_t stagedBytes)
@@ -24,50 +82,21 @@ __global__ void k_trace_exact(DrawParams p, const unsigned char* __restrict__ bl
     stage_blob(smem, blob, stagedBytes, &bar);
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
 
-    const int lane = threadIdx.x & 31;
-    const int sub = threadIdx.x % LANES;
     const long long chain = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / LANES;
     const long long totalChains = (long long)p.numRows * p.numFrames;
     if (chain >= totalChains) return;
-    // consecutive chains = the same row in consecutive frames: neighbouring lanes trace the same pixels with different
-    // RNG streams (coherent geometry, similar path lengths), and the expensive bottom rows are scheduled first
-    const int ri = (int)(chain / p.numFrames);
-    const int fi = (int)(chain % p.numFrames);
-    const int y = p.row0 + ri * p.rowStep;
-    const int frame = p.frame0 + fi;
+    const Chain ch = decode_chain(p, chain);
+    const GroupHitter<1, LANES> hitter = group_hitter<1, LANES>(threadIdx.x & 31);
 
-    GroupHitter<true, LANES> hitter;
-    hitter.sub = sub;
-    hitter.mask = LANES == 32 ? 0xffffffffu : (((1u << (LANES & 31)) - 1u) << (lane - sub));
-
-    uint32_t state = row_seed(y, frame);
+    uint32_t state = row_seed(ch.y, ch.frame);
     unsigned rc = 0;
-    const float lerpFac = lerp_fac(frame, p.flags);
-    const float oneMinus = 1.0f - lerpFac;
-    const size_t imgRow = (size_t)(p.packed ? ri : y) * p.width;
+    const float lerpFac = lerp_fac(ch.frame, p.flags);
     for (int x = 0; x < p.width; ++x)
     {
-        V3 col = pixel_exact(sc, p.cam, x, y, p.spp, p.invWidth, p.invHeight, state, rc, hitter);
-        if (sub == 0)
-        {
-            if (p.numFrames == 1)
-            {
-                // Test.cpp:293-295: prev*lerpFac + col*(1-lerpFac); alpha is never written by the CPU path
-                float4* px = reinterpret_cast<float4*>(p.image + (imgRow + x) * 4);
-                float4 prev = *px;
-                prev.x = prev.x * lerpFac + col.x * oneMinus;
-                prev.y = prev.y * lerpFac + col.y * oneMinus;
-                prev.z = prev.z * lerpFac + col.z * oneMinus;
-                *px = prev;
-            }
-            else
-            {
-                float4* px = reinterpret_cast<float4*>(p.scratch) + ((size_t)fi * p.numRows + ri) * p.width + x;
-                *px = make_float4(col.x, col.y, col.z, 0.0f);
-            }
-        }
+        V3 col = pixel_exact(sc, p.cam, x, ch.y, p.spp, p.invWidth, p.invHeight, state, rc, hitter);
+        if (hitter.sub == 0) store_pixel(p, ch, x, col, lerpFac);
     }
-    if (sub == 0) atomicAdd(p.rayCounter + fi, (unsigned long long)rc);
+    if (hitter.sub == 0) atomicAdd(p.rayCounter + ch.fi, (unsigned long long)rc);
 }
 
 // One thread per chain, flat form: every loop iteration is one xchain_step() = one sphere sweep, so the lanes of a
@@ -80,58 +109,24 @@ k_trace_exact_flat(DrawParams p, const unsigned char* __restrict__ blob, SceneBl
     __shared__ uint64_t bar;
     stage_blob(smem, blob, stagedBytes, &bar);
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    const int lane = threadIdx.x & 31;
-    const int sub = threadIdx.x % LANES;
     const long long chain = ((long long)blockIdx.x * blockDim.x + threadIdx.x) / LANES;
     const long long totalChains = (long long)p.numRows * p.numFrames;
     if (chain >= totalChains) return;
-    const int ri = (int)(chain / p.numFrames);
-    const int fi = (int)(chain % p.numFrames);
-    const int y = p.row0 + ri * p.rowStep;
-    const int frame = p.frame0 + fi;
-    const float lerpFac = lerp_fac(frame, p.flags);
-    const float oneMinus = 1.0f - lerpFac;
-    const size_t imgRow = (size_t)(p.packed ? ri : y) * p.width;
-    GroupHitter<true, LANES> hitter;       // LANES lanes share the chain: replicated state, split sweep (see k_trace_exact)
-    hitter.sub = sub;
-    hitter.mask = LANES == 32 ? 0xffffffffu : (((1u << (LANES & 31)) - 1u) << (lane - sub));
+    const Chain ch = decode_chain(p, chain);
+    const float lerpFac = lerp_fac(ch.frame, p.flags);
+    // LANES lanes share the chain: replicated state, split sweep (see k_trace_exact)
+    const GroupHitter<1, LANES> hitter = group_hitter<1, LANES>(threadIdx.x & 31);
     unsigned rc = 0;
     XChain c;
-    xchain_begin(c, p.cam, y, frame, p.invWidth, p.invHeight);
+    xchain_begin(c, p.cam, ch.y, ch.frame, p.invWidth, p.invHeight);
     while (c.x < p.width)
     {
         const int x = c.x;
         V3 col;
-        if (xchain_step(sc, p.cam, c, y, p.spp, p.width, p.invWidth, p.invHeight, rc, hitter, col) && sub == 0)
-        {
-            if (p.numFrames == 1)
-            {
-                float4* px = reinterpret_cast<float4*>(p.image + (imgRow + x) * 4);
-                float4 prev = *px;
-                prev.x = prev.x * lerpFac + col.x * oneMinus;
-                prev.y = prev.y * lerpFac + col.y * oneMinus;
-                prev.z = prev.z * lerpFac + col.z * oneMinus;
-                *px = prev;
-            }
-            else
-            {
-                float4* px = reinterpret_cast<float4*>(p.scratch) + ((size_t)fi * p.numRows + ri) * p.width + x;
-                *px = make_float4(col.x, col.y, col.z, 0.0f);
-            }
-        }
+        if (xchain_step(sc, p.cam, c, ch.y, p.spp, p.width, p.invWidth, p.invHeight, rc, hitter, col) && hitter.sub == 0)
+            store_pixel(p, ch, x, col, lerpFac);
     }
-    if (sub == 0) atomicAdd(p.rayCounter + fi, (unsigned long long)rc);
-}
-
-template <int LANES>
-static cudaError_t launch_exact_flat_t(const DrawParams& p, const SceneDev& sc, cudaStream_t stream)
-{
-    const long long threads = (long long)p.numRows * p.numFrames * LANES;
-    auto kern = k_trace_exact_flat<LANES>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
-    if (e != cudaSuccess) return e;
-    kern<<<(unsigned)((threads + 127) / 128), 128, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
-    return cudaGetLastError();
+    if (hitter.sub == 0) atomicAdd(p.rayCounter + ch.fi, (unsigned long long)rc);
 }
 
 // Sequential progressive blend of the per-frame colours (Test.cpp:272-276,293-295), one thread per pixel,
@@ -149,11 +144,8 @@ __global__ void k_resolve_exact(DrawParams p)
     for (int fi = 0; fi < p.numFrames; ++fi, s += n)
     {
         const float lerpFac = lerp_fac(p.frame0 + fi, p.flags);
-        const float oneMinus = 1.0f - lerpFac;
         float4 col = ld_stream_f4(reinterpret_cast<const float*>(s));
-        prev.x = prev.x * lerpFac + col.x * oneMinus;
-        prev.y = prev.y * lerpFac + col.y * oneMinus;
-        prev.z = prev.z * lerpFac + col.z * oneMinus;
+        blend(prev, v3(col.x, col.y, col.z), lerpFac);
     }
     *px = prev;
 }
@@ -174,19 +166,122 @@ __global__ void k_resolve_exact(DrawParams p)
 constexpr int kRingDepth = 16;      // events per shade warp in flight
 constexpr int kPixSlots = 16;       // pixels whose samples may be in flight (see the capacity argument in DESIGN.md)
 constexpr int kSplitMaxSpp = 8;
+enum { XE_BEGIN = 4, XE_QUIT = 5 };   // cluster kernel only: a chain starts / the path warp is done
 
-struct __align__(16) XEventSlot { float4 q0, q1, q2; };
+// One event of xpath_sample(): a, b, c in q0..q2.xyz, the RNG state in q1.w, and in q0.w the tag: the type (XE_*) in the
+// low 3 bits, above them the material id (XE_BEGIN: the chain index).
+struct __align__(16) XEventSlot
+{
+    float4 q0, q1, q2;
+    __device__ __forceinline__ int type() const { return __float_as_int(q0.w) & 7; }
+    __device__ __forceinline__ int mid() const { return __float_as_int(q0.w) >> 3; }
+};
+__device__ __forceinline__ XEventSlot make_event(int type, int mid, V3 a, V3 b, V3 c, uint32_t rng)
+{
+    return {make_float4(a.x, a.y, a.z, __int_as_float(type | (mid << 3))), make_float4(b.x, b.y, b.z, __uint_as_float(rng)),
+            make_float4(c.x, c.y, c.z, 0.0f)};
+}
+template <class LightFn>
+__device__ __forceinline__ bool shade_event(const SceneView& sc, XShade& sh, const XEventSlot& e, LightFn&& lights, V3& result)
+{
+    return xshade_event(sc, sh, e.type(), e.mid(), v3(e.q0.x, e.q0.y, e.q0.z), v3(e.q1.x, e.q1.y, e.q1.z),
+                        v3(e.q2.x, e.q2.y, e.q2.z), __float_as_uint(e.q1.w), lights, result);
+}
+
+// Event number `seq` of a ring: its slot, and the parity of that slot's barriers on this lap.
+struct RingPos { uint32_t slot, phase; };
+__device__ __forceinline__ RingPos ring_pos(uint32_t seq) { return {seq % kRingDepth, (seq / kRingDepth) & 1u}; }
+
+// Returns seq[h] and increments it. The unrolled select keeps the array in registers for a runtime h.
+template <int N>
+__device__ __forceinline__ uint32_t next_seq(uint32_t (&seq)[N], int h)
+{
+    uint32_t sq = 0;
+#pragma unroll
+    for (int i = 0; i < N; ++i) if (i == h) sq = seq[i];
+#pragma unroll
+    for (int i = 0; i < N; ++i) if (i == h) seq[i] = sq + 1;
+    return sq;
+}
 
 __device__ __forceinline__ void mbar_arrive(uint64_t* bar)
 {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 
+// lightE of a Lambert vertex on a shade warp (Test.cpp:96-133): the two half-warps (grp = lane / 16) sample and trace two
+// lights at a time, and the contributions are added in the reference's light order (Test.cpp:96).
+template <int SMODE>
+__device__ __forceinline__ V3 shade_lights(const SceneView& sc, const GroupHitter<SMODE, 16>& hitter, int grp, int mid, V3 pos,
+                                           V3 normal, V3 rdir, V3 albedo, uint32_t rng)
+{
+    V3 lightE = v3(0, 0, 0);
+    int myJ = -1, kk = 0;
+    uint32_t myRng = 0;
+    auto run_batch = [&]() {
+        V3 contrib = v3(0, 0, 0);
+        bool reached = false;
+        if (myJ >= 0)
+        {
+            const LightRec Lr = sc.lights[myJ];
+            V3 l;
+            sample_light<SMODE>(Lr, pos, normal, rdir, albedo, myRng, l, contrib);
+            float ts;
+            reached = hitter.hit(sc, pos, l, TPT_MIN_T, TPT_MAX_T, ts) == Lr.id;
+        }
+        __syncwarp();
+#pragma unroll
+        for (int g = 0; g < 2; ++g)
+        {
+            const bool r = __shfl_sync(0xffffffffu, reached ? 1 : 0, g * 16) != 0;
+            const V3 cg = v3(__shfl_sync(0xffffffffu, contrib.x, g * 16), __shfl_sync(0xffffffffu, contrib.y, g * 16),
+                             __shfl_sync(0xffffffffu, contrib.z, g * 16));
+            if (r) lightE = lightE + cg;
+        }
+        myJ = -1;
+    };
+    for (int j = 0; j < sc.nLights; ++j)
+    {
+        if (sc.lights[j].id == mid) continue;                  // Test.cpp:100
+        if ((kk & 1) == grp) { myJ = j; myRng = rng; }
+        XorShift32(rng); XorShift32(rng);                      // eps1, eps2 of this light (Test.cpp:112)
+        if ((++kk & 1) == 0) run_batch();
+    }
+    if (kk & 1) run_batch();
+    return lightE;
+}
+
+// Hands sample s of the pixel in slot ps to the slot; the warp whose sample completes the pixel sums the samples in sample
+// order (Test.cpp:289-291), scales by invSpp (Test.cpp:291) and stores the pixel. All 32 lanes call it.
+__device__ __forceinline__ void finish_sample(float (*pixRes)[kSplitMaxSpp][3], unsigned* pixCnt, int ps, int s, int spp,
+                                              float invSpp, V3 result, int lane, const DrawParams& p, const Chain& ch, int x,
+                                              float lerpFac)
+{
+    unsigned old = 0;
+    if (lane == 0)
+    {
+        pixRes[ps][s][0] = result.x; pixRes[ps][s][1] = result.y; pixRes[ps][s][2] = result.z;
+        __threadfence_block();
+        old = atomicInc(&pixCnt[ps], (unsigned)spp - 1u);      // wraps to 0 with the pixel's last sample
+    }
+    old = __shfl_sync(0xffffffffu, old, 0);
+    if (old == (unsigned)spp - 1u && lane == 0)
+    {
+        __threadfence_block();
+        V3 col = v3(0, 0, 0);
+        for (int t = 0; t < spp; ++t)
+            col = col + v3(((volatile float*)pixRes[ps][t])[0], ((volatile float*)pixRes[ps][t])[1], ((volatile float*)pixRes[ps][t])[2]);
+        store_pixel(p, ch, x, col * invSpp, lerpFac);
+    }
+    __syncwarp();
+}
+
 constexpr int split_block_threads(int H) { return H <= 3 ? 128 : 32 * (1 + H); }   // 4-warp CTAs: one role per SM sub-partition
 
 template <int H, int DRY = 0, int SMODE = 1>     // DRY: timing probes — 1 = shade warps only drain the rings, 2 = everything but the light sampling;
                                                  // SMODE: arithmetic flavour of the shade warps (1 = inlined: 882 Mray/s at 720p; 2 = shared out-of-line sqrt/div/libm: 780)
-__global__ void __launch_bounds__(split_block_threads(H))
+// SMODE 2 is held to 64 registers (8 CTAs per SM) like the other forms; ptxas would otherwise give it 72 to spill less
+__global__ void __launch_bounds__(split_block_threads(H), SMODE == 2 ? 8 : 0)
 k_trace_exact_split(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes)
 {
     extern __shared__ __align__(128) unsigned char smem[];
@@ -208,19 +303,15 @@ k_trace_exact_split(DrawParams p, const unsigned char* __restrict__ blob, SceneB
 
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;     // (rotating the roles over the 4 sub-partitions: no effect, measured)
     const long long chain = blockIdx.x;
-    // same chain order as k_trace_exact: consecutive chains = the same row in consecutive frames
-    const int ri = (int)(chain / p.numFrames), fi = (int)(chain % p.numFrames);
-    const int y = p.row0 + ri * p.rowStep;
-    const int frame = p.frame0 + fi;
+    const Chain ch = decode_chain(p, chain);
     const int spp = p.spp;
     const uint32_t totalSamples = (uint32_t)p.width * (uint32_t)spp;
 
     if (warp == 0)
     {
         // ---- PATH warp: the chain's RNG stream, sweeps split over the 32 lanes
-        GroupHitter<1, 32> hitter;
-        hitter.sub = lane; hitter.mask = 0xffffffffu;
-        uint32_t rng = row_seed(y, frame);
+        const GroupHitter<1, 32> hitter = group_hitter<1, 32>(lane);
+        uint32_t rng = row_seed(ch.y, ch.frame);
         unsigned rc = 0;
         uint32_t seq[H];
 #pragma unroll
@@ -231,76 +322,30 @@ k_trace_exact_split(DrawParams p, const unsigned char* __restrict__ blob, SceneB
             {
                 const int h = H == 1 ? 0 : (int)(k % (uint32_t)H);
                 auto emit = [&](int type, int mid, V3 a, V3 b, V3 c, uint32_t erng) {
-                                 uint32_t sq = 0;
-#pragma unroll
-                                 for (int hh = 0; hh < H; ++hh) if (hh == h) sq = seq[hh];
-                                 const uint32_t slot = sq % kRingDepth, phase = (sq / kRingDepth) & 1u;
-                                 mbar_wait_sleep(&emptyBar[h][slot], phase ^ 1u);      // slot free (passes at once on a fresh barrier)
+                                 const RingPos r = ring_pos(next_seq(seq, h));
+                                 mbar_wait_sleep(&emptyBar[h][r.slot], r.phase ^ 1u);      // slot free (passes at once on a fresh barrier)
                                  if (lane == 0)
                                  {
-                                     XEventSlot& e = ring[h][slot];
-                                     e.q0 = make_float4(a.x, a.y, a.z, __int_as_float(type | (mid << 2)));
-                                     e.q1 = make_float4(b.x, b.y, b.z, __uint_as_float(erng));
-                                     e.q2 = make_float4(c.x, c.y, c.z, 0.0f);
-                                     mbar_arrive(&fullBar[h][slot]);            // release: the stores above are visible to the waiter
+                                     ring[h][r.slot] = make_event(type, mid, a, b, c, erng);
+                                     mbar_arrive(&fullBar[h][r.slot]);          // release: the stores above are visible to the waiter
                                  }
-#pragma unroll
-                                 for (int hh = 0; hh < H; ++hh) if (hh == h) seq[hh] = sq + 1;
                              };
-                xpath_sample(sc, p.cam, x, y, p.invWidth, p.invHeight, rng, rc, hitter, emit);
+                xpath_sample(sc, p.cam, x, ch.y, p.invWidth, p.invHeight, rng, rc, hitter, emit);
             }
-        if (lane == 0) atomicAdd(p.rayCounter + fi, (unsigned long long)rc);
+        if (lane == 0) atomicAdd(p.rayCounter + ch.fi, (unsigned long long)rc);
         return;
     }
 
     // ---- SHADE warp h: samples k = h, h + H, ...
     const int h = warp - 1;
     if (h >= H) return;                                          // padding warp of the 4-warp CTA
-    const int grp = lane >> 4;                                   // half-warp = one light
-    GroupHitter<SMODE, 16> hitter;
-    hitter.sub = lane & 15; hitter.mask = 0xffffu << (grp * 16);
-    const float lerpFac = lerp_fac(frame, p.flags);
-    const float oneMinus = 1.0f - lerpFac;
+    const GroupHitter<SMODE, 16> hitter = group_hitter<SMODE, 16>(lane);   // half-warp = one light
+    const float lerpFac = lerp_fac(ch.frame, p.flags);
     const float invSpp = M<SMODE>::div_(1.0f, (float)spp);
-    const size_t imgRow = (size_t)(p.packed ? ri : y) * p.width;
     uint32_t seq = 0;
-
     auto lights = [&](int mid, V3 pos, V3 normal, V3 rdir, V3 albedo, uint32_t rng) -> V3 {
-        V3 lightE = v3(0, 0, 0);
-        if (DRY == 2) return lightE;                                // probe: shading without the light sampling
-        int myJ = -1, kk = 0;
-        uint32_t myRng = 0;
-        auto run_batch = [&]() {
-            V3 contrib = v3(0, 0, 0);
-            bool reached = false;
-            if (myJ >= 0)
-            {
-                const LightRec Lr = sc.lights[myJ];
-                V3 l;
-                sample_light<SMODE>(Lr, pos, normal, rdir, albedo, myRng, l, contrib);
-                float ts;
-                reached = hitter.hit(sc, pos, l, TPT_MIN_T, TPT_MAX_T, ts) == Lr.id;
-            }
-            __syncwarp();
-#pragma unroll
-            for (int g = 0; g < 2; ++g)                            // the reference's light order (Test.cpp:96)
-            {
-                const bool r = __shfl_sync(0xffffffffu, reached ? 1 : 0, g * 16) != 0;
-                const V3 cg = v3(__shfl_sync(0xffffffffu, contrib.x, g * 16), __shfl_sync(0xffffffffu, contrib.y, g * 16),
-                                 __shfl_sync(0xffffffffu, contrib.z, g * 16));
-                if (r) lightE = lightE + cg;
-            }
-            myJ = -1;
-        };
-        for (int j = 0; j < sc.nLights; ++j)
-        {
-            if (sc.lights[j].id == mid) continue;                  // Test.cpp:100
-            if ((kk & 1) == grp) { myJ = j; myRng = rng; }
-            XorShift32(rng); XorShift32(rng);                      // eps1, eps2 of this light (Test.cpp:112)
-            if ((++kk & 1) == 0) run_batch();
-        }
-        if (kk & 1) run_batch();
-        return lightE;
+        if (DRY == 2) return v3(0, 0, 0);                        // probe: shading without the light sampling
+        return shade_lights<SMODE>(sc, hitter, lane >> 4, mid, pos, normal, rdir, albedo, rng);
     };
 
     for (uint32_t k = (uint32_t)h; k < totalSamples; k += (uint32_t)H)
@@ -311,51 +356,16 @@ k_trace_exact_split(DrawParams p, const unsigned char* __restrict__ blob, SceneB
         V3 result;
         for (;;)
         {
-            const uint32_t slot = seq % kRingDepth, phase = (seq / kRingDepth) & 1u;
-            mbar_wait_sleep(&fullBar[h][slot], phase);
-            const XEventSlot& e = ring[h][slot];
-            const float4 q0 = e.q0, q1 = e.q1, q2 = e.q2;
+            const RingPos r = ring_pos(seq++);
+            mbar_wait_sleep(&fullBar[h][r.slot], r.phase);
+            const XEventSlot e = ring[h][r.slot];
             __syncwarp();
-            if (lane == 0) mbar_arrive(&emptyBar[h][slot]);
-            ++seq;
-            const int tm = __float_as_int(q0.w);
-            if (DRY == 1) { if ((tm & 3) >= XE_END_SKY) { result = v3(0, 0, 0); break; } continue; }   // probe: path warp alone
-            if (xshade_event(sc, sh, tm & 3, tm >> 2, v3(q0.x, q0.y, q0.z), v3(q1.x, q1.y, q1.z), v3(q2.x, q2.y, q2.z),
-                             __float_as_uint(q1.w), lights, result)) break;
+            if (lane == 0) mbar_arrive(&emptyBar[h][r.slot]);
+            if (DRY == 1) { if (e.type() >= XE_END_SKY) { result = v3(0, 0, 0); break; } continue; }   // probe: path warp alone
+            if (shade_event(sc, sh, e, lights, result)) break;
         }
         // hand the sample to its pixel; whoever completes the pixel finishes it
-        const int ps = x % kPixSlots;
-        unsigned old = 0;
-        if (lane == 0)
-        {
-            pixRes[ps][s][0] = result.x; pixRes[ps][s][1] = result.y; pixRes[ps][s][2] = result.z;
-            __threadfence_block();
-            old = atomicInc(&pixCnt[ps], (unsigned)spp - 1u);      // wraps to 0 with the pixel's last sample
-        }
-        old = __shfl_sync(0xffffffffu, old, 0);
-        if (old == (unsigned)spp - 1u && lane == 0)
-        {
-            __threadfence_block();
-            V3 col = v3(0, 0, 0);
-            for (int t = 0; t < spp; ++t)
-                col = col + v3(((volatile float*)pixRes[ps][t])[0], ((volatile float*)pixRes[ps][t])[1], ((volatile float*)pixRes[ps][t])[2]);
-            col = col * invSpp;                                    // Test.cpp:291
-            if (p.numFrames == 1)
-            {
-                float4* px = reinterpret_cast<float4*>(p.image + (imgRow + x) * 4);
-                float4 prev = *px;
-                prev.x = prev.x * lerpFac + col.x * oneMinus;      // Test.cpp:293-295, alpha untouched
-                prev.y = prev.y * lerpFac + col.y * oneMinus;
-                prev.z = prev.z * lerpFac + col.z * oneMinus;
-                *px = prev;
-            }
-            else
-            {
-                float4* px = reinterpret_cast<float4*>(p.scratch) + ((size_t)fi * p.numRows + ri) * p.width + x;
-                *px = make_float4(col.x, col.y, col.z, 0.0f);
-            }
-        }
-        __syncwarp();
+        finish_sample(pixRes, pixCnt, x % kPixSlots, s, spp, invSpp, result, lane, p, ch, x, lerpFac);
     }
 }
 
@@ -370,7 +380,6 @@ k_trace_exact_split(DrawParams p, const unsigned char* __restrict__ blob, SceneB
 constexpr int kCPathWarps = 10;
 constexpr int kCH = 2;
 constexpr int kCThreads = 32 * kCPathWarps * kCH;
-enum { XE_BEGIN = 4, XE_QUIT = 5 };
 
 struct ClusterShared
 {
@@ -395,20 +404,6 @@ __device__ __forceinline__ void cluster_sync_all()
 __device__ __forceinline__ void mbar_arrive_remote(uint32_t clusterAddr)
 {
     asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(clusterAddr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity)
-{
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1, %2;\n"
-        "@p bra DONE_C;\n"
-        "WAIT_LOOP_C:\n"
-        "nanosleep.u32 128;\n"
-        "mbarrier.try_wait.parity.acquire.cluster.shared::cta.b64 p, [%0], %1, %2;\n"
-        "@!p bra WAIT_LOOP_C;\n"
-        "DONE_C:\n"
-        "}\n" ::"r"(smem_u32(bar)), "r"(parity), "r"(100000u) : "memory");
 }
 __device__ __forceinline__ void st_cluster_f4(uint32_t clusterAddr, float4 v)
 {
@@ -440,27 +435,22 @@ k_trace_exact_cluster(DrawParams p, const unsigned char* __restrict__ blob, Scen
     if (rank == 0 && warp < kCPathWarps)
     {
         // ---- PATH warp `warp`
-        GroupHitter<1, 32> hitter;
-        hitter.sub = lane; hitter.mask = 0xffffffffu;
+        const GroupHitter<1, 32> hitter = group_hitter<1, 32>(lane);
         uint32_t seq[kCH];
 #pragma unroll
         for (int h = 0; h < kCH; ++h) seq[h] = 0;
         auto emit_to = [&](int h, int type, int mid, V3 a, V3 b, V3 c, uint32_t erng) {
-            uint32_t sq = 0;
-#pragma unroll
-            for (int hh = 0; hh < kCH; ++hh) if (hh == h) sq = seq[hh];
-            const uint32_t slot = sq % kRingDepth, phase = (sq / kRingDepth) & 1u;
-            mbar_wait_cluster(&cs.emptyBar[warp][h][slot], phase ^ 1u);
+            const RingPos r = ring_pos(next_seq(seq, h));
+            mbar_wait_sleep<true>(&cs.emptyBar[warp][h][r.slot], r.phase ^ 1u);
             if (lane == 0)
             {
-                const uint32_t e = map_to_cta(&cs.ring[warp][h][slot], 1);
-                st_cluster_f4(e, make_float4(a.x, a.y, a.z, __int_as_float(type | (mid << 3))));
-                st_cluster_f4(e + 16, make_float4(b.x, b.y, b.z, __uint_as_float(erng)));
-                st_cluster_f4(e + 32, make_float4(c.x, c.y, c.z, 0.0f));
-                mbar_arrive_remote(map_to_cta(&cs.fullBar[warp][h][slot], 1));
+                const XEventSlot ev = make_event(type, mid, a, b, c, erng);
+                const uint32_t e = map_to_cta(&cs.ring[warp][h][r.slot], 1);
+                st_cluster_f4(e, ev.q0);
+                st_cluster_f4(e + 16, ev.q1);
+                st_cluster_f4(e + 32, ev.q2);
+                mbar_arrive_remote(map_to_cta(&cs.fullBar[warp][h][r.slot], 1));
             }
-#pragma unroll
-            for (int hh = 0; hh < kCH; ++hh) if (hh == h) seq[hh] = sq + 1;
         };
         const V3 zero = v3(0, 0, 0);
         for (;;)
@@ -469,21 +459,20 @@ k_trace_exact_cluster(DrawParams p, const unsigned char* __restrict__ blob, Scen
             if (lane == 0) chainU = atomicAdd(p.workCounter, 1u);
             chainU = __shfl_sync(0xffffffffu, chainU, 0);
             if ((long long)chainU >= totalChains) break;
-            const int ri = (int)(chainU / (unsigned)p.numFrames), fi = (int)(chainU % (unsigned)p.numFrames);
-            const int y = p.row0 + ri * p.rowStep, frame = p.frame0 + fi;
+            const Chain ch = decode_chain(p, chainU);
 #pragma unroll
             for (int h = 0; h < kCH; ++h) emit_to(h, XE_BEGIN, (int)chainU, zero, zero, zero, 0u);
-            uint32_t rng = row_seed(y, frame);
+            uint32_t rng = row_seed(ch.y, ch.frame);
             unsigned rc = 0;
             uint32_t k = 0;
             for (int x = 0; x < p.width; ++x)
                 for (int s = 0; s < spp; ++s, ++k)
                 {
                     const int h = (int)(k % (uint32_t)kCH);
-                    xpath_sample(sc, p.cam, x, y, p.invWidth, p.invHeight, rng, rc, hitter,
+                    xpath_sample(sc, p.cam, x, ch.y, p.invWidth, p.invHeight, rng, rc, hitter,
                                  [&](int type, int mid, V3 a, V3 b, V3 c, uint32_t erng) { emit_to(h, type, mid, a, b, c, erng); });
                 }
-            if (lane == 0) atomicAdd(p.rayCounter + fi, (unsigned long long)rc);
+            if (lane == 0) atomicAdd(p.rayCounter + ch.fi, (unsigned long long)rc);
         }
 #pragma unroll
         for (int h = 0; h < kCH; ++h) emit_to(h, XE_QUIT, 0, zero, zero, zero, 0u);
@@ -492,113 +481,40 @@ k_trace_exact_cluster(DrawParams p, const unsigned char* __restrict__ blob, Scen
     {
         // ---- SHADE warp: serves path warp pw, samples k with k % kCH == h
         const int pw = warp / kCH, h = warp % kCH;
-        const int grp = lane >> 4;
-        GroupHitter<2, 16> hitter;
-        hitter.sub = lane & 15; hitter.mask = 0xffffu << (grp * 16);
+        const GroupHitter<2, 16> hitter = group_hitter<2, 16>(lane);
         const float invSpp = M<2>::div_(1.0f, (float)spp);
         uint32_t seq = 0, k = 0, pixBase = 0, chainsSeen = 0;
-        int ri = 0, fi = 0, y = 0, frame = 0;
-        float lerpFac = 0.0f, oneMinus = 1.0f;
-        size_t imgRow = 0;
+        Chain ch = {};
+        float lerpFac = 0.0f;
         XShade sh;
         xshade_begin(sh);
-
         auto lights = [&](int mid, V3 pos, V3 normal, V3 rdir, V3 albedo, uint32_t rng) -> V3 {
-            V3 lightE = v3(0, 0, 0);
-            int myJ = -1, kk = 0;
-            uint32_t myRng = 0;
-            auto run_batch = [&]() {
-                V3 contrib = v3(0, 0, 0);
-                bool reached = false;
-                if (myJ >= 0)
-                {
-                    const LightRec Lr = sc.lights[myJ];
-                    V3 l;
-                    sample_light<2>(Lr, pos, normal, rdir, albedo, myRng, l, contrib);
-                    float ts;
-                    reached = hitter.hit(sc, pos, l, TPT_MIN_T, TPT_MAX_T, ts) == Lr.id;
-                }
-                __syncwarp();
-#pragma unroll
-                for (int g = 0; g < 2; ++g)
-                {
-                    const bool r = __shfl_sync(0xffffffffu, reached ? 1 : 0, g * 16) != 0;
-                    const V3 cg = v3(__shfl_sync(0xffffffffu, contrib.x, g * 16), __shfl_sync(0xffffffffu, contrib.y, g * 16),
-                                     __shfl_sync(0xffffffffu, contrib.z, g * 16));
-                    if (r) lightE = lightE + cg;
-                }
-                myJ = -1;
-            };
-            for (int j = 0; j < sc.nLights; ++j)
-            {
-                if (sc.lights[j].id == mid) continue;
-                if ((kk & 1) == grp) { myJ = j; myRng = rng; }
-                XorShift32(rng); XorShift32(rng);
-                if ((++kk & 1) == 0) run_batch();
-            }
-            if (kk & 1) run_batch();
-            return lightE;
+            return shade_lights<2>(sc, hitter, lane >> 4, mid, pos, normal, rdir, albedo, rng);
         };
 
         for (;;)
         {
-            const uint32_t slot = seq % kRingDepth, phase = (seq / kRingDepth) & 1u;
-            mbar_wait_cluster(&cs.fullBar[pw][h][slot], phase);
-            const XEventSlot& e = cs.ring[pw][h][slot];
-            const float4 q0 = e.q0, q1 = e.q1, q2 = e.q2;
+            const RingPos r = ring_pos(seq++);
+            mbar_wait_sleep<true>(&cs.fullBar[pw][h][r.slot], r.phase);
+            const XEventSlot e = cs.ring[pw][h][r.slot];
             __syncwarp();
-            if (lane == 0) mbar_arrive_remote(map_to_cta(&cs.emptyBar[pw][h][slot], 0));
-            ++seq;
-            const int tm = __float_as_int(q0.w), type = tm & 7, mid = tm >> 3;
-            if (type == XE_QUIT) break;
-            if (type == XE_BEGIN)
+            if (lane == 0) mbar_arrive_remote(map_to_cta(&cs.emptyBar[pw][h][r.slot], 0));
+            if (e.type() == XE_QUIT) break;
+            if (e.type() == XE_BEGIN)
             {
                 pixBase = chainsSeen++ * (uint32_t)p.width;   // pixel slots are indexed by a running pixel number across chains
-                ri = mid / p.numFrames; fi = mid % p.numFrames;
-                y = p.row0 + ri * p.rowStep; frame = p.frame0 + fi;
-                lerpFac = lerp_fac(frame, p.flags); oneMinus = 1.0f - lerpFac;
-                imgRow = (size_t)(p.packed ? ri : y) * p.width;
+                ch = decode_chain(p, (unsigned)e.mid());
+                lerpFac = lerp_fac(ch.frame, p.flags);
                 k = (uint32_t)h;
                 xshade_begin(sh);
                 continue;
             }
             V3 result;
-            if (!xshade_event(sc, sh, type, mid, v3(q0.x, q0.y, q0.z), v3(q1.x, q1.y, q1.z), v3(q2.x, q2.y, q2.z),
-                              __float_as_uint(q1.w), lights, result)) continue;
+            if (!shade_event(sc, sh, e, lights, result)) continue;
             // sample k of the chain finished
             const int x = (int)(k / (uint32_t)spp), s = (int)(k - (uint32_t)x * (uint32_t)spp);
             const int ps = (int)((pixBase + (uint32_t)x) % (uint32_t)kPixSlots);
-            unsigned old = 0;
-            if (lane == 0)
-            {
-                cs.pixRes[pw][ps][s][0] = result.x; cs.pixRes[pw][ps][s][1] = result.y; cs.pixRes[pw][ps][s][2] = result.z;
-                __threadfence_block();
-                old = atomicInc(&cs.pixCnt[pw][ps], (unsigned)spp - 1u);
-            }
-            old = __shfl_sync(0xffffffffu, old, 0);
-            if (old == (unsigned)spp - 1u && lane == 0)
-            {
-                __threadfence_block();
-                V3 col = v3(0, 0, 0);
-                for (int t = 0; t < spp; ++t)
-                    col = col + v3(((volatile float*)cs.pixRes[pw][ps][t])[0], ((volatile float*)cs.pixRes[pw][ps][t])[1], ((volatile float*)cs.pixRes[pw][ps][t])[2]);
-                col = col * invSpp;
-                if (p.numFrames == 1)
-                {
-                    float4* px = reinterpret_cast<float4*>(p.image + (imgRow + x) * 4);
-                    float4 prev = *px;
-                    prev.x = prev.x * lerpFac + col.x * oneMinus;
-                    prev.y = prev.y * lerpFac + col.y * oneMinus;
-                    prev.z = prev.z * lerpFac + col.z * oneMinus;
-                    *px = prev;
-                }
-                else
-                {
-                    float4* px = reinterpret_cast<float4*>(p.scratch) + ((size_t)fi * p.numRows + ri) * p.width + x;
-                    *px = make_float4(col.x, col.y, col.z, 0.0f);
-                }
-            }
-            __syncwarp();
+            finish_sample(cs.pixRes[pw], cs.pixCnt[pw], ps, s, spp, invSpp, result, lane, p, ch, x, lerpFac);
             k += (uint32_t)kCH;
             xshade_begin(sh);
         }
@@ -608,48 +524,53 @@ k_trace_exact_cluster(DrawParams p, const unsigned char* __restrict__ blob, Scen
     cluster_sync_all();
 }
 
-static cudaError_t launch_exact_cluster(const DrawParams& p, const SceneDev& sc, cudaStream_t stream)
+// Allows `dyn` bytes of dynamic shared memory for one of the trace kernels and launches it.
+template <class Kernel>
+static cudaError_t launch_chains(Kernel kern, long long grid, int block, size_t dyn, const DrawParams& p, const SceneDev& sc,
+                                 cudaStream_t stream)
 {
-    // one CTA per SM: ask for more than half of an SM's shared memory
-    const size_t wantDyn = 118 * 1024;
-    const size_t dyn = sc.stagedBytes > wantDyn ? sc.stagedBytes : wantDyn;
-    cudaError_t e = cudaFuncSetAttribute(k_trace_exact_cluster, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
     if (e != cudaSuccess) return e;
-    e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
-    if (e != cudaSuccess) return e;
-    const long long totalChains = (long long)p.numRows * p.numFrames;
-    int dev = 0, numSMs = 132;
-    cudaGetDevice(&dev);
-    cudaDeviceGetAttribute(&numSMs, cudaDevAttrMultiProcessorCount, dev);
-    long long clusters = numSMs / 2;
-    const long long need = (totalChains + kCPathWarps - 1) / kCPathWarps;
-    if (clusters > need) clusters = need;
-    k_trace_exact_cluster<<<(unsigned)(2 * clusters), kCThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
+    kern<<<(unsigned)grid, block, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
     return cudaGetLastError();
 }
 
+static cudaError_t launch_exact_cluster(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
+{
+    const long long totalChains = (long long)p.numRows * p.numFrames;
+    if (p.spp > kSplitMaxSpp || totalChains >= (1LL << 27)) return cudaErrorInvalidValue;   // the chain index travels in a tag
+    cudaError_t e = cudaMemsetAsync(p.workCounter, 0, sizeof(unsigned int), stream);
+    if (e != cudaSuccess) return e;
+    long long clusters = numSMs / 2;
+    const long long need = (totalChains + kCPathWarps - 1) / kCPathWarps;
+    if (clusters > need) clusters = need;
+    // one CTA per SM: ask for more than half of an SM's shared memory
+    const size_t wantDyn = 118 * 1024;
+    const size_t dyn = sc.stagedBytes > wantDyn ? sc.stagedBytes : wantDyn;
+    return launch_chains(k_trace_exact_cluster, 2 * clusters, kCThreads, dyn, p, sc, stream);
+}
+
+// one CTA per chain; a pixel slot holds at most kSplitMaxSpp samples
 template <int H, int DRY = 0, int SMODE = 1>
 static cudaError_t launch_exact_split_t(const DrawParams& p, const SceneDev& sc, cudaStream_t stream)
 {
     const long long totalChains = (long long)p.numRows * p.numFrames;
-    auto kern = k_trace_exact_split<H, DRY, SMODE>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
-    if (e != cudaSuccess) return e;
-    kern<<<(unsigned)totalChains, split_block_threads(H), sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
-    return cudaGetLastError();
+    if (p.spp > kSplitMaxSpp || totalChains > 0x7fffffffLL) return cudaErrorInvalidValue;
+    return launch_chains(k_trace_exact_split<H, DRY, SMODE>, totalChains, split_block_threads(H), sc.stagedBytes, p, sc, stream);
 }
 
 template <int LANES>
-static cudaError_t launch_exact_t(const DrawParams& p, const SceneDev& sc, cudaStream_t stream, int blockThreads)
+static cudaError_t launch_exact_t(const DrawParams& p, const SceneDev& sc, cudaStream_t stream, int block)
 {
-    const long long totalChains = (long long)p.numRows * p.numFrames;
-    const long long threads = totalChains * LANES;
-    const int grid = (int)((threads + blockThreads - 1) / blockThreads);
-    auto kern = k_trace_exact<LANES>;
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
-    if (e != cudaSuccess) return e;
-    kern<<<grid, blockThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
-    return cudaGetLastError();
+    const long long threads = (long long)p.numRows * p.numFrames * LANES;
+    return launch_chains(k_trace_exact<LANES>, (threads + block - 1) / block, block, sc.stagedBytes, p, sc, stream);
+}
+
+template <int LANES>
+static cudaError_t launch_exact_flat_t(const DrawParams& p, const SceneDev& sc, cudaStream_t stream)
+{
+    const long long threads = (long long)p.numRows * p.numFrames * LANES;
+    return launch_chains(k_trace_exact_flat<LANES>, (threads + 127) / 128, 128, sc.stagedBytes, p, sc, stream);
 }
 
 __global__ void k_debug_libm(int fn, const float* __restrict__ in, float* __restrict__ out, long long n)
@@ -678,7 +599,7 @@ cudaError_t launch_resolve_exact(const DrawParams& p, cudaStream_t stream)
     return cudaGetLastError();
 }
 
-cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, cudaStream_t stream, bool resolve)
+cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, int numSMs, cudaStream_t stream, bool resolve)
 {
     const long long totalChains = (long long)p.numRows * p.numFrames;
     if (lanes <= 0)
@@ -687,9 +608,10 @@ cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, cud
         // chain, then 8; from ~100k chains one lane per chain in the flat form fills the GPU on its own
         lanes = totalChains >= 100000 ? 1 : (totalChains >= 20000 ? 8 : (totalChains <= 2400 && p.spp <= kSplitMaxSpp ? 65 : 32));
     }
-    cudaError_t e;
+    // nested form: smaller CTAs when there are few chains, so that they still spread over all SMs
     const long long threads = totalChains * lanes;
-    const int block = threads >= 132LL * 256 ? 128 : (threads >= 132LL * 64 ? 64 : 32);   // H100: 132 SMs
+    const int block = threads >= numSMs * 256LL ? 128 : (threads >= numSMs * 64LL ? 64 : 32);
+    cudaError_t e;
     switch (lanes)
     {
     case 1: e = launch_exact_flat_t<1>(p, sc, stream); break;
@@ -698,18 +620,15 @@ cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, cud
     case 9: e = launch_exact_flat_t<8>(p, sc, stream); break;        // flat form with 8 lanes per chain: measured 2x SLOWER than
                                                                      // the nested form at 11 520 chains (221 vs 111 ms), comparison only
     case 32: e = launch_exact_t<32>(p, sc, stream, block); break;
+    // split kernel: path warp + 1..4 shade warps per chain
+    case 64: e = launch_exact_split_t<1>(p, sc, stream); break;
+    case 65: e = launch_exact_split_t<2>(p, sc, stream); break;
+    case 66: e = launch_exact_split_t<3>(p, sc, stream); break;
+    case 67: e = launch_exact_split_t<4>(p, sc, stream); break;
+    case 68: e = launch_exact_split_t<2, 2>(p, sc, stream); break;  // 68 / 69: timing probes (no light sampling / path warp
+    case 69: e = launch_exact_split_t<2, 1>(p, sc, stream); break;  // alone); the image is NOT valid
+    case 70: e = launch_exact_cluster(p, sc, numSMs, stream); break; // split kernel, roles on different SMs (2-CTA clusters)
     case 71: e = launch_exact_split_t<2, 0, 2>(p, sc, stream); break;   // comparison: shade warps calling shared out-of-line sqrt/div/libm
-    case 70:                                                         // split kernel, roles on different SMs (2-CTA clusters)
-        if (p.spp > kSplitMaxSpp || totalChains >= (1LL << 27)) return cudaErrorInvalidValue;
-        e = launch_exact_cluster(p, sc, stream);
-        break;
-    case 64: case 65: case 66: case 67: case 68: case 69:            // split kernel: path warp + 1..4 shade warps per chain
-        if (p.spp > kSplitMaxSpp || totalChains > 0x7fffffffLL) return cudaErrorInvalidValue;
-        e = lanes == 64 ? launch_exact_split_t<1>(p, sc, stream) : lanes == 65 ? launch_exact_split_t<2>(p, sc, stream)
-          : lanes == 66 ? launch_exact_split_t<3>(p, sc, stream) : lanes == 67 ? launch_exact_split_t<4>(p, sc, stream)
-          : lanes == 68 ? launch_exact_split_t<2, 2>(p, sc, stream)  // 68 / 69: timing probes (no light sampling / path warp
-          : launch_exact_split_t<2, 1>(p, sc, stream);               // alone); the image is NOT valid
-        break;
     default: return cudaErrorInvalidValue;
     }
     if (e != cudaSuccess) return e;

@@ -16,9 +16,9 @@ struct SceneDev
                                  // then rounds no worse than the reference form (see FastHitterK)
 };
 
-// lanes: 0 = choose from the number of (frame,row) chains; 1, 8 or 32 to force.
+// lanes: 0 = choose from the number of (frame,row) chains; 1, 2, 8, 9, 32 or 64..71 to force (see tpt_exact.cu).
 // resolve = false: with numFrames > 1 only the per-frame colours are written to p.scratch (no blend into the image)
-cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, cudaStream_t stream, bool resolve = true);
+cudaError_t launch_exact(const DrawParams& p, const SceneDev& sc, int lanes, int numSMs, cudaStream_t stream, bool resolve = true);
 // the reference's progressive blend (Test.cpp:272-276,293-295) of p.numFrames frames of per-frame colours in p.scratch
 cudaError_t launch_resolve_exact(const DrawParams& p, cudaStream_t stream);
 cudaError_t launch_debug_libm(int fn, const float* dIn, float* dOut, long long n, cudaStream_t stream);
