@@ -321,8 +321,8 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
     // The gate |s|^2 <= 128 + 2 r^2 keeps (|s| + |o|)^2 within a small multiple of max(r^2, 128) for origins inside the
     // scene's extent (|o|^2 <= 128), i.e. the expanded form is no worse than ~8x the reference form's own bound for small
     // spheres and BETTER than it for huge ones (ground sphere r = 100: 2 s.o ~ 400 vs |co|^2 ~ 10^4). The bound is not
-    // what the parity claim rests on: tests/test_gpu_fast.py compares kform 0 and 1 against the bit-exact mode at
-    // >= 16k spp, overall and per first-hit material.
+    // what the parity claim rests on: tests/test_gpu_configs.py and tests/test_gpu_light_sampling.py compare kform 0
+    // and 1 against the bit-exact mode at >= 16k spp, overall and per first-hit material.
     ctx->scene.kformOk = true;
     for (int i = 0; i < count; ++i)
     {
