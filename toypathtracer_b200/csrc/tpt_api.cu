@@ -444,7 +444,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     const bool waveFits = (long long)((numRows * (long long)width + 127) / 128) * 128 * ctx->spp * (numFrames < 256 ? numFrames : 256) <= 0x7fffffffLL;
     SceneDev autoScene = ctx->scene;
     autoScene.kformMode = ctx->fastKForm;
-    int fastVariant = ctx->fastVariant < 0 ? (ctx->scene.count >= 1024 && waveFits && fast_queue_kform(autoScene) < 2 ? 7 : 3) : ctx->fastVariant;
+    // (the wavefront keeps 1 + the light index in 16 bits: scenes with 65 535 or more lights stay on the slab queue)
+    int fastVariant = ctx->fastVariant < 0 ? (ctx->scene.count >= 1024 && waveFits && fast_queue_kform(autoScene) < 2 &&
+                                              ctx->scene.nLights < 0xffff ? 7 : 3) : ctx->fastVariant;
     if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && (ctx->fastVariant < 0 || fast_variant_writes_final_pixels(ctx->fastVariant)))
     {
         // Host-buffer draw whose `prev` has zero weight, into page-locked memory the GPU can address: the trace kernel's

@@ -1399,7 +1399,9 @@ constexpr int kWaveFields = 11;
 constexpr int kWaveChunk = 4096;       // paths taken from the global counter at a time
 enum { WF_O = 0, WF_D, WF_THR, WF_COL, WF_NEXT, WF_THRALB, WF_NL, WF_ALB, WF_PEND, WF_POS, WF_NRM };
 enum { WT_MISS = 0, WT_LAMBERT, WT_METAL, WT_DIEL, WT_SHADOW, WT_TERMINAL, WT_COUNT };
-constexpr int kKindFree = 255;
+// a slot's state word (WF_D.w): bits 0-15 kind (0 path ray, 1 + j shadow ray of light j, kKindFree), bits 16-23 depth,
+// bit 24 doMaterialE. The launcher refuses nLights >= kKindFree.
+constexpr int kKindFree = 0xffff;
 
 struct WaveArgs
 {
@@ -1458,7 +1460,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         // ---- phase 1: regenerate own slot if free, then sweep
         float4 fd = WFLD(WF_D, tid);
         int misc = __float_as_int(fd.w);
-        int kind = misc & 0xff;
+        int kind = misc & 0xffff;
         {
             const unsigned need = __ballot_sync(0xffffffffu, kind == kKindFree);
             if (need)
@@ -1482,7 +1484,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                         float u = ((float)x + RandomFloat01(rng)) * p.invWidth;
                         float v = ((float)y + RandomFloat01(rng)) * p.invHeight;
                         Ray r = fast_get_ray(p.cam, u, v, rng);
-                        kind = 0; misc = 0 | (0 << 8) | (1 << 16);
+                        kind = 0; misc = 0 | (0 << 16) | (1 << 24);
                         fd = make_float4(r.dir.x, r.dir.y, r.dir.z, __int_as_float(misc));
                         WFLD(WF_O, tid) = make_float4(r.orig.x, r.orig.y, r.orig.z, 0.0f);
                         WFLD(WF_D, tid) = fd;
@@ -1509,7 +1511,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                 const V3 pos = o + d * t;
                 const V3 normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];
                 const int mid = id < sc.count ? id : sc.count;
-                const int depth = (misc >> 8) & 0xff;
+                const int depth = (misc >> 16) & 0xff;
                 const int mtype = f_as_i(sc.matA[mid].w);
                 type = depth >= TPT_MAX_DEPTH ? WT_TERMINAL : (mtype == kLambert ? WT_LAMBERT : (mtype == kMetal ? WT_METAL : WT_DIEL));
                 WFLD(WF_POS, tid) = make_float4(pos.x, pos.y, pos.z, __int_as_float(mid));
@@ -1555,11 +1557,11 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                     V3 col = v3(fcol.x, fcol.y, fcol.z), thr = v3(fthr.x, fthr.y, fthr.z);
                     uint32_t rng = __float_as_uint(fthr.w);
                     const V3 d = v3(fdd.x, fdd.y, fdd.z);
-                    const bool doMatE = (m2 >> 16) & 1;
+                    const bool doMatE = (m2 >> 24) & 1;
                     if (T == WT_MISS) { col = col + thr * sky(d, sc); finished = true; }
                     else if (T == WT_SHADOW)
                     {
-                        const int j = (m2 & 0xff) - 1;
+                        const int j = (m2 & 0xffff) - 1;
                         const int hid = __float_as_int(WFLD(WF_POS, slot).w);
                         if (hid == sc.lights[j].id) { const float4 pe = WFLD(WF_PEND, slot); col = col + v3(pe.x, pe.y, pe.z); }
                         wantLight = true;   // next light index = j + 1, kept in kind
@@ -1583,7 +1585,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                             WFLD(WF_NL, slot) = make_float4(nl.x, nl.y, nl.z, 0.0f);
                             WFLD(WF_ALB, slot) = make_float4(mat.albedo.x, mat.albedo.y, mat.albedo.z, 0.0f);
                             WFLD(WF_O, slot) = make_float4(pos.x, pos.y, pos.z, 0.0f);
-                            m2 = (m2 & ~0xff) | 0;      // kind := "before light 0" (light phase advances it)
+                            m2 = (m2 & ~0xffff) | 0;    // kind := "before light 0" (light phase advances it)
                             wantLight = true;
                         }
                         else
@@ -1604,8 +1606,8 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                             {
                                 if (doMatE) col = col + thr * mat.emissive;
                                 thr = thr * att;
-                                const int depth = ((m2 >> 8) & 0xff) + 1;
-                                m2 = 0 | (depth << 8) | (1 << 16);
+                                const int depth = ((m2 >> 16) & 0xff) + 1;
+                                m2 = 0 | (depth << 16) | (1 << 24);
                                 WFLD(WF_O, slot) = make_float4(pos.x, pos.y, pos.z, 0.0f);
                                 fdd = make_float4(outDir.x, outDir.y, outDir.z, 0.0f);
                             }
@@ -1647,7 +1649,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                     int m2 = __float_as_int(fdd.w);
                     const float4 fta = WFLD(WF_THRALB, slot);
                     const int mid = __float_as_int(fta.w);
-                    int j = m2 & 0xff;                 // kind k = shadow ray of light k-1 just returned -> next is light k
+                    int j = m2 & 0xffff;               // kind k = shadow ray of light k-1 just returned -> next is light k
                     while (j < sc.nLights && sc.lights[j].id == mid) ++j;
                     if (j < sc.nLights)
                     {
@@ -1676,16 +1678,16 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                         WFLD(WF_PEND, slot) = make_float4(pend.x, pend.y, pend.z, 0.0f);
                         fthr.w = __uint_as_float(rng);
                         WFLD(WF_THR, slot) = fthr;
-                        m2 = (m2 & ~0xff) | (1 + j);
+                        m2 = (m2 & ~0xffff) | (1 + j);
                         WFLD(WF_D, slot) = make_float4(l.x, l.y, l.z, __int_as_float(m2));
                     }
                     else
                     {
                         const float4 fnx = WFLD(WF_NEXT, slot);
                         float4 fthr = WFLD(WF_THR, slot);
-                        const int depth = ((m2 >> 8) & 0xff) + 1;
+                        const int depth = ((m2 >> 16) & 0xff) + 1;
                         // doMaterialE = false after a Lambert vertex (Test.cpp:214), unless light sampling is off
-                        m2 = 0 | (depth << 8) | ((emission_after_lambert(sc) ? 1 : 0) << 16);
+                        m2 = 0 | (depth << 16) | ((emission_after_lambert(sc) ? 1 : 0) << 24);
                         WFLD(WF_D, slot) = make_float4(fnx.x, fnx.y, fnx.z, __int_as_float(m2));
                         WFLD(WF_THR, slot) = make_float4(fta.x, fta.y, fta.z, fthr.w);
                     }
@@ -1928,6 +1930,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
     }
     if (variant == 6 || variant == 7)
     {
+        if (sc.nLights >= kKindFree) return cudaErrorInvalidValue;     // 1 + light index must stay below the free marker
         auto kern = variant == 6 ? k_fast_wave<3> : k_fast_wave<4>;
         const FastSmem lay = fast_smem(sc.stagedBytes, 0, kWaveFields * kWaveSlots * 16);
         const long long total = ((regionPix + 127) / 128) * 128 * S;      // whole 128-pixel slabs; tail pixels are skipped
