@@ -127,6 +127,32 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
              float* backbuffer, int bufferOnDevice, unsigned testFlags, int mode,
              long long* outRayCount, long long* outRaysPerFrame, void* cudaStream);
 
+/* Fast-mode radiance estimates for n caller-supplied rays in the current scene — other projections (panoramas, fisheye,
+ * orthographic, stereo), many small views in one launch, a sparse set of pixels, or rays made by torch code.
+ *   rays6             n rays of 6 floats {o.xyz, d.xyz} (the layout of tpt_debug_hit); directions need not be unit length,
+ *                     they are normalised on load. A device buffer may have any 4-byte alignment (a row slice of an
+ *                     (N, 6) tensor is only 8-byte aligned).
+ *   out4              n float4: out4[i] = (r, g, b, 0), the mean over `spp` samples of ray i's path radiance with the
+ *                     estimator of TPT_MODE_FAST (scene options as for a fast draw: "light_sampling", "mitsuba_compare",
+ *                     "fast_kform", scenes past 64 KB of blob). A device buffer must be 16-byte aligned. A ray with a
+ *                     non-finite component, or whose direction does not normalise to a finite non-zero vector (zero
+ *                     length, or a squared length that underflows or overflows float), is not traced: (0, 0, 0, 0).
+ *   raysOnDevice / outOnDevice
+ *                     0: host pointer, copied in / out inside the call, and the call is synchronous
+ *                     1: device pointer of the context's device (or mapped host memory), used in place on `cudaStream`;
+ *                        without host buffers the host only synchronises when a ray count is requested
+ *   spp, frame        sample s of ray i draws from the stream pixel_seed(i * spp + s, frame) of the fast mode: the same
+ *                     frame gives the same result, different frames independent ones, so averaging calls with frames
+ *                     0, 1, 2, ... refines the estimates progressively. n * spp must not exceed 2^32.
+ *   outRayCount       NULL or receives the number of rays traced (path and shadow rays; untraced rays add none).
+ *   cudaStream        a cudaStream_t (NULL = the context's own stream).
+ * n == 0 launches nothing and reports 0 rays. The draw's blend and `prev` play no part. Ordering and accounting are those
+ * of tpt_draw: the call runs after the context's previous draw (or trace) and after the scene upload, and counts toward
+ * tpt_read_ray_count, tpt_last_kernel_ms and tpt_last_launch_count. Null pointers, n < 0, spp < 1, n * spp > 2^32, a
+ * misaligned device buffer or one on another device are refused (tpt_last_error gives the reason). */
+int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
+                   float* out4, int outOnDevice, long long* outRayCount, void* cudaStream);
+
 /* Rays traced by all draws since the last call of this function (synchronises the stream). */
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStream, long long* outRays);
 /* Device time (CUDA events on the launching stream) of the kernels of the most recent tpt_draw, in ms. */

@@ -75,6 +75,7 @@ def _load_lib():
     L.tpt_tonemap_rgba8.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci, ci, ci, vp]; L.tpt_tonemap_rgba8.restype = ci
     L.tpt_debug_libm.argtypes = [vp, ci, vp, vp, cll]; L.tpt_debug_libm.restype = ci
     L.tpt_debug_hit.argtypes = [vp, ci, vp, vp, vp, cll]; L.tpt_debug_hit.restype = ci
+    L.tpt_trace_rays.argtypes = [vp, vp, ci, cll, ci, ci, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_rays.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -185,6 +186,39 @@ class Context:
         if per_frame:
             return int(total.value), [int(v) for v in pf]
         return int(total.value) if want_rays else None
+
+    def trace_rays(self, rays, spp: int = 4, frame: int = 0, out=None, stream: int = 0, want_rays: bool = True, n=None):
+        """tpt_trace_rays: fast-mode radiance estimates (mean of `spp` samples, streams keyed by `frame`) for caller rays
+        {o.xyz, d.xyz}. `rays` is an (N, 6) float32 numpy array, a torch tensor (CPU or CUDA; a row slice is fine) or a
+        DevicePtr together with `n`. Without `out` the result is a new (N, 4) array of the same kind as `rays` (numpy, CPU or
+        CUDA tensor; a DevicePtr gets a CUDA tensor); `out` may be any buffer of N float4. Returns (out, rays traced), or
+        out alone when want_rays is False (device buffers then stay asynchronous on `stream`)."""
+        if isinstance(rays, DevicePtr):
+            if n is None:
+                raise TptError("trace_rays: a DevicePtr needs n")
+            raddr, ron, keep = rays.addr, True, rays
+        else:
+            if tuple(rays.shape[1:]) != (6,) or len(rays.shape) != 2:
+                raise TptError("trace_rays: rays must have shape (N, 6)")
+            if n is not None and int(n) != rays.shape[0]:
+                raise TptError("trace_rays: n does not match rays")
+            n = rays.shape[0]
+            raddr, ron, keep = _as_ptr(rays)
+        n = int(n)
+        if out is None:
+            if isinstance(rays, np.ndarray):
+                out = np.empty((n, 4), np.float32)
+            else:
+                import torch
+                dev = rays.device if hasattr(rays, "device") else torch.device("cuda", self.device)
+                out = torch.empty((n, 4), dtype=torch.float32, device=dev)
+        oaddr, oon, keep_out = _as_ptr(out)
+        total = ctypes.c_longlong(0)
+        rc = self._L.tpt_trace_rays(self._h, ctypes.c_void_p(raddr), 1 if ron else 0, n, int(spp), int(frame),
+                                    ctypes.c_void_p(oaddr), 1 if oon else 0, ctypes.byref(total) if want_rays else None,
+                                    ctypes.c_void_p(stream) if stream else None)
+        self._check(rc, "tpt_trace_rays")
+        return (out, int(total.value)) if want_rays else out
 
     def read_ray_count(self, stream: int = 0) -> int:
         out = ctypes.c_longlong(0)
@@ -357,4 +391,4 @@ def set_mode(mode: int):
     _load_shim().tpt_shim_set_mode(mode)
 
 
-from .scenes import reference_scene, stress_scene, make_camera  # noqa: E402,F401
+from .scenes import reference_scene, stress_scene, make_camera, camera_rays  # noqa: E402,F401

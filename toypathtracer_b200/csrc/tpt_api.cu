@@ -74,7 +74,8 @@ struct tpt_context
     size_t maxScratchBytes = (size_t)8 << 30;
 
     // buffers
-    float* dImage = nullptr; size_t imageCap = 0;      // staging image for host-pointer draws
+    float* dImage = nullptr; size_t imageCap = 0;      // staging image for host-pointer draws (and host tpt_trace_rays outputs)
+    float* dRays = nullptr; size_t raysCap = 0;        // staging of host tpt_trace_rays inputs
     float* dScratch = nullptr; size_t scratchCap = 0;  // exact mode per-frame colours
     unsigned long long* dRayCounters = nullptr; int rayCounterCap = 0;   // [numFrames]
     unsigned long long* dAccum = nullptr;              // [0] total since last read, [1] last draw total
@@ -226,7 +227,7 @@ void tpt_destroy(tpt_context* ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->registeredPtr) cudaHostUnregister(ctx->registeredPtr);
-    cudaFree(ctx->dImage); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
+    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
     cudaFree(ctx->dAccum); cudaFree(ctx->dWork);
     for (int i = 0; i < 2; ++i)
     {
@@ -391,6 +392,79 @@ static int ensure(tpt_context* ctx, void** p, size_t* cap, size_t bytes, const c
     return 0;
 }
 
+// Prologue of a call that traces (tpt_draw, tpt_trace_rays). One context = one scene blob, one set of counters: calls are
+// ordered in issue order even across streams, and the scene they read must have landed (tpt_set_scene uploads
+// asynchronously on its own stream). Returns the call's stream and the scene with the context's sweep-form option applied.
+static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* stream, SceneDev* scene)
+{
+    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+    *stream = cudaStreamArg ? (cudaStream_t)cudaStreamArg : ctx->stream;
+    if (ctx->haveLastDraw && ctx->lastDrawStream != *stream) CK(cudaStreamWaitEvent(*stream, ctx->lastDraw, 0), "order after previous draw");
+    CK(cudaStreamWaitEvent(*stream, ctx->uploadDone[ctx->curBlob], 0), "wait for scene upload");
+    *scene = ctx->scene;
+    scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
+    scene->kformMode = ctx->fastKForm;
+    return 0;
+}
+
+// Zeroes the call's `n` ray counters (one per frame) and starts its kernel timing.
+static int start_kernels(tpt_context* ctx, cudaStream_t stream, int n)
+{
+    if (n > ctx->rayCounterCap)
+    {
+        CK(cudaStreamSynchronize(stream), "sync before counter realloc");
+        cudaFree(ctx->dRayCounters); ctx->dRayCounters = nullptr; ctx->rayCounterCap = 0;
+        CK(cudaMalloc(&ctx->dRayCounters, (size_t)n * sizeof(unsigned long long)), "cudaMalloc counters");
+        ctx->rayCounterCap = n;
+    }
+    CK(cudaMemsetAsync(ctx->dRayCounters, 0, (size_t)n * sizeof(unsigned long long), stream), "zero counters");
+    ctx->lastLaunches = 0;
+    CK(cudaEventRecord(ctx->evStart, stream), "event record");
+    return 0;
+}
+
+// Ends the kernel timing and folds the call's `n` ray counters into the running totals (tpt_read_ray_count) and, when
+// the caller wants the counts, into page-locked memory that finish_call reads.
+static int finish_kernels(tpt_context* ctx, cudaStream_t stream, int n, bool wantCounts)
+{
+    CK(cudaEventRecord(ctx->evStop, stream), "event record");
+    ctx->haveTiming = true;
+    if (wantCounts && n > ctx->hPinnedCap)
+    {
+        if (ctx->hPinned) cudaFreeHost(ctx->hPinned);
+        ctx->hPinned = nullptr; ctx->hPinnedCap = 0;
+        CK(cudaMallocHost(&ctx->hPinned, (size_t)n * sizeof(unsigned long long)), "cudaMallocHost");
+        ctx->hPinnedCap = n;
+    }
+    k_accumulate_rays<<<1, 1, 0, stream>>>(ctx->dRayCounters, n, ctx->dAccum, wantCounts ? ctx->hPinned : nullptr);
+    CK(cudaGetLastError(), "accumulate launch");
+    ctx->lastLaunches += 1;
+    return 0;
+}
+
+// Epilogue after the call's last copy: the next call orders after this one and the next scene upload into this blob slot
+// after it. The host synchronises only to read the counts back, or because the call had host buffers (synchronous then).
+static int finish_call(tpt_context* ctx, cudaStream_t stream, int n, bool hostBuffers, long long* outRayCount, long long* outPerFrame)
+{
+    CK(cudaEventRecord(ctx->lastDraw, stream), "draw end event");
+    CK(cudaEventRecord(ctx->blobLastUse[ctx->curBlob], stream), "scene last-use event");
+    ctx->lastDrawStream = stream; ctx->haveLastDraw = true;
+    if (outRayCount || outPerFrame)
+    {
+        CK(cudaStreamSynchronize(stream), "stream sync");     // the counts were stored into hPinned by k_accumulate_rays
+        long long total = 0;
+        for (int i = 0; i < n; ++i)
+        {
+            total += (long long)ctx->hPinned[i];
+            if (outPerFrame) outPerFrame[i] = (long long)ctx->hPinned[i];
+        }
+        if (outRayCount) *outRayCount = total;
+    }
+    else if (hostBuffers)
+        CK(cudaStreamSynchronize(stream), "stream sync");
+    return 0;
+}
+
 int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
              int row0, int numRows, int rowStep, int packed,
              float* backbuffer, int bufferOnDevice, unsigned testFlags, int mode,
@@ -412,15 +486,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         return 0;
     }
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
-    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
-    cudaStream_t stream = cudaStreamArg ? (cudaStream_t)cudaStreamArg : ctx->stream;
-    // One context = one scene blob, one set of counters: draws are ordered in issue order even across streams, and the
-    // scene this draw reads must have landed (tpt_set_scene uploads asynchronously on its own stream).
-    if (ctx->haveLastDraw && ctx->lastDrawStream != stream) CK(cudaStreamWaitEvent(stream, ctx->lastDraw, 0), "order after previous draw");
-    CK(cudaStreamWaitEvent(stream, ctx->uploadDone[ctx->curBlob], 0), "wait for scene upload");
-    SceneDev scene = ctx->scene;
-    scene.kformOk = scene.kformOk && ctx->fastKForm != 0;
-    scene.kformMode = ctx->fastKForm;
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
 
     const size_t bufRows = packed ? (size_t)numRows : (size_t)height;
     const size_t bufBytes = bufRows * width * 4 * sizeof(float);
@@ -492,16 +560,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     }
     if (mode == TPT_MODE_FAST && framesPerLaunch > 256) framesPerLaunch = 256;
 
-
-    if (numFrames > ctx->rayCounterCap)
-    {
-        CK(cudaStreamSynchronize(stream), "sync before counter realloc");
-        cudaFree(ctx->dRayCounters); ctx->dRayCounters = nullptr; ctx->rayCounterCap = 0;
-        CK(cudaMalloc(&ctx->dRayCounters, (size_t)numFrames * sizeof(unsigned long long)), "cudaMalloc counters");
-        ctx->rayCounterCap = numFrames;
-    }
-    CK(cudaMemsetAsync(ctx->dRayCounters, 0, (size_t)numFrames * sizeof(unsigned long long), stream), "zero counters");
-
+    if (int r = start_kernels(ctx, stream, numFrames)) return r;
     DrawParams p;
     memset(&p, 0, sizeof(p));
     p.cam = ctx->cam;
@@ -517,8 +576,6 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     // that is in the buffer, unless the staging image was not uploaded (host buffer) or the caller waived it.
     p.zeroAlpha = (ctx->fastAlphaZero || (!bufferOnDevice && !needPrev)) ? 1 : 0;     // (zero-copy: never reads host memory)
 
-    ctx->lastLaunches = 0;
-    CK(cudaEventRecord(ctx->evStart, stream), "event record");
     // Host-buffer fast draws: split the rows into bands, one stream per band (earlier band = higher priority). Each
     // stream runs prepare + trace for its band and then copies the band to the caller's buffer, so the D2H of band b
     // overlaps the tracing of band b+1 and the persistent CTAs of band b+1 fill the SMs as band b's tail drains.
@@ -656,19 +713,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         }
         if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     }
-    CK(cudaEventRecord(ctx->evStop, stream), "event record");
-    ctx->haveTiming = true;
-    const bool wantCounts = outRayCount || outRaysPerFrame;
-    if (wantCounts && numFrames > ctx->hPinnedCap)
-    {
-        if (ctx->hPinned) cudaFreeHost(ctx->hPinned);
-        ctx->hPinned = nullptr; ctx->hPinnedCap = 0;
-        CK(cudaMallocHost(&ctx->hPinned, (size_t)numFrames * sizeof(unsigned long long)), "cudaMallocHost");
-        ctx->hPinnedCap = numFrames;
-    }
-    k_accumulate_rays<<<1, 1, 0, stream>>>(ctx->dRayCounters, numFrames, ctx->dAccum, wantCounts ? ctx->hPinned : nullptr);
-    CK(cudaGetLastError(), "accumulate launch");
-    ctx->lastLaunches += 1;
+    if (int r = finish_kernels(ctx, stream, numFrames, outRayCount || outRaysPerFrame)) return r;
 
     if (!bufferOnDevice && !pipelined && !zeroCopy)
     {
@@ -677,24 +722,81 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         cudaError_t e = copy_rows(backbuffer, dImage, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream);
         if (e != cudaSuccess) return fail(ctx, e, "D2H backbuffer");
     }
-    CK(cudaEventRecord(ctx->lastDraw, stream), "draw end event");
-    CK(cudaEventRecord(ctx->blobLastUse[ctx->curBlob], stream), "scene last-use event");
-    ctx->lastDrawStream = stream; ctx->haveLastDraw = true;
+    // host-buffer draws are synchronous like DrawTest
+    return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
+}
 
-    if (outRayCount || outRaysPerFrame)
+// A device buffer of tpt_trace_rays must be addressable by the context's device: its own memory, or mapped host memory.
+static int check_device_buffer(tpt_context* ctx, const void* ptr, const char* name)
+{
+    cudaPointerAttributes attr;
+    char msg[160];
+    if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess || attr.type == cudaMemoryTypeUnregistered)
     {
-        CK(cudaStreamSynchronize(stream), "stream sync");     // the counts were stored into hPinned by k_accumulate_rays
-        long long total = 0;
-        for (int i = 0; i < numFrames; ++i)
-        {
-            total += (long long)ctx->hPinned[i];
-            if (outRaysPerFrame) outRaysPerFrame[i] = (long long)ctx->hPinned[i];
-        }
-        if (outRayCount) *outRayCount = total;
+        (void)cudaGetLastError();
+        snprintf(msg, sizeof(msg), "tpt_trace_rays: device %s is not CUDA memory", name);
+        return fail_msg(ctx, msg);
     }
-    else if (!bufferOnDevice)
-        CK(cudaStreamSynchronize(stream), "stream sync"); // host-buffer draws are synchronous like DrawTest
+    if ((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device != ctx->device)
+    {
+        snprintf(msg, sizeof(msg), "tpt_trace_rays: device %s lives on device %d, the context on device %d", name, attr.device, ctx->device);
+        return fail_msg(ctx, msg);
+    }
     return 0;
+}
+
+int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
+                   float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!ctx->haveScene) return fail_msg(ctx, "tpt_trace_rays: no scene (call tpt_set_scene first)");
+    if (!rays6 || !out4) return fail_msg(ctx, "tpt_trace_rays: null rays6 or out4");
+    if (n < 0) return fail_msg(ctx, "tpt_trace_rays: n < 0");
+    if (spp < 1) return fail_msg(ctx, "tpt_trace_rays: spp < 1");
+    // the sample stream of (ray i, sample s) is i * spp + s in 32 bits, and so is the ray index
+    if (n > (1LL << 32) / spp || n > 0xffffffffLL) return fail_msg(ctx, "tpt_trace_rays: n * spp > 2^32 (32-bit sample streams)");
+    if (raysOnDevice && ((uintptr_t)rays6 & 3)) return fail_msg(ctx, "tpt_trace_rays: device rays6 is not 4-byte aligned");
+    if (outOnDevice && ((uintptr_t)out4 & 15)) return fail_msg(ctx, "tpt_trace_rays: device out4 is not 16-byte aligned");
+    if (raysOnDevice) { if (int r = check_device_buffer(ctx, rays6, "rays6")) return r; }
+    if (outOnDevice) { if (int r = check_device_buffer(ctx, out4, "out4")) return r; }
+    if (n == 0)
+    {
+        if (outRayCount) *outRayCount = 0;
+        ctx->lastLaunches = 0;
+        return 0;
+    }
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+    const float* dRays = rays6;
+    float* dOut = out4;
+    if (!raysOnDevice)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dRays, &ctx->raysCap, (size_t)n * 24, "cudaMalloc rays")) return r;
+        CK(cudaMemcpyAsync(ctx->dRays, rays6, (size_t)n * 24, cudaMemcpyHostToDevice, stream), "H2D rays");
+        dRays = ctx->dRays;
+    }
+    if (!outOnDevice)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, (size_t)n * 16, "cudaMalloc ray outputs")) return r;
+        dOut = ctx->dImage;
+    }
+    if (int r = start_kernels(ctx, stream, 1)) return r;
+    DrawParams p;
+    memset(&p, 0, sizeof(p));
+    p.spp = spp;
+    p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
+    p.image = dOut;
+    p.rayCounter = ctx->dRayCounters;
+    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    p.rays = dRays;
+    p.numRays = (uint32_t)n;
+    cudaError_t e = launch_fast_rays(p, scene, ctx->numSMs, stream);
+    if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+    ctx->lastLaunches += 1;
+    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
+    if (!outOnDevice) CK(cudaMemcpyAsync(out4, dOut, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H ray outputs");
+    return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
 }
 
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStreamArg, long long* outRays)

@@ -427,6 +427,50 @@ __device__ __forceinline__ void generate_slab_rays(const DrawParams& p, float4 (
     }
 }
 
+// Caller rays of one slab (tpt_trace_rays): rays [r0, r0 + count) of p.rays, count <= kSlabPix. The warp reads their
+// 6 * count floats as rows of 32 consecutive floats (coalesced at any 4-byte alignment of p.rays) into its shared buffer, each
+// lane then takes rays `lane` and `lane + 32` from there, normalises the direction and seeds the stream with
+// pixel_seed(ray * spp + sample, frame). A ray with a non-finite component, or whose direction does not normalise to a finite
+// non-zero vector (zero length, or a squared length that underflows or overflows), is dropped: the survivors are written
+// compacted, in ray order, as {origin.xyz, rng state} {direction.xyz, ray index}. Returns their number.
+__device__ __forceinline__ uint32_t load_slab_rays(const DrawParams& p, float4 (*rays)[2], int lane, uint32_t count,
+                                                   uint32_t r0, uint32_t sample, uint32_t frame)
+{
+    float* raw = reinterpret_cast<float*>(rays);
+    const float* src = p.rays + (size_t)r0 * 6;
+#pragma unroll
+    for (uint32_t k = 0; k < 6 * kSlabPix; k += 32)
+        if (k + lane < 6 * count) raw[k + lane] = __ldg(src + k + lane);
+    __syncwarp();
+    float v[2][6];
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int j = 0; j < 6; ++j) v[h][j] = (uint32_t)(lane + 32 * h) < count ? raw[(lane + 32 * h) * 6 + j] : 0.0f;
+    __syncwarp();
+    uint32_t base = 0;
+    const unsigned ltMask = (1u << lane) - 1u;
+#pragma unroll
+    for (int h = 0; h < 2; ++h)
+    {
+        const uint32_t q = (uint32_t)lane + 32u * h;
+        const V3 o = v3(v[h][0], v[h][1], v[h][2]);
+        const V3 d = M<false>::normalize(v3(v[h][3], v[h][4], v[h][5]));
+        const bool ok = q < count && isfinite(o.x) && isfinite(o.y) && isfinite(o.z) && isfinite(d.x) && isfinite(d.y) &&
+                        isfinite(d.z) && (d.x != 0.0f || d.y != 0.0f || d.z != 0.0f);
+        const unsigned m = __ballot_sync(0xffffffffu, ok);
+        if (ok)
+        {
+            const uint32_t slot = base + (uint32_t)__popc(m & ltMask);
+            const uint32_t rng = pixel_seed((r0 + q) * (uint32_t)p.spp + sample, frame);
+            rays[slot][0] = make_float4(o.x, o.y, o.z, __uint_as_float(rng));
+            rays[slot][1] = make_float4(d.x, d.y, d.z, __uint_as_float(r0 + q));
+        }
+        base += (uint32_t)__popc(m);
+    }
+    return base;
+}
+
 struct QPath
 {
     V3 o, d;
@@ -944,7 +988,9 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // per SM when the sphere arrays fill most of an SM's shared memory.
 // Dynamic shared memory (FastSmem): [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
 // The body is shared by k_fast_queue (light sampling) and k_fast_queue_nolight (DO_LIGHT_SAMPLING 0) below.
-template <int THREADS, int KFORM, int LS>
+// RAYS: the ray source. false: camera rays of the image region; true (k_fast_rays): the caller's p.numRays rays
+// (load_slab_rays), a slab being 64 consecutive rays x one sample index, finished paths adding col / spp to p.image[ray].
+template <int THREADS, int KFORM, int LS, bool RAYS = false>
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
@@ -969,7 +1015,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
     const unsigned ltMask = (1u << lane) - 1u;
-    const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
+    const uint32_t regionPix = RAYS ? p.numRays : (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
     
     unsigned rc = 0;
@@ -1014,15 +1060,19 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
                 const uint32_t pix0 = mtile * kSlabPix;
                 slabEnd = regionPix - pix0 < (uint32_t)kSlabPix ? regionPix - pix0 : (uint32_t)kSlabPix;
                 slabCur = 0;
-                slabRi0 = (int)(pix0 / (uint32_t)p.width);
-                slabX0 = (int)(pix0 - (uint32_t)slabRi0 * (uint32_t)p.width);
+                if constexpr (!RAYS)
+                {
+                    slabRi0 = (int)(pix0 / (uint32_t)p.width);
+                    slabX0 = (int)(pix0 - (uint32_t)slabRi0 * (uint32_t)p.width);
+                }
                 const uint32_t fi = s / (uint32_t)p.spp;
                 slabSample = s - fi * (uint32_t)p.spp;
                 slabFrame = (uint32_t)p.frame0 + fi;
                 slabW = invSpp * sW[fi];
                 slabBand = bandDone ? mtile / mtilesPerBand : 0u;
                 __syncwarp();       // every lane has popped what it needed from the previous slab
-                generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, slabX0, slabRi0, slabSample, slabFrame, -1);
+                if constexpr (RAYS) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
+                else generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, slabX0, slabRi0, slabSample, slabFrame, -1);
                 __syncwarp();
             }
             const uint32_t avail = slabEnd - slabCur;
@@ -1095,6 +1145,26 @@ k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, Scene
                      uint32_t raysOffset)
 {
     fast_queue_body<THREADS, KFORM, kLsOff>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+}
+
+// tpt_trace_rays: the slab queue on caller rays (RAYS = true), with the same launch shapes as k_fast_queue and the
+// DO_LIGHT_SAMPLING 0 twin. Only the instances pick_queue<true> can choose are instantiated.
+template <int THREADS, int MINB, int KFORM>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+            uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+            uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOn, true>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+}
+
+template <int THREADS, int MINB, int KFORM>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                    uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+                    uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOff, true>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
 }
 
 // ---- variant 8 ------------------------------------------------------------------------------------------------
@@ -1770,27 +1840,67 @@ float prev_weight(int frame0, int numFrames, unsigned flags)
 }
 
 using QueueKernel = decltype(&k_fast_queue<128, TPT_QUEUE_MINB, 0>);
-template <int THREADS, int MINB>
+// RAYS: the tpt_trace_rays family (k_fast_rays) instead of the camera-ray one (k_fast_queue)
+template <bool RAYS, int THREADS, int MINB, int KFORM>
+static QueueKernel queue_instance(const SceneDev& sc)
+{
+    if constexpr (RAYS) return light_twin(sc, k_fast_rays<THREADS, MINB, KFORM>, k_fast_rays_nolight<THREADS, MINB, KFORM>);
+    else return light_twin(sc, k_fast_queue<THREADS, MINB, KFORM>, k_fast_queue_nolight<THREADS, MINB, KFORM>);
+}
+template <bool RAYS, int THREADS, int MINB>
 static QueueKernel queue_kernel(const SceneDev& sc, int kform)
 {
-    return for_kform<3>(kform, [&](auto K) {
-        return light_twin(sc, k_fast_queue<THREADS, MINB, decltype(K)::value>, k_fast_queue_nolight<THREADS, MINB, decltype(K)::value>);
-    });
+    return for_kform<3>(kform, [&](auto K) { return queue_instance<RAYS, THREADS, MINB, decltype(K)::value>(sc); });
 }
 
-static cudaError_t launch_queue(QueueKernel kern, int threads, int kform, const DrawParams& p, const SceneDev& sc, int numSMs,
+struct QueuePick
+{
+    QueueKernel kern;
+    int threads, kform;
+};
+// The slab-queue instance for `samples` samples of each of `regionPix` pixels or rays (variants 3/4/9; tpt_trace_rays
+// takes variant 3's choice). Small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays
+// fill most of an SM's shared memory: ONE 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs
+// x 4 warps with a copy each). Long launches (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80;
+// short ones keep 6, where a warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant
+// 9 forces the 8-CTA instance (A/B runs).
+template <bool RAYS>
+static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix, long long samples, int numSMs)
+{
+    QueuePick q;
+    q.kform = fast_queue_kform(sc);
+    const bool big = fast_smem(sc.stagedBytes, q.kform >= 2 ? simd_count(sc) * 16 : 0, 4 * 2048).bytes > 36 * 1024 ||
+                     sc.stagedBytes != sc.layout.totalBytes;
+    const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
+    q.threads = big ? TPT_BIG_THREADS : 128;
+    if (big) q.kern = queue_kernel<RAYS, TPT_BIG_THREADS, 1>(sc, q.kform);
+    else if (q.kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) q.kern = queue_instance<RAYS, 128, 8, 2>(sc);
+    else if (!RAYS && variant == 4) q.kern = queue_kernel<false, 128, 7>(sc, q.kform);
+    else q.kern = queue_kernel<RAYS, 128, TPT_QUEUE_MINB>(sc, q.kform);
+    return q;
+}
+
+// regionPix: pixels of the draw's region, or tpt_trace_rays' ray count. The accumulation buffer is prepared first: a draw's
+// region blended by the weight of `prev` (k_prepare_image), caller rays' float4 outputs zeroed.
+template <bool RAYS>
+static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const DrawParams& p, const SceneDev& sc, int numSMs,
                                 cudaStream_t stream, unsigned int* bandDone, int numBands, unsigned int* bandExpected)
 {
-    const FastSmem lay = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0, (uint32_t)(threads / 32) * kSlabPix * 32, true);
-    const long long regionPix = (long long)p.numRows * p.width;
+    const QueueKernel kern = q.kern;
+    const int threads = q.threads;
+    const FastSmem lay = fast_smem(sc.stagedBytes, q.kform >= 2 ? simd_count(sc) * 16 : 0, (uint32_t)(threads / 32) * kSlabPix * 32, true);
     const uint32_t S = (uint32_t)(p.spp * p.numFrames);
     const long long slabs = ((regionPix + kSlabPix - 1) / kSlabPix) * S;
     if (slabs > 0x7fffffffLL) return cudaErrorInvalidValue;
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, threads, lay.bytes, numSMs, (slabs + threads / 32 - 1) / (threads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
-    k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
-    e = cudaGetLastError();
+    if constexpr (RAYS) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
+    else
+    {
+        k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
+        e = cudaGetLastError();
+    }
     if (e != cudaSuccess) return e;
     // optional progress bands (host-buffer draws): band b = macro-tiles [b*mpb, (b+1)*mpb)
     const uint32_t mtiles = (uint32_t)((regionPix + kSlabPix - 1) / kSlabPix);
@@ -1861,6 +1971,12 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
     return cudaGetLastError();
 }
 
+cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
+{
+    const QueuePick q = pick_queue<true>(sc, 3, p.numRays, p.spp, numSMs);
+    return launch_queue<true>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
+}
+
 int fast_slab_pixels() { return kSlabPix; }
 
 int fast_kernel_launches(const DrawParams&, int variant) { return (variant == 3 || variant == 4 || variant == 9 || variant == 6 || variant == 7) ? 2 : 1; }
@@ -1893,22 +2009,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
     }
     if (variant == 3 || variant == 4 || variant == 9)
     {
-        const int kform = fast_queue_kform(sc);
-        // small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays fill most of an SM's
-        // shared memory: ONE 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs x 4 warps
-        // with a copy each)
-        const bool big = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0, 4 * 2048).bytes > 36 * 1024 ||
-                         sc.stagedBytes != sc.layout.totalBytes;
-        // long draws (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80; short ones keep 6, where a
-        // warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant 9 forces the 8-CTA
-        // instance (A/B runs).
-        const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * p.spp * p.numFrames / ((long long)numSMs * 32);
-        QueueKernel kern = variant == 4 ? queue_kernel<128, 7>(sc, kform) : queue_kernel<128, TPT_QUEUE_MINB>(sc, kform);
-        int threads = 128;
-        if (big) { kern = queue_kernel<TPT_BIG_THREADS, 1>(sc, kform); threads = TPT_BIG_THREADS; }
-        else if (kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48)))
-            kern = light_twin(sc, k_fast_queue<128, 8, 2>, k_fast_queue_nolight<128, 8, 2>);
-        return launch_queue(kern, threads, kform, p, sc, numSMs, stream, bandDone, numBands, bandExpected);
+        const QueuePick q = pick_queue<false>(sc, variant, regionPix, (long long)p.spp * p.numFrames, numSMs);
+        return launch_queue<false>(q, regionPix, p, sc, numSMs, stream, bandDone, numBands, bandExpected);
     }
     if (variant == 8)
     {

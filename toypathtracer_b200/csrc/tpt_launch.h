@@ -32,6 +32,10 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
 // form a band.
 cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, int numSMs, cudaStream_t stream,
                         unsigned int* bandDone = nullptr, int numBands = 0, unsigned int* bandExpected = nullptr);
+// tpt_trace_rays: fast-mode radiance of p.numRays (>= 1) caller rays p.rays, p.spp samples each with streams
+// pixel_seed(ray * spp + sample, p.frame0), mean written to the float4 p.image[ray] (zeroed first); p.numFrames = 1, p.flags = 0.
+// Runs the slab-queue instance variant 3 would run for the scene.
+cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 // TPT_MODE_REFGPU (tpt_refgpu.cuh): strict arithmetic (tpt_exact.cu) / GPU-native arithmetic (tpt_fast.cu)
 cudaError_t launch_refgpu_exact(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 cudaError_t launch_refgpu_fast(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);

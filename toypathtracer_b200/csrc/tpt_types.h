@@ -88,6 +88,8 @@ struct DrawParams
     float* scratch;           // exact mode, numFrames > 1: [numFrames][numRows][width] float4 per-frame colours
     unsigned long long* rayCounter; // [numFrames] in exact mode, [1] in fast mode
     unsigned int* workCounter;      // persistent kernels: next tile
+    const float* rays;        // tpt_trace_rays: numRays caller rays {o.xyz, d.xyz}, 4-byte aligned; `image` gets one float4 per ray
+    uint32_t numRays;
 };
 
 } // namespace tpt

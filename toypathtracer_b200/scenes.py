@@ -33,6 +33,27 @@ def make_camera(lookfrom, lookat, vup, vfov, aspect, aperture, focus_dist) -> np
     return cam
 
 
+def camera_rays(camera, width: int, height: int, per_pixel: int = 1, seed: int = 0) -> np.ndarray:
+    """Rays of the thin-lens camera (Camera::GetRay, Cpp/Source/Maths.h:437-442) for Context.trace_rays: an
+    (width * height * per_pixel, 6) float32 array {o.xyz, d.xyz}, `per_pixel` rays per pixel, each with a uniform jitter
+    inside its pixel and a uniform sample of the lens disk. Pixel-major: the rays of pixel (x, y) are rows
+    (y * width + x) * per_pixel + k, with row y = 0 at the bottom like the backbuffer. Computed in float64 from the float32
+    camera, unit directions, deterministic in `seed`."""
+    cam = {k: np.asarray(camera[k], np.float64).reshape(-1)
+           for k in ("origin", "lowerLeftCorner", "horizontal", "vertical", "uu", "vv", "lensRadius")}
+    rng = np.random.default_rng(seed)
+    n = width * height * per_pixel
+    pix = np.arange(n) // per_pixel
+    s = (pix % width + rng.random(n)) / width
+    t = (pix // width + rng.random(n)) / height
+    r = cam["lensRadius"][0] * np.sqrt(rng.random(n))
+    phi = 2.0 * np.pi * rng.random(n)
+    offset = (r * np.cos(phi))[:, None] * cam["uu"] + (r * np.sin(phi))[:, None] * cam["vv"]
+    d = cam["lowerLeftCorner"] + s[:, None] * cam["horizontal"] + t[:, None] * cam["vertical"] - cam["origin"] - offset
+    d /= np.linalg.norm(d, axis=1, keepdims=True)
+    return np.concatenate([cam["origin"] + offset, d], axis=1).astype(np.float32)
+
+
 def reference_scene(width: int, height: int, time: float = 0.0, flags: int = 0, big_scene: bool = True,
                     mitsuba_compare: bool = False):
     """(spheres, materials, camera, emissives) of the reference scene at this aspect ratio, produced by the
