@@ -153,6 +153,43 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
 int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
                    float* out4, int outOnDevice, long long* outRayCount, void* cudaStream);
 
+/* First-hit AOVs (arbitrary output values) of the fast mode: the denoiser guides, depth, mask and id buffers that go next
+ * to an image. One nearest-hit query per sample, no shading. Outputs, per pixel or per ray; each pointer may be NULL (not
+ * written), but not all three:
+ *   albedo4           float4 (albedo.rgb, coverage): the stored albedo of the hit sphere's material, whatever its type,
+ *                     and 1 for a hit; a miss adds zeros.
+ *   normal4           float4 (normal.xyz, depth): (hit - centre) * invRadius as the renderer shades with it (not flipped
+ *                     toward the ray, not renormalised), and the distance t along the unit direction; a miss adds zeros.
+ *   ids               int32: the id of the hit sphere, -1 for a miss.
+ * A hit on a padding sphere (id >= count, possible with the reference-form sweep only) reports the all-zero material and
+ * a zero normal, as the draw sees it.
+ * Float4 device buffers must be 16-byte aligned and ids 4-byte aligned. Host buffers are staged through the context and
+ * make the call synchronous. Ordering and accounting are those of tpt_draw: one ray per traced sample counts toward
+ * outRayCount and tpt_read_ray_count, and tpt_last_kernel_ms / tpt_last_launch_count describe the call. Bad arguments are
+ * refused (tpt_last_error gives the reason).
+ *
+ * tpt_draw_aovs: the AOVs of the pixels a fast-mode tpt_draw with the same frameCount, numFrames, width, height, row
+ * region, testFlags, spp and scene traces. Sample s of frame f of pixel (x, y) uses exactly that draw's camera ray
+ * (stream pixel_seed((y * width + x) * spp + s, f), pixel jitter, lens sample) and its slab-queue sweep form, so the AOVs
+ * describe the primary hits of fast variants 3 and 8. The float4 outputs are blended like the image:
+ * out = prev * wPrev + sum_f w_f * mean_f (all four components; `prev` is not read when its weight is 0), so buffers kept
+ * next to the backbuffer and drawn with the same arguments accumulate over the same samples, progressive rendering
+ * included. ids is not blended: each call writes the id of sample 0 of frame frameCount. The row region (row0, numRows,
+ * rowStep, packed), the buffer sizes (width*height pixels, or numRows with `packed`) and numRows == 0 are as in tpt_draw;
+ * other rows are not touched. numFrames <= 256. Host float4 buffers are uploaded only when `prev` has weight.
+ *
+ * tpt_trace_aovs: the AOVs of n caller rays {o.xyz, d.xyz}, loaded, validated and normalised as tpt_trace_rays does (same
+ * alignment of rays6). Deterministic: coverage is 0 or 1 and depth is in world units whatever the length of the given
+ * direction. An untraceable ray (non-finite component, or a direction that does not normalise) gives zeros and id -1 and
+ * adds no rays. n <= 2^32 - 1; n == 0 launches nothing. */
+int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
+                  int row0, int numRows, int rowStep, int packed,
+                  float* albedo4, float* normal4, int* ids, int buffersOnDevice, unsigned testFlags,
+                  long long* outRayCount, void* cudaStream);
+int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n,
+                   float* albedo4, float* normal4, int* ids, int outOnDevice,
+                   long long* outRayCount, void* cudaStream);
+
 /* Rays traced by all draws since the last call of this function (synchronises the stream). */
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStream, long long* outRays);
 /* Device time (CUDA events on the launching stream) of the kernels of the most recent tpt_draw, in ms. */

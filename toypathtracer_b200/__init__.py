@@ -76,6 +76,9 @@ def _load_lib():
     L.tpt_debug_libm.argtypes = [vp, ci, vp, vp, cll]; L.tpt_debug_libm.restype = ci
     L.tpt_debug_hit.argtypes = [vp, ci, vp, vp, vp, cll]; L.tpt_debug_hit.restype = ci
     L.tpt_trace_rays.argtypes = [vp, vp, ci, cll, ci, ci, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_rays.restype = ci
+    L.tpt_draw_aovs.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, ci, cu, ctypes.POINTER(cll), vp]
+    L.tpt_draw_aovs.restype = ci
+    L.tpt_trace_aovs.argtypes = [vp, vp, ci, cll, vp, vp, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_aovs.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -98,19 +101,43 @@ class DevicePtr:
         self.addr = int(addr)
 
 
-def _as_ptr(buf) -> Tuple[int, bool, object]:
-    """(address, on_device, keepalive) for a numpy array, a torch tensor or a raw device address."""
+def _as_ptr(buf, dtype: str = "float32") -> Tuple[int, bool, object]:
+    """(address, on_device, keepalive) for a numpy array, a torch tensor or a raw device address of element type `dtype`
+    ("float32", or "int32" for id buffers)."""
     if isinstance(buf, DevicePtr):
         return buf.addr, True, buf
     if isinstance(buf, np.ndarray):
-        if buf.dtype != np.float32 or not buf.flags["C_CONTIGUOUS"]:
-            raise TptError("backbuffer must be a C-contiguous float32 array")
+        if buf.dtype != np.dtype(dtype) or not buf.flags["C_CONTIGUOUS"]:
+            raise TptError(f"backbuffer must be a C-contiguous {dtype} array")
         return buf.ctypes.data, False, buf
     if hasattr(buf, "data_ptr"):  # torch tensor
-        if not buf.is_contiguous() or str(buf.dtype) != "torch.float32":
-            raise TptError("backbuffer tensor must be contiguous float32")
+        if not buf.is_contiguous() or str(buf.dtype) != f"torch.{dtype}":
+            raise TptError(f"backbuffer tensor must be contiguous {dtype}")
         return int(buf.data_ptr()), bool(buf.is_cuda), buf
     raise TptError("unsupported backbuffer type")
+
+
+def _numel(buf) -> int:
+    return int(buf.size) if isinstance(buf, np.ndarray) else int(buf.numel())
+
+
+def _aov_ptrs(what: str, albedo, normal, ids, pixels: int):
+    """Addresses of the AOV outputs that are given (float4 albedo and normal, int32 ids, `pixels` entries each unless a
+    DevicePtr), their common kind (on device or not) and keepalives."""
+    ptrs, kinds, keep = [], set(), []
+    for name, buf, dtype, per in (("albedo", albedo, "float32", 4), ("normal", normal, "float32", 4), ("ids", ids, "int32", 1)):
+        if buf is None:
+            ptrs.append(None)
+            continue
+        if not isinstance(buf, DevicePtr) and _numel(buf) != pixels * per:
+            raise TptError(f"{what}: {name} must hold {pixels} x {per} {dtype} values, not {_numel(buf)}")
+        addr, on_dev, k = _as_ptr(buf, dtype)
+        ptrs.append(ctypes.c_void_p(addr)); kinds.add(on_dev); keep.append(k)
+    if not kinds:
+        raise TptError(f"{what}: no output buffer (albedo, normal or ids)")
+    if len(kinds) > 1:
+        raise TptError(f"{what}: the outputs must be all host or all device buffers")
+    return ptrs, kinds.pop(), keep
 
 
 class Context:
@@ -219,6 +246,56 @@ class Context:
                                     ctypes.c_void_p(stream) if stream else None)
         self._check(rc, "tpt_trace_rays")
         return (out, int(total.value)) if want_rays else out
+
+    def draw_aovs(self, frame: int, num_frames: int, width: int, height: int, albedo=None, normal=None, ids=None,
+                  flags: int = 0, rows: Optional[Tuple[int, int, int, int]] = None, stream: int = 0, want_rays: bool = True):
+        """tpt_draw_aovs: first-hit AOVs of the fast draw draw(frame, num_frames, width, height, ..., flags, MODE_FAST,
+        rows) would make, into any of albedo (albedo.rgb, coverage), normal (normal.xyz, depth) — float32 buffers of
+        4 values per pixel, blended over their contents like the image — and ids (int32, sample 0's sphere id or -1).
+        Buffers hold width x height pixels (numRows with a packed row region), all host or all device; rows = (row0,
+        numRows, rowStep, packed). Returns the rays traced (one per sample) if want_rays, else None."""
+        row0, nrows, step, packed = rows if rows is not None else (0, height, 1, 0)
+        (pa, pn, pi), on_dev, _keep = _aov_ptrs("draw_aovs", albedo, normal, ids, (nrows if packed else height) * width)
+        total = ctypes.c_longlong(0)
+        rc = self._L.tpt_draw_aovs(self._h, frame, num_frames, width, height, row0, nrows, step, packed, pa, pn, pi,
+                                   1 if on_dev else 0, flags, ctypes.byref(total) if want_rays else None,
+                                   ctypes.c_void_p(stream) if stream else None)
+        self._check(rc, "tpt_draw_aovs")
+        return int(total.value) if want_rays else None
+
+    def trace_aovs(self, rays, albedo=None, normal=None, ids=None, n=None, stream: int = 0, want_rays: bool = True):
+        """tpt_trace_aovs: first-hit AOVs of caller rays {o.xyz, d.xyz} (buffers as for trace_rays). albedo and normal
+        receive N float4 (albedo.rgb, coverage) and (normal.xyz, depth), ids N int32 (-1: miss or untraceable ray); any
+        of them may be omitted, and without all three they are allocated, (N, 4), (N, 4) and (N,), of the kind of `rays`
+        (a DevicePtr gets CUDA tensors). Returns ((albedo, normal, ids), rays traced), or the tuple alone when want_rays
+        is False."""
+        if isinstance(rays, DevicePtr):
+            if n is None:
+                raise TptError("trace_aovs: a DevicePtr needs n")
+            raddr, ron, keep = rays.addr, True, rays
+        else:
+            if tuple(rays.shape[1:]) != (6,) or len(rays.shape) != 2:
+                raise TptError("trace_aovs: rays must have shape (N, 6)")
+            if n is not None and int(n) != rays.shape[0]:
+                raise TptError("trace_aovs: n does not match rays")
+            n = rays.shape[0]
+            raddr, ron, keep = _as_ptr(rays)
+        n = int(n)
+        if albedo is None and normal is None and ids is None:
+            if isinstance(rays, np.ndarray):
+                albedo, normal, ids = np.empty((n, 4), np.float32), np.empty((n, 4), np.float32), np.empty(n, np.int32)
+            else:
+                import torch
+                dev = rays.device if hasattr(rays, "device") else torch.device("cuda", self.device)
+                albedo = torch.empty((n, 4), dtype=torch.float32, device=dev)
+                normal = torch.empty((n, 4), dtype=torch.float32, device=dev)
+                ids = torch.empty(n, dtype=torch.int32, device=dev)
+        (pa, pn, pi), oon, _keep = _aov_ptrs("trace_aovs", albedo, normal, ids, n)
+        total = ctypes.c_longlong(0)
+        rc = self._L.tpt_trace_aovs(self._h, ctypes.c_void_p(raddr), 1 if ron else 0, n, pa, pn, pi, 1 if oon else 0,
+                                    ctypes.byref(total) if want_rays else None, ctypes.c_void_p(stream) if stream else None)
+        self._check(rc, "tpt_trace_aovs")
+        return ((albedo, normal, ids), int(total.value)) if want_rays else (albedo, normal, ids)
 
     def read_ray_count(self, stream: int = 0) -> int:
         out = ctypes.c_longlong(0)

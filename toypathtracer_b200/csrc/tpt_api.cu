@@ -75,7 +75,10 @@ struct tpt_context
 
     // buffers
     float* dImage = nullptr; size_t imageCap = 0;      // staging image for host-pointer draws (and host tpt_trace_rays outputs)
-    float* dRays = nullptr; size_t raysCap = 0;        // staging of host tpt_trace_rays inputs
+    float* dRays = nullptr; size_t raysCap = 0;        // staging of host tpt_trace_rays / tpt_trace_aovs inputs
+    float* dAovAlbedo = nullptr; size_t aovAlbedoCap = 0;   // staging of host AOV outputs (tpt_draw_aovs, tpt_trace_aovs)
+    float* dAovNormal = nullptr; size_t aovNormalCap = 0;
+    int* dAovIds = nullptr; size_t aovIdsCap = 0;
     float* dScratch = nullptr; size_t scratchCap = 0;  // exact mode per-frame colours
     unsigned long long* dRayCounters = nullptr; int rayCounterCap = 0;   // [numFrames]
     unsigned long long* dAccum = nullptr;              // [0] total since last read, [1] last draw total
@@ -227,7 +230,7 @@ void tpt_destroy(tpt_context* ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->registeredPtr) cudaHostUnregister(ctx->registeredPtr);
-    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
+    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dAovAlbedo); cudaFree(ctx->dAovNormal); cudaFree(ctx->dAovIds); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
     cudaFree(ctx->dAccum); cudaFree(ctx->dWork);
     for (int i = 0; i < 2; ++i)
     {
@@ -371,13 +374,16 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     return fail_msg(ctx, "tpt_set_option: unknown key");
 }
 
-// Copies the rows y_i = row0 + i*rowStep (or the packed band) of a float4 image between host and device.
-static cudaError_t copy_rows(float* dst, const float* src, int width, int row0, int numRows, int rowStep, int packed,
-                             cudaMemcpyKind kind, cudaStream_t stream)
+// Copies the rows y_i = row0 + i*rowStep (or the packed band) of an image of pixBytes-byte pixels (float4 by default)
+// between host and device.
+static cudaError_t copy_rows(void* dstBase, const void* srcBase, int width, int row0, int numRows, int rowStep, int packed,
+                             cudaMemcpyKind kind, cudaStream_t stream, size_t pixBytes = 16)
 {
-    const size_t rowBytes = (size_t)width * 16;
+    char* dst = (char*)dstBase;
+    const char* src = (const char*)srcBase;
+    const size_t rowBytes = (size_t)width * pixBytes;
     if (packed) return cudaMemcpyAsync(dst, src, rowBytes * numRows, kind, stream);
-    const size_t off = (size_t)row0 * width * 4;
+    const size_t off = (size_t)row0 * rowBytes;
     if (rowStep == 1) return cudaMemcpyAsync(dst + off, src + off, rowBytes * numRows, kind, stream);
     return cudaMemcpy2DAsync(dst + off, rowBytes * rowStep, src + off, rowBytes * rowStep, rowBytes, numRows, kind, stream);
 }
@@ -726,20 +732,21 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
 }
 
-// A device buffer of tpt_trace_rays must be addressable by the context's device: its own memory, or mapped host memory.
-static int check_device_buffer(tpt_context* ctx, const void* ptr, const char* name)
+// A device buffer of tpt_trace_rays (or the AOV calls, named by fn) must be addressable by the context's device: its own
+// memory, or mapped host memory.
+static int check_device_buffer(tpt_context* ctx, const void* ptr, const char* name, const char* fn = "tpt_trace_rays")
 {
     cudaPointerAttributes attr;
     char msg[160];
     if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess || attr.type == cudaMemoryTypeUnregistered)
     {
         (void)cudaGetLastError();
-        snprintf(msg, sizeof(msg), "tpt_trace_rays: device %s is not CUDA memory", name);
+        snprintf(msg, sizeof(msg), "%s: device %s is not CUDA memory", fn, name);
         return fail_msg(ctx, msg);
     }
     if ((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device != ctx->device)
     {
-        snprintf(msg, sizeof(msg), "tpt_trace_rays: device %s lives on device %d, the context on device %d", name, attr.device, ctx->device);
+        snprintf(msg, sizeof(msg), "%s: device %s lives on device %d, the context on device %d", fn, name, attr.device, ctx->device);
         return fail_msg(ctx, msg);
     }
     return 0;
@@ -796,6 +803,169 @@ int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (!outOnDevice) CK(cudaMemcpyAsync(out4, dOut, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H ray outputs");
+    return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
+}
+
+// Outputs of tpt_draw_aovs / tpt_trace_aovs (fn): at least one buffer; device buffers aligned (float4 outputs to 16 bytes,
+// ids to 4) and addressable by the context's device.
+static int check_aov_outputs(tpt_context* ctx, const char* fn, const float* albedo4, const float* normal4, const int* ids, int onDevice)
+{
+    char msg[160];
+    if (!albedo4 && !normal4 && !ids)
+    {
+        snprintf(msg, sizeof(msg), "%s: albedo4, normal4 and ids are all null", fn);
+        return fail_msg(ctx, msg);
+    }
+    if (!onDevice) return 0;
+    const struct { const void* ptr; const char* name; int align; } outs[3] = {{albedo4, "albedo4", 16}, {normal4, "normal4", 16}, {ids, "ids", 4}};
+    for (const auto& o : outs)
+    {
+        if (!o.ptr) continue;
+        if ((uintptr_t)o.ptr & (uintptr_t)(o.align - 1))
+        {
+            snprintf(msg, sizeof(msg), "%s: device %s is not %d-byte aligned", fn, o.name, o.align);
+            return fail_msg(ctx, msg);
+        }
+        if (int r = check_device_buffer(ctx, o.ptr, o.name, fn)) return r;
+    }
+    return 0;
+}
+
+// Host AOV outputs of `pixels` pixels: each given buffer is replaced by the context's staging buffer for it.
+static int stage_aov_outputs(tpt_context* ctx, size_t pixels, float*& albedo4, float*& normal4, int*& ids)
+{
+    if (albedo4)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dAovAlbedo, &ctx->aovAlbedoCap, pixels * 16, "cudaMalloc AOV albedo4")) return r;
+        albedo4 = ctx->dAovAlbedo;
+    }
+    if (normal4)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dAovNormal, &ctx->aovNormalCap, pixels * 16, "cudaMalloc AOV normal4")) return r;
+        normal4 = ctx->dAovNormal;
+    }
+    if (ids)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dAovIds, &ctx->aovIdsCap, pixels * 4, "cudaMalloc AOV ids")) return r;
+        ids = ctx->dAovIds;
+    }
+    return 0;
+}
+
+int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
+                  int row0, int numRows, int rowStep, int packed,
+                  float* albedo4, float* normal4, int* ids, int buffersOnDevice, unsigned testFlags,
+                  long long* outRayCount, void* cudaStreamArg)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!ctx->haveScene) return fail_msg(ctx, "tpt_draw_aovs: no scene (call tpt_set_scene first)");
+    if (width <= 0 || height <= 0 || numFrames <= 0 || frameCount < 0 || numRows < 0 || rowStep <= 0 || row0 < 0)
+        return fail_msg(ctx, "tpt_draw_aovs: bad arguments");
+    if (numFrames > 256) return fail_msg(ctx, "tpt_draw_aovs: numFrames > 256");
+    if (int r = check_aov_outputs(ctx, "tpt_draw_aovs", albedo4, normal4, ids, buffersOnDevice)) return r;
+    if (numRows == 0)
+    {
+        if (outRayCount) *outRayCount = 0;
+        ctx->lastLaunches = 0;
+        return 0;
+    }
+    if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw_aovs: rows outside the image");
+    if ((long long)numRows * width > 0xffffffe0LL) return fail_msg(ctx, "tpt_draw_aovs: more than 2^32 - 32 pixels");
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+
+    float* dAlbedo = albedo4;
+    float* dNormal = normal4;
+    int* dIds = ids;
+    if (!buffersOnDevice)
+    {
+        const size_t bufPix = (packed ? (size_t)numRows : (size_t)height) * width;
+        if (int r = stage_aov_outputs(ctx, bufPix, dAlbedo, dNormal, dIds)) return r;
+        // the float4 outputs are `prev` of the blend when it has weight; ids are not blended
+        if (prev_weight(frameCount, numFrames, testFlags) != 0.0f)
+        {
+            if (albedo4) CK(copy_rows(dAlbedo, albedo4, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream), "H2D albedo4");
+            if (normal4) CK(copy_rows(dNormal, normal4, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream), "H2D normal4");
+        }
+    }
+    if (int r = start_kernels(ctx, stream, 1)) return r;
+    DrawParams p;
+    memset(&p, 0, sizeof(p));
+    p.cam = ctx->cam;
+    p.width = width; p.height = height;
+    p.row0 = row0; p.numRows = numRows; p.rowStep = rowStep; p.packed = packed ? 1 : 0;
+    p.frame0 = frameCount; p.numFrames = numFrames;
+    p.spp = ctx->spp;
+    p.flags = testFlags;
+    p.invWidth = 1.0f / (float)width;
+    p.invHeight = 1.0f / (float)height;
+    p.rayCounter = ctx->dRayCounters;
+    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    cudaError_t e = launch_fast_aovs(p, scene, false, dAlbedo, dNormal, dIds, ctx->numSMs, stream);
+    if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+    ctx->lastLaunches += 1;
+    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
+    if (!buffersOnDevice)
+    {
+        if (albedo4) CK(copy_rows(albedo4, dAlbedo, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream), "D2H albedo4");
+        if (normal4) CK(copy_rows(normal4, dNormal, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream), "D2H normal4");
+        if (ids) CK(copy_rows(ids, dIds, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream, 4), "D2H ids");
+    }
+    return finish_call(ctx, stream, 1, !buffersOnDevice, outRayCount, nullptr);
+}
+
+int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n,
+                   float* albedo4, float* normal4, int* ids, int outOnDevice,
+                   long long* outRayCount, void* cudaStreamArg)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!ctx->haveScene) return fail_msg(ctx, "tpt_trace_aovs: no scene (call tpt_set_scene first)");
+    if (!rays6) return fail_msg(ctx, "tpt_trace_aovs: null rays6");
+    if (n < 0) return fail_msg(ctx, "tpt_trace_aovs: n < 0");
+    if (n > 0xffffffffLL) return fail_msg(ctx, "tpt_trace_aovs: n > 2^32 - 1 (32-bit ray indices)");
+    if (raysOnDevice && ((uintptr_t)rays6 & 3)) return fail_msg(ctx, "tpt_trace_aovs: device rays6 is not 4-byte aligned");
+    if (int r = check_aov_outputs(ctx, "tpt_trace_aovs", albedo4, normal4, ids, outOnDevice)) return r;
+    if (raysOnDevice) { if (int r = check_device_buffer(ctx, rays6, "rays6", "tpt_trace_aovs")) return r; }
+    if (n == 0)
+    {
+        if (outRayCount) *outRayCount = 0;
+        ctx->lastLaunches = 0;
+        return 0;
+    }
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+    const float* dRays = rays6;
+    if (!raysOnDevice)
+    {
+        if (int r = ensure(ctx, (void**)&ctx->dRays, &ctx->raysCap, (size_t)n * 24, "cudaMalloc rays")) return r;
+        CK(cudaMemcpyAsync(ctx->dRays, rays6, (size_t)n * 24, cudaMemcpyHostToDevice, stream), "H2D rays");
+        dRays = ctx->dRays;
+    }
+    float* dAlbedo = albedo4;
+    float* dNormal = normal4;
+    int* dIds = ids;
+    if (!outOnDevice) { if (int r = stage_aov_outputs(ctx, (size_t)n, dAlbedo, dNormal, dIds)) return r; }
+    if (int r = start_kernels(ctx, stream, 1)) return r;
+    DrawParams p;
+    memset(&p, 0, sizeof(p));
+    p.spp = 1;
+    p.numFrames = 1;
+    p.rayCounter = ctx->dRayCounters;
+    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    p.rays = dRays;
+    p.numRays = (uint32_t)n;
+    cudaError_t e = launch_fast_aovs(p, scene, true, dAlbedo, dNormal, dIds, ctx->numSMs, stream);
+    if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+    ctx->lastLaunches += 1;
+    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
+    if (!outOnDevice)
+    {
+        if (albedo4) CK(cudaMemcpyAsync(albedo4, dAlbedo, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H albedo4");
+        if (normal4) CK(cudaMemcpyAsync(normal4, dNormal, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H normal4");
+        if (ids) CK(cudaMemcpyAsync(ids, dIds, (size_t)n * 4, cudaMemcpyDeviceToHost, stream), "D2H ids");
+    }
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
 }
 

@@ -82,6 +82,14 @@ __device__ __forceinline__ Ray fast_get_ray(const Camera88& c, float s, float t,
     r.dir = M<false>::normalize(ld3(c.lowerLeftCorner) + s * ld3(c.horizontal) + t * ld3(c.vertical) - ld3(c.origin) - offset);
     return r;
 }
+// The camera ray of one fast-mode sample of pixel (x, y), drawn from the sample's stream: the pixel jitter, then the lens
+// sample (Test.cpp:286-288 + Maths.h:437-442). The image kernels and the AOV pass build their primary rays with it.
+__device__ __forceinline__ Ray fast_camera_ray(const DrawParams& p, int x, int y, uint32_t& rng)
+{
+    float u = ((float)x + RandomFloat01(rng)) * p.invWidth;
+    float v = ((float)y + RandomFloat01(rng)) * p.invHeight;
+    return fast_get_ray(p.cam, u, v, rng);
+}
 
 __device__ __forceinline__ void blend_weights(const DrawParams& p, float* w, float& wPrev)
 {
@@ -141,9 +149,7 @@ k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             V3 col = v3(0, 0, 0);
             for (int s = 0; s < p.spp; ++s)
             {
-                float u = ((float)x + RandomFloat01(state)) * p.invWidth;
-                float v = ((float)y + RandomFloat01(state)) * p.invHeight;
-                Ray r = fast_get_ray(p.cam, u, v, state);
+                Ray r = fast_camera_ray(p, x, y, state);
                 col = col + trace_fast(sc, r, state, rc, hitter);
             }
             acc = acc + col * (invSpp * sW[fi]);
@@ -233,9 +239,7 @@ k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlo
                         const int y = p.row0 + ri * p.rowStep;
                         st.rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + (uint32_t)(sIdx % p.spp),
                                             (uint32_t)(p.frame0 + fi));
-                        float u = ((float)x + RandomFloat01(st.rng)) * p.invWidth;
-                        float v = ((float)y + RandomFloat01(st.rng)) * p.invHeight;
-                        Ray r = fast_get_ray(p.cam, u, v, st.rng);
+                        Ray r = fast_camera_ray(p, x, y, st.rng);
                         st.o = r.orig; st.d = r.dir;
                         st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
                         st.pix = pixIn; st.weight = invSpp * sW[fi];
@@ -418,9 +422,7 @@ __device__ __forceinline__ void generate_slab_rays(const DrawParams& p, float4 (
         while (x >= p.width) { x -= p.width; ++ri; }
         const int y = p.row0 + ri * p.rowStep;
         uint32_t rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + sample, frame);
-        float u = ((float)x + RandomFloat01(rng)) * p.invWidth;
-        float v = ((float)y + RandomFloat01(rng)) * p.invHeight;
-        Ray r = fast_get_ray(p.cam, u, v, rng);
+        Ray r = fast_camera_ray(p, x, y, rng);
         const uint32_t tag = tileBase < 0 ? (uint32_t)((p.packed ? ri : y) * p.width + x) : (uint32_t)tileBase + q;
         rays[q][0] = make_float4(r.orig.x, r.orig.y, r.orig.z, __uint_as_float(rng));
         rays[q][1] = make_float4(r.dir.x, r.dir.y, r.dir.z, __uint_as_float(tag));
@@ -1193,9 +1195,7 @@ __device__ __forceinline__ void generate_group_rays(const DrawParams& p, float4 
         const int y = p.row0 + ri * p.rowStep;
         const uint32_t s = s0 + sl, fi = s / (uint32_t)p.spp, ss = s - fi * (uint32_t)p.spp;
         uint32_t rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + ss, (uint32_t)p.frame0 + fi);
-        float u = ((float)x + RandomFloat01(rng)) * p.invWidth;
-        float v = ((float)y + RandomFloat01(rng)) * p.invHeight;
-        Ray r = fast_get_ray(p.cam, u, v, rng);
+        Ray r = fast_camera_ray(p, x, y, rng);
         rays[q][0] = make_float4(r.orig.x, r.orig.y, r.orig.z, __uint_as_float(rng));
         rays[q][1] = make_float4(r.dir.x, r.dir.y, r.dir.z, __uint_as_float(px | (slot << 4) | (fi << 8)));
     }
@@ -1975,6 +1975,140 @@ cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs
 {
     const QueuePick q = pick_queue<true>(sc, 3, p.numRays, p.spp, numSMs);
     return launch_queue<true>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
+}
+
+// ---- first-hit AOVs (tpt_draw_aovs, tpt_trace_aovs) ----------------------------------------------------------------
+// One nearest-hit sweep per sample and no shading: per pixel (or caller ray) albedo4 = (albedo.rgb, coverage) and
+// normal4 = (normal.xyz, depth) of the primary hits, ids = the sphere id of sample 0. Persistent CTAs stage the scene as
+// k_debug_hit does (blob + pair array, no ray buffers: every scene the slab queue stages fits); a warp pulls 32
+// consecutive pixels or rays from the work counter and each lane owns one of them for all its samples, so every lane does
+// exactly one sweep per sample and the warp stays converged. A pixel's result depends on its own samples only: the output
+// is bitwise the same for any grid size or row sharding.
+// RAYS = false: the draw's pixels y = row0 + i * rowStep; sample s of frame f uses the fast draw's camera ray
+//   (pixel_seed((y * width + x) * spp + s, f), fast_camera_ray), frames blended like the image with prev * wPrev.
+// RAYS = true: p.numRays caller rays {o.xyz, d.xyz}, loaded and normalised as load_slab_rays does; untraceable rays give
+//   zeros and id -1 and are not counted.
+constexpr int kAovThreads = 256, kAovMinBlocks = 3;     // <= 85 registers: three CTAs (24 warps) per SM for scenes that leave the shared memory to them
+
+struct AovSample { V3 albedo, normal; float cov, t; };
+
+template <class Hitter>
+__device__ __forceinline__ int aov_sample(const SceneView& sc, const Hitter& hitter, V3 o, V3 d, AovSample& a)
+{
+    float t = TPT_MAX_T;
+    const int id = hitter.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
+    if (id < 0) { a.albedo = v3(0, 0, 0); a.normal = v3(0, 0, 0); a.cov = 0.0f; a.t = 0.0f; return id; }
+    const Q4 s = ld_sph(sc, id);
+    const V3 pos = o + d * t;
+    a.normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];     // path_step's normal: not flipped, not renormalised
+    const Q4 m = sc.matA[id < sc.count ? id : sc.count];         // a padded sphere (form 0) has the all-zero material
+    a.albedo = v3(m.x, m.y, m.z);
+    a.cov = 1.0f; a.t = t;
+    return id;
+}
+
+template <bool RAYS, int KFORM>
+__global__ void __launch_bounds__(kAovThreads, kAovMinBlocks)
+k_fast_aov(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes,
+           uint32_t numChunks, float wPrev, float* __restrict__ albedo4, float* __restrict__ normal4, int* __restrict__ ids)
+{
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ uint64_t bar;
+    __shared__ float sW[kMaxFramesPerDraw];
+    stage_blob(smem, blob, stagedBytes, &bar);
+    if (!RAYS && threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); }
+    SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);     // (its barrier also publishes sW)
+    const int lane = threadIdx.x & 31;
+    const uint32_t n = RAYS ? p.numRays : (uint32_t)p.numRows * (uint32_t)p.width;
+    const float invSpp = 1.0f / (float)p.spp;
+    unsigned rc = 0;
+    for (;;)
+    {
+        uint32_t chunk = 0;
+        if (lane == 0) chunk = atomicAdd(p.workCounter, 1u);
+        chunk = __shfl_sync(0xffffffffu, chunk, 0);
+        if (chunk >= numChunks) break;
+        const uint32_t i = chunk * 32u + (uint32_t)lane;
+        if (i >= n) continue;
+        AovSample acc{v3(0, 0, 0), v3(0, 0, 0), 0.0f, 0.0f};
+        int id0 = -1;
+        size_t off = i;
+        if constexpr (RAYS)
+        {
+            const float* r = p.rays + (size_t)i * 6;
+            const V3 o = v3(__ldg(r), __ldg(r + 1), __ldg(r + 2));
+            const V3 d = M<false>::normalize(v3(__ldg(r + 3), __ldg(r + 4), __ldg(r + 5)));
+            const bool ok = isfinite(o.x) && isfinite(o.y) && isfinite(o.z) && isfinite(d.x) && isfinite(d.y) && isfinite(d.z) &&
+                            (d.x != 0.0f || d.y != 0.0f || d.z != 0.0f);
+            if (ok) { id0 = aov_sample(sc, hitter, o, d, acc); ++rc; }
+        }
+        else
+        {
+            const int ri = (int)(i / (uint32_t)p.width), x = (int)(i - (uint32_t)ri * (uint32_t)p.width);
+            const int y = p.row0 + ri * p.rowStep;
+            for (int fi = 0; fi < p.numFrames; ++fi)
+            {
+                AovSample fs{v3(0, 0, 0), v3(0, 0, 0), 0.0f, 0.0f};
+                for (int s = 0; s < p.spp; ++s)
+                {
+                    uint32_t rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + (uint32_t)s, (uint32_t)(p.frame0 + fi));
+                    const Ray r = fast_camera_ray(p, x, y, rng);
+                    AovSample a;
+                    const int id = aov_sample(sc, hitter, r.orig, r.dir, a);
+                    if (fi == 0 && s == 0) id0 = id;
+                    fs.albedo = fs.albedo + a.albedo; fs.normal = fs.normal + a.normal; fs.cov += a.cov; fs.t += a.t;
+                }
+                rc += (unsigned)p.spp;
+                const float w = invSpp * sW[fi];
+                acc.albedo = acc.albedo + fs.albedo * w; acc.normal = acc.normal + fs.normal * w;
+                acc.cov += fs.cov * w; acc.t += fs.t * w;
+            }
+            off = (size_t)(p.packed ? ri : y) * p.width + x;
+        }
+        float4 va = make_float4(acc.albedo.x, acc.albedo.y, acc.albedo.z, acc.cov);
+        float4 vn = make_float4(acc.normal.x, acc.normal.y, acc.normal.z, acc.t);
+        // out = prev * wPrev + sum_f w_f mean_f, all four components; a zero weight does not read prev (NaN * 0)
+        if (albedo4)
+        {
+            if (!RAYS && wPrev != 0.0f)
+            {
+                const float4 q = ld_stream_f4(albedo4 + off * 4);
+                va = make_float4(fmaf(q.x, wPrev, va.x), fmaf(q.y, wPrev, va.y), fmaf(q.z, wPrev, va.z), fmaf(q.w, wPrev, va.w));
+            }
+            *reinterpret_cast<float4*>(albedo4 + off * 4) = va;
+        }
+        if (normal4)
+        {
+            if (!RAYS && wPrev != 0.0f)
+            {
+                const float4 q = ld_stream_f4(normal4 + off * 4);
+                vn = make_float4(fmaf(q.x, wPrev, vn.x), fmaf(q.y, wPrev, vn.y), fmaf(q.z, wPrev, vn.z), fmaf(q.w, wPrev, vn.w));
+            }
+            *reinterpret_cast<float4*>(normal4 + off * 4) = vn;
+        }
+        if (ids) ids[off] = id0;
+    }
+    flush_ray_count(p.rayCounter, rc, lane);
+}
+
+cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays, float* albedo4, float* normal4, int* ids,
+                             int numSMs, cudaStream_t stream)
+{
+    if (!rays && p.numFrames > kMaxFramesPerDraw) return cudaErrorInvalidValue;
+    const int kform = fast_queue_kform(sc);
+    auto kern = rays ? for_kform<3>(kform, [](auto K) { return k_fast_aov<true, decltype(K)::value>; })
+                     : for_kform<3>(kform, [](auto K) { return k_fast_aov<false, decltype(K)::value>; });
+    // [staged blob | pair array (forms 2/3)], nothing behind it
+    const size_t dyn = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0).buffers;
+    const long long n = rays ? (long long)p.numRays : (long long)p.numRows * p.width;
+    const long long chunks = (n + 31) / 32;
+    long long grid = 0;
+    cudaError_t e = persistent_grid(kern, kAovThreads, dyn, numSMs, (chunks + kAovThreads / 32 - 1) / (kAovThreads / 32), p, stream, grid);
+    if (e != cudaSuccess) return e;
+    kern<<<(unsigned)grid, kAovThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, (uint32_t)chunks,
+                                                       rays ? 0.0f : prev_weight(p.frame0, p.numFrames, p.flags), albedo4, normal4, ids);
+    return cudaGetLastError();
 }
 
 int fast_slab_pixels() { return kSlabPix; }

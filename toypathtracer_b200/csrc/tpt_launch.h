@@ -36,6 +36,11 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
 // pixel_seed(ray * spp + sample, p.frame0), mean written to the float4 p.image[ray] (zeroed first); p.numFrames = 1, p.flags = 0.
 // Runs the slab-queue instance variant 3 would run for the scene.
 cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
+// tpt_draw_aovs (rays = false: the region of p, frames [p.frame0, p.frame0 + p.numFrames) at p.spp, blended over the outputs
+// with the weight of `prev`) and tpt_trace_aovs (rays = true: p.numRays >= 1 caller rays p.rays): first-hit albedo4,
+// normal4 and ids (each may be null) with the slab queue's sweep form, one ray counted per traced sample.
+cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays, float* albedo4, float* normal4, int* ids,
+                             int numSMs, cudaStream_t stream);
 // TPT_MODE_REFGPU (tpt_refgpu.cuh): strict arithmetic (tpt_exact.cu) / GPU-native arithmetic (tpt_fast.cu)
 cudaError_t launch_refgpu_exact(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 cudaError_t launch_refgpu_fast(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
