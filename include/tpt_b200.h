@@ -190,6 +190,35 @@ int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
                    float* albedo4, float* normal4, int* ids, int outOnDevice,
                    long long* outRayCount, void* cudaStream);
 
+/* Per-pixel sample sums and second moments of the fast draw's own samples, for all pixels or a caller-listed subset: what
+ * adaptive sampling needs (learn how noisy each pixel is, then trace more samples for the noisy ones only).
+ *   pixels            n linear pixel indices y * width + x (row 0 = bottom) of a width x height image; duplicates and any
+ *                     order are allowed. NULL = every pixel 0 .. width * height - 1, and then n must be width * height.
+ *   spp               samples per listed entry. Sample s of pixel p is exactly the fast draw's: stream
+ *                     pixel_seed(p * spp + s, frame), pixel jitter and lens sample (fast_camera_ray), then the estimator of
+ *                     TPT_MODE_FAST with the scene options of a fast draw ("light_sampling", "mitsuba_compare",
+ *                     "fast_kform", scenes past 64 KB of blob). So one call with pixels = NULL and the context's spp traces
+ *                     the samples of tpt_draw(frame, 1, ..., TPT_MODE_FAST) at zero `prev` weight, and calls with frame + 1,
+ *                     frame + 2, ... give independent further samples. width * height * spp must not exceed 2^32.
+ *   sum4              n float4, ACCUMULATED: entry i receives += (sum r, sum g, sum b, spp) over its samples. Zero it once,
+ *                     then add calls; mean = sum.rgb / sum.w.
+ *   sq4               NULL, or n float4 accumulated as += (sum r^2, sum g^2, sum b^2, 0): with sum4 it gives the unbiased
+ *                     per-pixel variance (sq - sum^2 / w) / (w - 1) over any number of calls.
+ *   buffersOnDevice   0: host pointers, staged through the context (sum4 and sq4 are uploaded, since the call adds to
+ *                     them) and the call is synchronous; 1: device pointers of the context's device (or mapped host
+ *                     memory), pixels 4-byte and sum4 / sq4 16-byte aligned.
+ *   outRayCount       NULL or receives the number of rays traced (path and shadow rays).
+ * An index outside [0, width * height) is found on the device before anything is traced: the call then traces nothing,
+ * adds nothing and fails, tpt_last_error naming the first such entry. A call with a pixel list is therefore synchronous;
+ * one with pixels = NULL and device buffers synchronises only when a ray count is requested. n == 0 (an empty list, so
+ * pixels and sum4 must still be non-NULL) launches nothing and reads no buffer.
+ * Ordering and accounting are those of tpt_draw. NULL sum4, n < 0, spp < 1, width * height * spp > 2^32, a misaligned
+ * device buffer or one on another device are refused (tpt_last_error gives the reason). */
+int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
+                     const int* pixels, long long n, int spp,
+                     float* sum4, float* sq4, int buffersOnDevice,
+                     long long* outRayCount, void* cudaStream);
+
 /* Rays traced by all draws since the last call of this function (synchronises the stream). */
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStream, long long* outRays);
 /* Device time (CUDA events on the launching stream) of the kernels of the most recent tpt_draw, in ms. */

@@ -79,6 +79,8 @@ def _load_lib():
     L.tpt_draw_aovs.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, ci, cu, ctypes.POINTER(cll), vp]
     L.tpt_draw_aovs.restype = ci
     L.tpt_trace_aovs.argtypes = [vp, vp, ci, cll, vp, vp, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_aovs.restype = ci
+    L.tpt_draw_samples.argtypes = [vp, ci, ci, ci, vp, cll, ci, vp, vp, ci, ctypes.POINTER(cll), vp]
+    L.tpt_draw_samples.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -140,6 +142,54 @@ def _aov_ptrs(what: str, albedo, normal, ids, pixels: int):
     return ptrs, kinds.pop(), keep
 
 
+_CUDA_STREAM_LEGACY = 1            # cudaStreamLegacy: torch's default stream, whose handle reads as 0
+_NO_ENTRIES = (ctypes.c_int * 1)()  # the address draw_samples passes for an empty pixel list
+
+
+def _cuda_device(*bufs):
+    """The device of the first CUDA torch tensor among bufs, or None."""
+    for b in bufs:
+        if getattr(b, "is_cuda", False):
+            return b.device
+    return None
+
+
+def _torch_stream(dev) -> int:
+    """Handle of torch's current stream on `dev` for the library's cudaStream argument (0 would mean the context's own
+    stream, so torch's legacy default stream is passed as cudaStreamLegacy)."""
+    import torch
+    return torch.cuda.current_stream(dev).cuda_stream or _CUDA_STREAM_LEGACY
+
+
+LUMA = (0.2126, 0.7152, 0.0722)    # Rec. 709 luminance weights of the adaptive stopping rule
+
+
+def adaptive_pixels(sum4, sq4, rel_err: float, max_spp: int, shape: Optional[Tuple[int, int]] = None):
+    """The stopping rule of Context.render_adaptive, on torch tensors of draw_samples sums (N, 4) and squares (N, 4):
+    the int32 indices of the pixels that have fewer than max_spp samples and whose standard error of the mean luminance
+    exceeds rel_err * (mean luminance + 0.05). Per channel the variance is the unbiased sample variance
+    (sq - sum^2 / n) / (n - 1); the moments hold no covariances between channels, so the luminance's standard error is
+    taken as sum_c LUMA_c * se_c, an upper bound that is exact when the channels' noise is fully correlated (a path's
+    colour mostly scales as one). A pixel with one sample has no variance estimate and is always picked.
+    With shape = (height, width) (the sums of a whole image, row-major) the picked set is grown by the 3 x 3
+    neighbourhood of every picked pixel. A few samples cannot see a rare event: a pixel on the edge of a light's mirror
+    image whose first 4 samples all hit (or all missed) the light has a zero sample variance and would stop with a
+    wrong value; its neighbours across the edge are noisy, and the dilation refines it with them."""
+    import torch
+    cnt = sum4[:, 3]
+    n = cnt.clamp(min=2.0).unsqueeze(1)
+    mean = sum4[:, :3] / n
+    var = ((sq4[:, :3] - sum4[:, :3] * mean) / (n - 1.0)).clamp(min=0.0)
+    w = torch.tensor(LUMA, dtype=sum4.dtype, device=sum4.device)
+    se = (var / n).sqrt() @ w
+    lum = (sum4[:, :3] / cnt.clamp(min=1.0).unsqueeze(1)) @ w
+    noisy = (se > rel_err * (lum + 0.05)) | (cnt < 2)
+    if shape is not None:
+        grown = torch.nn.functional.max_pool2d(noisy.view(1, 1, *shape).to(torch.float32), 3, stride=1, padding=1)
+        noisy = grown.view(-1) > 0
+    return ((cnt < max_spp) & noisy).nonzero().squeeze(1).to(torch.int32)
+
+
 class Context:
     """One CUDA device's renderer state (scene blob, scratch, counters): ``tpt_context`` of include/tpt_b200.h."""
 
@@ -153,6 +203,7 @@ class Context:
         self._h = h
         self.device = device
         self.count = 0
+        self.spp = 4          # the library's default, kept in step by set_spp
 
     def close(self):
         if getattr(self, "_h", None) is not None and self._h.value:
@@ -192,6 +243,7 @@ class Context:
 
     def set_spp(self, spp: int):
         self._check(self._L.tpt_set_spp(self._h, spp), "tpt_set_spp")
+        self.spp = int(spp)
 
     def set_option(self, key: str, value: int):
         self._check(self._L.tpt_set_option(self._h, key.encode(), int(value)), f"tpt_set_option({key})")
@@ -296,6 +348,114 @@ class Context:
                                     ctypes.byref(total) if want_rays else None, ctypes.c_void_p(stream) if stream else None)
         self._check(rc, "tpt_trace_aovs")
         return ((albedo, normal, ids), int(total.value)) if want_rays else (albedo, normal, ids)
+
+    def draw_samples(self, frame: int, width: int, height: int, pixels=None, spp: Optional[int] = None, sum4=None,
+                     sq4=None, stream: int = 0, want_rays: bool = True, n=None):
+        """tpt_draw_samples: `spp` more samples (default: the context's spp) of the fast draw of a width x height image for
+        each entry of `pixels` — linear indices y * width + x, int32, duplicates and any order allowed; None = every
+        pixel — ADDED to sum4 (sum r, g, b, sample count) and, when given, sq4 (sum r^2, g^2, b^2, 0), both (N, 4) float32.
+        Sample s of pixel p at `frame` is the draw's own (stream pixel_seed(p * spp + s, frame)), so an all-pixel call at
+        the context's spp traces tpt_draw(frame, 1, ..., MODE_FAST)'s samples and frames frame + 1, frame + 2, ... add
+        independent ones. Buffers are numpy arrays, torch tensors (CPU or CUDA) or DevicePtr (a DevicePtr list needs
+        `n`), all host or all device. Without sum4 and sq4 both are allocated zeroed, of the kind of `pixels` (a CUDA
+        tensor on the context's device for pixels=None or a DevicePtr). When any buffer is a CUDA tensor (allocated ones
+        included) and `stream` is 0, the call runs on torch's current stream of that device, so it is ordered with the
+        torch work around it; outputs allocated for an explicit `stream` are zeroed on that stream. Returns
+        ((sum4, sq4), rays traced), or the pair alone when want_rays is False. A call with a pixel list is synchronous."""
+        numpix = int(width) * int(height)
+        spp = self.spp if spp is None else int(spp)
+        if pixels is None:
+            if n is not None and int(n) != numpix:
+                raise TptError("draw_samples: without pixels n must be width * height")
+            n, paddr, pon, kind = numpix, None, None, None
+        elif isinstance(pixels, DevicePtr):
+            if n is None:
+                raise TptError("draw_samples: a DevicePtr needs n")
+            paddr, pon, kind = pixels.addr, True, None
+        else:
+            if len(pixels.shape) != 1:
+                raise TptError("draw_samples: pixels must have shape (N,)")
+            if n is not None and int(n) != pixels.shape[0]:
+                raise TptError("draw_samples: n does not match pixels")
+            n = pixels.shape[0]
+            paddr, pon, _keep = _as_ptr(pixels, "int32")
+            kind = pixels
+        n = int(n)
+        if n < 0:
+            raise TptError("draw_samples: n < 0")
+        if sum4 is None and sq4 is not None:
+            raise TptError("draw_samples: sq4 needs sum4")
+        alloc_dev = None
+        if sum4 is None:
+            if isinstance(kind, np.ndarray):
+                sum4, sq4 = np.zeros((n, 4), np.float32), np.zeros((n, 4), np.float32)
+            else:
+                import torch
+                alloc_dev = kind.device if kind is not None else torch.device("cuda", self.device)
+        # Torch CUDA tensors are written and read on torch's streams, which the library does not know: without an
+        # explicit stream the call runs on torch's current stream of their device, after the torch work that filled
+        # them (and the zeroing of outputs allocated here) and before the torch work that reads the sums.
+        tdev = _cuda_device(pixels, sum4, sq4) or (alloc_dev if alloc_dev is not None and alloc_dev.type == "cuda" else None)
+        explicit = bool(stream)
+        if tdev is not None and not explicit:
+            stream = _torch_stream(tdev)
+        if alloc_dev is not None:
+            import contextlib
+            import torch
+            # outputs for an explicit stream are zeroed on it, so the call cannot overtake the fill
+            other = explicit and alloc_dev.type == "cuda" and stream != _torch_stream(alloc_dev)
+            on = torch.cuda.stream(torch.cuda.ExternalStream(stream, device=alloc_dev)) if other else contextlib.nullcontext()
+            with on:
+                sum4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
+                sq4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
+        # empty buffers have no data pointer; the library reads none of an empty list's, but NULL means "no list"
+        if paddr == 0 and n == 0:
+            paddr = ctypes.addressof(_NO_ENTRIES)
+        ptrs, kinds, keep = [], set() if pon is None else {pon}, []
+        for name, buf in (("sum4", sum4), ("sq4", sq4)):
+            if buf is None:
+                ptrs.append(None)
+                continue
+            if not isinstance(buf, DevicePtr) and _numel(buf) != n * 4:
+                raise TptError(f"draw_samples: {name} must hold {n} x 4 float32 values, not {_numel(buf)}")
+            addr, on_dev, k = _as_ptr(buf)
+            if addr == 0 and n == 0:
+                addr = ctypes.addressof(_NO_ENTRIES)
+            ptrs.append(ctypes.c_void_p(addr)); kinds.add(on_dev); keep.append(k)
+        if len(kinds) > 1:
+            raise TptError("draw_samples: pixels, sum4 and sq4 must be all host or all device buffers")
+        total = ctypes.c_longlong(0)
+        rc = self._L.tpt_draw_samples(self._h, int(frame), int(width), int(height),
+                                      None if paddr is None else ctypes.c_void_p(paddr), n, spp, ptrs[0], ptrs[1],
+                                      1 if kinds.pop() else 0, ctypes.byref(total) if want_rays else None,
+                                      ctypes.c_void_p(stream) if stream else None)
+        self._check(rc, "tpt_draw_samples")
+        return ((sum4, sq4), int(total.value)) if want_rays else (sum4, sq4)
+
+    def render_adaptive(self, width: int, height: int, base_spp: int = 4, max_spp: int = 64, rel_err: float = 0.05,
+                        frame: int = 0):
+        """Adaptive fast-mode render on the device: one draw_samples pass over every pixel at base_spp (frame `frame`),
+        then rounds at frames frame + 1, frame + 2, ... that give base_spp more samples to the pixels adaptive_pixels
+        picks, until it picks none or every pixel has max_spp. Returns (image float32 [h, w, 4] with alpha 0, samples
+        per pixel int32 [h, w], rays traced), all but the ray count CUDA tensors on the context's device. Every step —
+        the library calls, the rule, the index conversion and the scatter of the sums — runs on torch's current stream."""
+        import torch
+        if base_spp < 1 or max_spp < base_spp:
+            raise TptError("render_adaptive: need 1 <= base_spp <= max_spp")
+        dev = torch.device("cuda", self.device)
+        # every buffer is a CUDA tensor, so each draw_samples call runs on torch's current stream
+        (s, q), rays = self.draw_samples(frame, width, height, None, base_spp)
+        for f in range(frame + 1, frame + 1 + (max_spp - base_spp) // base_spp):
+            idx = adaptive_pixels(s, q, rel_err, max_spp, (height, width))
+            if idx.numel() == 0:
+                break
+            (ds, dq), r = self.draw_samples(f, width, height, idx, base_spp)
+            s.index_add_(0, idx.long(), ds)
+            q.index_add_(0, idx.long(), dq)
+            rays += r
+        image = torch.zeros((height, width, 4), dtype=torch.float32, device=dev)
+        image.view(-1, 4)[:, :3] = s[:, :3] / s[:, 3:]
+        return image, s[:, 3].round().to(torch.int32).view(height, width), rays
 
     def read_ray_count(self, stream: int = 0) -> int:
         out = ctypes.c_longlong(0)

@@ -79,6 +79,10 @@ struct tpt_context
     float* dAovAlbedo = nullptr; size_t aovAlbedoCap = 0;   // staging of host AOV outputs (tpt_draw_aovs, tpt_trace_aovs)
     float* dAovNormal = nullptr; size_t aovNormalCap = 0;
     int* dAovIds = nullptr; size_t aovIdsCap = 0;
+    int* dPixels = nullptr; size_t pixelsCap = 0;      // staging of host tpt_draw_samples lists (sum4 goes through dImage)
+    float* dSq4 = nullptr; size_t sq4Cap = 0;
+    unsigned long long* dBadPixel = nullptr;           // tpt_draw_samples' index check, and its page-locked copy
+    unsigned long long* hBadPixel = nullptr;
     float* dScratch = nullptr; size_t scratchCap = 0;  // exact mode per-frame colours
     unsigned long long* dRayCounters = nullptr; int rayCounterCap = 0;   // [numFrames]
     unsigned long long* dAccum = nullptr;              // [0] total since last read, [1] last draw total
@@ -230,7 +234,7 @@ void tpt_destroy(tpt_context* ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->registeredPtr) cudaHostUnregister(ctx->registeredPtr);
-    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dAovAlbedo); cudaFree(ctx->dAovNormal); cudaFree(ctx->dAovIds); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
+    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dAovAlbedo); cudaFree(ctx->dAovNormal); cudaFree(ctx->dAovIds); cudaFree(ctx->dPixels); cudaFree(ctx->dSq4); cudaFree(ctx->dBadPixel); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
     cudaFree(ctx->dAccum); cudaFree(ctx->dWork);
     for (int i = 0; i < 2; ++i)
     {
@@ -244,6 +248,7 @@ void tpt_destroy(tpt_context* ctx)
     if (ctx->tlKernelEnd) cudaEventDestroy(ctx->tlKernelEnd);
     for (int b = 0; b < 16; ++b) if (ctx->tlBand[b]) cudaEventDestroy(ctx->tlBand[b]);
     if (ctx->hPinned) cudaFreeHost(ctx->hPinned);
+    if (ctx->hBadPixel) cudaFreeHost(ctx->hBadPixel);
     for (int b = 0; b < tpt_context::kMaxBands; ++b)
     {
         if (ctx->bandStream[b]) cudaStreamDestroy(ctx->bandStream[b]);
@@ -967,6 +972,108 @@ int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
         if (ids) CK(cudaMemcpyAsync(ids, dIds, (size_t)n * 4, cudaMemcpyDeviceToHost, stream), "D2H ids");
     }
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
+}
+
+int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
+                     const int* pixels, long long n, int spp,
+                     float* sum4, float* sq4, int buffersOnDevice,
+                     long long* outRayCount, void* cudaStreamArg)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!ctx->haveScene) return fail_msg(ctx, "tpt_draw_samples: no scene (call tpt_set_scene first)");
+    if (width <= 0 || height <= 0 || frame < 0) return fail_msg(ctx, "tpt_draw_samples: bad arguments");
+    if (n < 0) return fail_msg(ctx, "tpt_draw_samples: n < 0");
+    if (spp < 1) return fail_msg(ctx, "tpt_draw_samples: spp < 1");
+    // the sample stream of (pixel p, sample s) is p * spp + s in 32 bits
+    const long long numPix = (long long)width * height;
+    if (numPix > (1LL << 32) / spp) return fail_msg(ctx, "tpt_draw_samples: width * height * spp > 2^32 (32-bit sample streams)");
+    if (!sum4) return fail_msg(ctx, "tpt_draw_samples: null sum4");
+    if (!pixels && n != numPix) return fail_msg(ctx, "tpt_draw_samples: without a pixel list n must be width * height");
+    if (n == 0)
+    {
+        // an empty list: nothing to trace, no buffer is read
+        if (outRayCount) *outRayCount = 0;
+        ctx->lastLaunches = 0;
+        return 0;
+    }
+    const long long slab = fast_slab_pixels();
+    if (n > 0xffffffffLL || (n + slab - 1) / slab * spp > 0x7fffffffLL)
+        return fail_msg(ctx, "tpt_draw_samples: n * spp too large (2^31 slabs of 64 entries x one sample)");
+    if (buffersOnDevice)
+    {
+        if (pixels && ((uintptr_t)pixels & 3)) return fail_msg(ctx, "tpt_draw_samples: device pixels is not 4-byte aligned");
+        if ((uintptr_t)sum4 & 15) return fail_msg(ctx, "tpt_draw_samples: device sum4 is not 16-byte aligned");
+        if (sq4 && ((uintptr_t)sq4 & 15)) return fail_msg(ctx, "tpt_draw_samples: device sq4 is not 16-byte aligned");
+        if (pixels) { if (int r = check_device_buffer(ctx, pixels, "pixels", "tpt_draw_samples")) return r; }
+        if (int r = check_device_buffer(ctx, sum4, "sum4", "tpt_draw_samples")) return r;
+        if (sq4) { if (int r = check_device_buffer(ctx, sq4, "sq4", "tpt_draw_samples")) return r; }
+    }
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+    if (pixels && !ctx->dBadPixel)
+    {
+        CK(cudaMalloc(&ctx->dBadPixel, sizeof(unsigned long long)), "cudaMalloc index check");
+        CK(cudaMallocHost(&ctx->hBadPixel, sizeof(unsigned long long)), "cudaMallocHost index check");
+    }
+    const int* dPixels = pixels;
+    float* dSum = sum4;
+    float* dSq = sq4;
+    if (!buffersOnDevice)
+    {
+        // the outputs accumulate: host sums go up and come back
+        if (pixels)
+        {
+            if (int r = ensure(ctx, (void**)&ctx->dPixels, &ctx->pixelsCap, (size_t)n * 4, "cudaMalloc pixels")) return r;
+            CK(cudaMemcpyAsync(ctx->dPixels, pixels, (size_t)n * 4, cudaMemcpyHostToDevice, stream), "H2D pixels");
+            dPixels = ctx->dPixels;
+        }
+        if (int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, (size_t)n * 16, "cudaMalloc sum4")) return r;
+        CK(cudaMemcpyAsync(ctx->dImage, sum4, (size_t)n * 16, cudaMemcpyHostToDevice, stream), "H2D sum4");
+        dSum = ctx->dImage;
+        if (sq4)
+        {
+            if (int r = ensure(ctx, (void**)&ctx->dSq4, &ctx->sq4Cap, (size_t)n * 16, "cudaMalloc sq4")) return r;
+            CK(cudaMemcpyAsync(ctx->dSq4, sq4, (size_t)n * 16, cudaMemcpyHostToDevice, stream), "H2D sq4");
+            dSq = ctx->dSq4;
+        }
+    }
+    if (int r = start_kernels(ctx, stream, 1)) return r;
+    DrawParams p;
+    memset(&p, 0, sizeof(p));
+    p.cam = ctx->cam;
+    p.width = width; p.height = height;
+    p.row0 = 0; p.numRows = height; p.rowStep = 1;
+    p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
+    p.spp = spp;
+    p.invWidth = 1.0f / (float)width;
+    p.invHeight = 1.0f / (float)height;
+    p.image = dSum;
+    p.sq4 = dSq;
+    p.pixels = dPixels;
+    p.numRays = (uint32_t)n;
+    p.rayCounter = ctx->dRayCounters;
+    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    cudaError_t e = launch_fast_samples(p, scene, ctx->dBadPixel, ctx->numSMs, stream);
+    if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+    ctx->lastLaunches += fast_samples_launches(p);
+    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
+    if (pixels) CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream), "D2H index check");
+    if (!buffersOnDevice)
+    {
+        CK(cudaMemcpyAsync(sum4, dSum, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H sum4");
+        if (sq4) CK(cudaMemcpyAsync(sq4, dSq, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H sq4");
+    }
+    // a pixel list makes the call synchronous: its index check is the call's result
+    if (int r = finish_call(ctx, stream, 1, !buffersOnDevice || pixels, outRayCount, nullptr)) return r;
+    if (pixels && *ctx->hBadPixel != ~0ull)
+    {
+        char msg[200];
+        snprintf(msg, sizeof(msg), "tpt_draw_samples: pixels[%llu] = %d is outside the %d x %d image (nothing was traced)",
+                 *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, width, height);
+        return fail_msg(ctx, msg);
+    }
+    return 0;
 }
 
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStreamArg, long long* outRays)

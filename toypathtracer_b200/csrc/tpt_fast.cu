@@ -405,9 +405,9 @@ __global__ void k_prepare_image(DrawParams p, float wPrev)
     *reinterpret_cast<float4*>(px) = v;   // stays in L2 for the reductions that follow
 }
 
-__device__ __forceinline__ void red_add_f4(float* addr, float x, float y, float z)
+__device__ __forceinline__ void red_add_f4(float* addr, float x, float y, float z, float w = 0.0f)
 {
-    asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(addr), "f"(x), "f"(y), "f"(z), "f"(0.0f) : "memory");
+    asm volatile("red.global.add.v4.f32 [%0], {%1,%2,%3,%4};" ::"l"(addr), "f"(x), "f"(y), "f"(z), "f"(w) : "memory");
 }
 
 // Camera rays of one slab (<= kSlabPix consecutive pixels of the region, one sample index), generated by the whole warp
@@ -471,6 +471,27 @@ __device__ __forceinline__ uint32_t load_slab_rays(const DrawParams& p, float4 (
         base += (uint32_t)__popc(m);
     }
     return base;
+}
+
+// Camera rays of one slab of a pixel list (tpt_draw_samples): entries [e0, e0 + count) of p.pixels, count <= kSlabPix, or
+// the pixels e0, e0 + 1, ... when p.pixels is null. Each pass of the warp reads 32 consecutive indices (one coalesced
+// 128-byte row, two for a full slab) and builds each entry's ray exactly as generate_slab_rays builds the draw's ray for
+// that pixel and sample: stream pixel_seed(pixel * spp + sample, frame), then fast_camera_ray. Tag = the entry index. The
+// indices were checked against the image before the launch (k_check_pixels). (Loading both rows before generating the
+// rays kept two more values live and made the 64-register instance spill 68 B instead of 8.)
+__device__ __forceinline__ void generate_list_rays(const DrawParams& p, float4 (*rays)[2], int lane, uint32_t count,
+                                                   uint32_t e0, uint32_t sample, uint32_t frame)
+{
+    for (uint32_t q = (uint32_t)lane; q < count; q += 32)
+    {
+        const uint32_t pix = p.pixels ? (uint32_t)__ldg(p.pixels + e0 + q) : e0 + q;
+        const int y = (int)(pix / (uint32_t)p.width);
+        const int x = (int)(pix - (uint32_t)y * (uint32_t)p.width);
+        uint32_t rng = pixel_seed(pix * (uint32_t)p.spp + sample, frame);
+        Ray r = fast_camera_ray(p, x, y, rng);
+        rays[q][0] = make_float4(r.orig.x, r.orig.y, r.orig.z, __uint_as_float(rng));
+        rays[q][1] = make_float4(r.dir.x, r.dir.y, r.dir.z, __uint_as_float(e0 + q));
+    }
 }
 
 struct QPath
@@ -990,14 +1011,21 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // per SM when the sphere arrays fill most of an SM's shared memory.
 // Dynamic shared memory (FastSmem): [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
 // The body is shared by k_fast_queue (light sampling) and k_fast_queue_nolight (DO_LIGHT_SAMPLING 0) below.
-// RAYS: the ray source. false: camera rays of the image region; true (k_fast_rays): the caller's p.numRays rays
+// SRC: the ray source. kSrcCamera: camera rays of the image region. kSrcRays (k_fast_rays): the caller's p.numRays rays
 // (load_slab_rays), a slab being 64 consecutive rays x one sample index, finished paths adding col / spp to p.image[ray].
-template <int THREADS, int KFORM, int LS, bool RAYS = false>
+// kSrcPixels (k_fast_samples): the draw's camera rays for the p.numRays entries of a pixel list (generate_list_rays), a
+// slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
+// MOMENTS, (col^2, 0) to p.sq4[entry].
+enum QueueSource { kSrcCamera = 0, kSrcRays = 1, kSrcPixels = 2 };
+template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false>
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                 uint32_t raysOffset)
 {
+    // a pixel list with an index outside the image traces nothing (the call reports the index)
+    if constexpr (SRC == kSrcPixels)
+        if (p.pixels && *p.badPixel != ~0ull) return;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     __shared__ float sW[kMaxFramesPerDraw];
@@ -1017,7 +1045,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
     const unsigned ltMask = (1u << lane) - 1u;
-    const uint32_t regionPix = RAYS ? p.numRays : (uint32_t)((long long)p.numRows * p.width);
+    const uint32_t regionPix = SRC != kSrcCamera ? p.numRays : (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
     
     unsigned rc = 0;
@@ -1062,7 +1090,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
                 const uint32_t pix0 = mtile * kSlabPix;
                 slabEnd = regionPix - pix0 < (uint32_t)kSlabPix ? regionPix - pix0 : (uint32_t)kSlabPix;
                 slabCur = 0;
-                if constexpr (!RAYS)
+                if constexpr (SRC == kSrcCamera)
                 {
                     slabRi0 = (int)(pix0 / (uint32_t)p.width);
                     slabX0 = (int)(pix0 - (uint32_t)slabRi0 * (uint32_t)p.width);
@@ -1073,7 +1101,8 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
                 slabW = invSpp * sW[fi];
                 slabBand = bandDone ? mtile / mtilesPerBand : 0u;
                 __syncwarp();       // every lane has popped what it needed from the previous slab
-                if constexpr (RAYS) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
+                if constexpr (SRC == kSrcRays) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
+                else if constexpr (SRC == kSrcPixels) generate_list_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
                 else generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, slabX0, slabRi0, slabSample, slabFrame, -1);
                 __syncwarp();
             }
@@ -1104,7 +1133,13 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
 
         if (path_step<LS>(sc, st, rc, hitter))
         {
-            red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x * st.weight, st.col.y * st.weight, st.col.z * st.weight);
+            if constexpr (SRC == kSrcPixels)
+            {
+                red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x, st.col.y, st.col.z, 1.0f);
+                if constexpr (MOMENTS)
+                    red_add_f4(p.sq4 + (size_t)st.pixOff * 4, st.col.x * st.col.x, st.col.y * st.col.y, st.col.z * st.col.z);
+            }
+            else red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x * st.weight, st.col.y * st.weight, st.col.z * st.weight);
             st.active = false;
             if (bandDone)
             {
@@ -1157,7 +1192,7 @@ k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
             uint32_t raysOffset)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, true>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
 }
 
 template <int THREADS, int MINB, int KFORM>
@@ -1166,7 +1201,40 @@ k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneB
                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                     uint32_t raysOffset)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, true>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+}
+
+// tpt_draw_samples: the slab queue on a pixel list (SRC = kSrcPixels), per-entry sums and, with MOMENTS, sums of squares.
+// Same launch shapes and instances as k_fast_rays.
+template <int THREADS, int MINB, int KFORM, bool MOMENTS>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_samples(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+               uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
+               uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+                                                                 mtilesPerBand, raysOffset);
+}
+
+template <int THREADS, int MINB, int KFORM, bool MOMENTS>
+__global__ void __launch_bounds__(THREADS, MINB)
+k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                       uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone,
+                       uint32_t mtilesPerBand, uint32_t raysOffset)
+{
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+                                                                  mtilesPerBand, raysOffset);
+}
+
+// tpt_draw_samples' index check: the smallest (entry << 32 | index) of the entries whose index lies outside [0, numPix)
+// into *bad, which stays ~0 when there is none.
+__global__ void k_check_pixels(const int* __restrict__ pixels, long long n, long long numPix, unsigned long long* bad)
+{
+    for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    {
+        const int v = __ldg(pixels + i);
+        if (v < 0 || v >= numPix) atomicMin(bad, ((unsigned long long)i << 32) | (uint32_t)v);
+    }
 }
 
 // ---- variant 8 ------------------------------------------------------------------------------------------------
@@ -1840,17 +1908,20 @@ float prev_weight(int frame0, int numFrames, unsigned flags)
 }
 
 using QueueKernel = decltype(&k_fast_queue<128, TPT_QUEUE_MINB, 0>);
-// RAYS: the tpt_trace_rays family (k_fast_rays) instead of the camera-ray one (k_fast_queue)
-template <bool RAYS, int THREADS, int MINB, int KFORM>
+// SRC: the camera-ray family (k_fast_queue), tpt_trace_rays' (k_fast_rays) or tpt_draw_samples' (k_fast_samples, MOMENTS
+// selecting the instance that also adds squares)
+template <int SRC, bool MOMENTS, int THREADS, int MINB, int KFORM>
 static QueueKernel queue_instance(const SceneDev& sc)
 {
-    if constexpr (RAYS) return light_twin(sc, k_fast_rays<THREADS, MINB, KFORM>, k_fast_rays_nolight<THREADS, MINB, KFORM>);
+    if constexpr (SRC == kSrcRays) return light_twin(sc, k_fast_rays<THREADS, MINB, KFORM>, k_fast_rays_nolight<THREADS, MINB, KFORM>);
+    else if constexpr (SRC == kSrcPixels)
+        return light_twin(sc, k_fast_samples<THREADS, MINB, KFORM, MOMENTS>, k_fast_samples_nolight<THREADS, MINB, KFORM, MOMENTS>);
     else return light_twin(sc, k_fast_queue<THREADS, MINB, KFORM>, k_fast_queue_nolight<THREADS, MINB, KFORM>);
 }
-template <bool RAYS, int THREADS, int MINB>
+template <int SRC, bool MOMENTS, int THREADS, int MINB>
 static QueueKernel queue_kernel(const SceneDev& sc, int kform)
 {
-    return for_kform<3>(kform, [&](auto K) { return queue_instance<RAYS, THREADS, MINB, decltype(K)::value>(sc); });
+    return for_kform<3>(kform, [&](auto K) { return queue_instance<SRC, MOMENTS, THREADS, MINB, decltype(K)::value>(sc); });
 }
 
 struct QueuePick
@@ -1858,13 +1929,13 @@ struct QueuePick
     QueueKernel kern;
     int threads, kform;
 };
-// The slab-queue instance for `samples` samples of each of `regionPix` pixels or rays (variants 3/4/9; tpt_trace_rays
-// takes variant 3's choice). Small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays
+// The slab-queue instance for `samples` samples of each of `regionPix` pixels, rays or list entries (variants 3/4/9;
+// tpt_trace_rays and tpt_draw_samples take variant 3's choice). Small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays
 // fill most of an SM's shared memory: ONE 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs
 // x 4 warps with a copy each). Long launches (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80;
 // short ones keep 6, where a warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant
 // 9 forces the 8-CTA instance (A/B runs).
-template <bool RAYS>
+template <int SRC, bool MOMENTS = false>
 static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix, long long samples, int numSMs)
 {
     QueuePick q;
@@ -1873,16 +1944,17 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
                      sc.stagedBytes != sc.layout.totalBytes;
     const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
     q.threads = big ? TPT_BIG_THREADS : 128;
-    if (big) q.kern = queue_kernel<RAYS, TPT_BIG_THREADS, 1>(sc, q.kform);
-    else if (q.kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) q.kern = queue_instance<RAYS, 128, 8, 2>(sc);
-    else if (!RAYS && variant == 4) q.kern = queue_kernel<false, 128, 7>(sc, q.kform);
-    else q.kern = queue_kernel<RAYS, 128, TPT_QUEUE_MINB>(sc, q.kform);
+    if (big) q.kern = queue_kernel<SRC, MOMENTS, TPT_BIG_THREADS, 1>(sc, q.kform);
+    else if (q.kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) q.kern = queue_instance<SRC, MOMENTS, 128, 8, 2>(sc);
+    else if (SRC == kSrcCamera && variant == 4) q.kern = queue_kernel<kSrcCamera, false, 128, 7>(sc, q.kform);
+    else q.kern = queue_kernel<SRC, MOMENTS, 128, TPT_QUEUE_MINB>(sc, q.kform);
     return q;
 }
 
-// regionPix: pixels of the draw's region, or tpt_trace_rays' ray count. The accumulation buffer is prepared first: a draw's
-// region blended by the weight of `prev` (k_prepare_image), caller rays' float4 outputs zeroed.
-template <bool RAYS>
+// regionPix: pixels of the draw's region, tpt_trace_rays' ray count or the length of tpt_draw_samples' list. The
+// accumulation buffer is prepared first: a draw's region blended by the weight of `prev` (k_prepare_image), caller rays'
+// float4 outputs zeroed; tpt_draw_samples adds to the caller's sums as they are.
+template <int SRC>
 static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const DrawParams& p, const SceneDev& sc, int numSMs,
                                 cudaStream_t stream, unsigned int* bandDone, int numBands, unsigned int* bandExpected)
 {
@@ -1895,8 +1967,8 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, threads, lay.bytes, numSMs, (slabs + threads / 32 - 1) / (threads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
-    if constexpr (RAYS) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
-    else
+    if constexpr (SRC == kSrcRays) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
+    else if constexpr (SRC == kSrcCamera)
     {
         k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
         e = cudaGetLastError();
@@ -1973,8 +2045,29 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
 
 cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
 {
-    const QueuePick q = pick_queue<true>(sc, 3, p.numRays, p.spp, numSMs);
-    return launch_queue<true>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
+    const QueuePick q = pick_queue<kSrcRays>(sc, 3, p.numRays, p.spp, numSMs);
+    return launch_queue<kSrcRays>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
+}
+
+int fast_samples_launches(const DrawParams& p) { return p.pixels ? 2 : 1; }
+
+cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
+                                cudaStream_t stream)
+{
+    if (p.pixels)
+    {
+        cudaError_t e = cudaMemsetAsync(badPixel, 0xff, sizeof(unsigned long long), stream);
+        if (e != cudaSuccess) return e;
+        const long long blocks = ((long long)p.numRays + 255) / 256;
+        k_check_pixels<<<(unsigned)(blocks < 4LL * numSMs ? blocks : 4LL * numSMs), 256, 0, stream>>>(
+            p.pixels, p.numRays, (long long)p.width * p.height, badPixel);
+        if ((e = cudaGetLastError()) != cudaSuccess) return e;
+    }
+    DrawParams q = p;
+    q.badPixel = badPixel;
+    const QueuePick k = p.sq4 ? pick_queue<kSrcPixels, true>(sc, 3, p.numRays, p.spp, numSMs)
+                              : pick_queue<kSrcPixels, false>(sc, 3, p.numRays, p.spp, numSMs);
+    return launch_queue<kSrcPixels>(k, p.numRays, q, sc, numSMs, stream, nullptr, 0, nullptr);
 }
 
 // ---- first-hit AOVs (tpt_draw_aovs, tpt_trace_aovs) ----------------------------------------------------------------
@@ -2143,8 +2236,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
     }
     if (variant == 3 || variant == 4 || variant == 9)
     {
-        const QueuePick q = pick_queue<false>(sc, variant, regionPix, (long long)p.spp * p.numFrames, numSMs);
-        return launch_queue<false>(q, regionPix, p, sc, numSMs, stream, bandDone, numBands, bandExpected);
+        const QueuePick q = pick_queue<kSrcCamera>(sc, variant, regionPix, (long long)p.spp * p.numFrames, numSMs);
+        return launch_queue<kSrcCamera>(q, regionPix, p, sc, numSMs, stream, bandDone, numBands, bandExpected);
     }
     if (variant == 8)
     {

@@ -36,6 +36,15 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
 // pixel_seed(ray * spp + sample, p.frame0), mean written to the float4 p.image[ray] (zeroed first); p.numFrames = 1, p.flags = 0.
 // Runs the slab-queue instance variant 3 would run for the scene.
 cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
+// tpt_draw_samples: p.spp samples of each of the p.numRays (>= 1) entries of the pixel list p.pixels (null: pixels 0 ..
+// numRays - 1 of the width x height image), sample s of pixel i being the fast draw's camera ray with stream
+// pixel_seed(i * spp + s, p.frame0). Adds (sum of col, spp) to the float4 p.image[entry] and, when p.sq4 is not null,
+// (sum of col^2, 0) to p.sq4[entry]; p.numFrames = 1, p.flags = 0. A list is checked first: the smallest
+// (entry << 32 | index) of an index outside the image lands in *badPixel (device; ~0 when there is none) and then nothing
+// is traced. Runs the slab-queue instance variant 3 would run for the scene.
+cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
+                                cudaStream_t stream);
+int fast_samples_launches(const DrawParams& p);
 // tpt_draw_aovs (rays = false: the region of p, frames [p.frame0, p.frame0 + p.numFrames) at p.spp, blended over the outputs
 // with the weight of `prev`) and tpt_trace_aovs (rays = true: p.numRays >= 1 caller rays p.rays): first-hit albedo4,
 // normal4 and ids (each may be null) with the slab queue's sweep form, one ray counted per traced sample.

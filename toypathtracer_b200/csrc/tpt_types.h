@@ -90,6 +90,11 @@ struct DrawParams
     unsigned int* workCounter;      // persistent kernels: next tile
     const float* rays;        // tpt_trace_rays: numRays caller rays {o.xyz, d.xyz}, 4-byte aligned; `image` gets one float4 per ray
     uint32_t numRays;
+    // tpt_draw_samples: numRays list entries, pixel indices y * width + x (null: entry i is pixel i); `image` (sum4) and sq4
+    // get one float4 per entry. badPixel: the index check's result, ~0 when every index is inside the image.
+    const int* pixels;
+    float* sq4;
+    const unsigned long long* badPixel;
 };
 
 } // namespace tpt
