@@ -123,27 +123,59 @@ def _numel(buf) -> int:
     return int(buf.size) if isinstance(buf, np.ndarray) else int(buf.numel())
 
 
-def _aov_ptrs(what: str, albedo, normal, ids, pixels: int):
-    """Addresses of the AOV outputs that are given (float4 albedo and normal, int32 ids, `pixels` entries each unless a
-    DevicePtr), their common kind (on device or not) and keepalives."""
+_CUDA_STREAM_LEGACY = 1            # cudaStreamLegacy: torch's default stream, whose handle reads as 0
+_NO_ENTRIES = (ctypes.c_int * 1)()  # the address passed for an empty buffer: it has no data pointer, and NULL means "none"
+
+
+def _entries(what: str, name: str, buf, n, row: Tuple[int, ...]) -> int:
+    """The entry count of a caller input `name` of shape (N, *row), or of a DevicePtr, which needs `n`; a given n must
+    match the buffer."""
+    if isinstance(buf, DevicePtr):
+        if n is None:
+            raise TptError(f"{what}: a DevicePtr needs n")
+        return int(n)
+    if tuple(buf.shape[1:]) != row or len(buf.shape) != 1 + len(row):
+        raise TptError(f"{what}: {name} must have shape (N,{''.join(f' {d}' for d in row)})")
+    if n is not None and int(n) != buf.shape[0]:
+        raise TptError(f"{what}: n does not match {name}")
+    return int(buf.shape[0])
+
+
+def _buffer_ptrs(what: str, bufs, entries: int):
+    """Addresses of the given buffers among `bufs`, (name, buffer or None, dtype, values per entry) each, which must hold
+    `entries` entries unless a DevicePtr; their common kind (on device or not) and keepalives."""
     ptrs, kinds, keep = [], set(), []
-    for name, buf, dtype, per in (("albedo", albedo, "float32", 4), ("normal", normal, "float32", 4), ("ids", ids, "int32", 1)):
+    for name, buf, dtype, per in bufs:
         if buf is None:
             ptrs.append(None)
             continue
-        if not isinstance(buf, DevicePtr) and _numel(buf) != pixels * per:
-            raise TptError(f"{what}: {name} must hold {pixels} x {per} {dtype} values, not {_numel(buf)}")
+        if not isinstance(buf, DevicePtr) and _numel(buf) != entries * per:
+            raise TptError(f"{what}: {name} must hold {entries} x {per} {dtype} values, not {_numel(buf)}")
         addr, on_dev, k = _as_ptr(buf, dtype)
+        if addr == 0 and entries == 0:
+            addr = ctypes.addressof(_NO_ENTRIES)
         ptrs.append(ctypes.c_void_p(addr)); kinds.add(on_dev); keep.append(k)
+    names = [b[0] for b in bufs]
     if not kinds:
-        raise TptError(f"{what}: no output buffer (albedo, normal or ids)")
+        raise TptError(f"{what}: no output buffer ({', '.join(names[:-1])} or {names[-1]})")
     if len(kinds) > 1:
-        raise TptError(f"{what}: the outputs must be all host or all device buffers")
+        raise TptError(f"{what}: {', '.join(names[:-1])} and {names[-1]} must be all host or all device buffers")
     return ptrs, kinds.pop(), keep
 
 
-_CUDA_STREAM_LEGACY = 1            # cudaStreamLegacy: torch's default stream, whose handle reads as 0
-_NO_ENTRIES = (ctypes.c_int * 1)()  # the address draw_samples passes for an empty pixel list
+def _aovs(albedo, normal, ids):
+    """The AOV outputs for _buffer_ptrs: float4 albedo and normal, int32 ids."""
+    return [("albedo", albedo, "float32", 4), ("normal", normal, "float32", 4), ("ids", ids, "int32", 1)]
+
+
+def _alloc_like(like, device: int, specs):
+    """New outputs of (shape, dtype name) `specs` of the kind of input `like`: numpy arrays for a numpy array, else torch
+    tensors on like's device (CUDA device `device` for a DevicePtr)."""
+    if isinstance(like, np.ndarray):
+        return [np.empty(shape, dtype) for shape, dtype in specs]
+    import torch
+    dev = like.device if hasattr(like, "device") else torch.device("cuda", device)
+    return [torch.empty(shape, dtype=getattr(torch, dtype), device=dev) for shape, dtype in specs]
 
 
 def _cuda_device(*bufs):
@@ -220,6 +252,15 @@ class Context:
         if rc != 0:
             raise TptError(f"{what} failed ({rc}): {self._L.tpt_last_error(self._h).decode()}")
 
+    def _call(self, fn: str, want_rays: bool, stream: int, *args) -> int:
+        """Library call `fn`(context, *args, outRayCount, cudaStream) of a caller-buffer function; returns the rays it
+        traced (0 when not want_rays). Stream 0 is the context's own stream."""
+        total = ctypes.c_longlong(0)
+        rc = getattr(self._L, fn)(self._h, *args, ctypes.byref(total) if want_rays else None,
+                                  ctypes.c_void_p(stream) if stream else None)
+        self._check(rc, fn)
+        return int(total.value)
+
     def set_scene(self, spheres: np.ndarray, materials: np.ndarray, camera: np.ndarray,
                   emissives: Optional[np.ndarray] = None):
         """Raw scene as exported by GetSceneDesc (Test.cpp:377-384)."""
@@ -272,32 +313,14 @@ class Context:
         DevicePtr together with `n`. Without `out` the result is a new (N, 4) array of the same kind as `rays` (numpy, CPU or
         CUDA tensor; a DevicePtr gets a CUDA tensor); `out` may be any buffer of N float4. Returns (out, rays traced), or
         out alone when want_rays is False (device buffers then stay asynchronous on `stream`)."""
-        if isinstance(rays, DevicePtr):
-            if n is None:
-                raise TptError("trace_rays: a DevicePtr needs n")
-            raddr, ron, keep = rays.addr, True, rays
-        else:
-            if tuple(rays.shape[1:]) != (6,) or len(rays.shape) != 2:
-                raise TptError("trace_rays: rays must have shape (N, 6)")
-            if n is not None and int(n) != rays.shape[0]:
-                raise TptError("trace_rays: n does not match rays")
-            n = rays.shape[0]
-            raddr, ron, keep = _as_ptr(rays)
-        n = int(n)
+        n = _entries("trace_rays", "rays", rays, n, (6,))
+        raddr, ron, _keep = _as_ptr(rays)
         if out is None:
-            if isinstance(rays, np.ndarray):
-                out = np.empty((n, 4), np.float32)
-            else:
-                import torch
-                dev = rays.device if hasattr(rays, "device") else torch.device("cuda", self.device)
-                out = torch.empty((n, 4), dtype=torch.float32, device=dev)
-        oaddr, oon, keep_out = _as_ptr(out)
-        total = ctypes.c_longlong(0)
-        rc = self._L.tpt_trace_rays(self._h, ctypes.c_void_p(raddr), 1 if ron else 0, n, int(spp), int(frame),
-                                    ctypes.c_void_p(oaddr), 1 if oon else 0, ctypes.byref(total) if want_rays else None,
-                                    ctypes.c_void_p(stream) if stream else None)
-        self._check(rc, "tpt_trace_rays")
-        return (out, int(total.value)) if want_rays else out
+            (out,) = _alloc_like(rays, self.device, [((n, 4), "float32")])
+        (po,), oon, _keep_out = _buffer_ptrs("trace_rays", [("out", out, "float32", 4)], n)
+        total = self._call("tpt_trace_rays", want_rays, stream, ctypes.c_void_p(raddr), 1 if ron else 0, n, int(spp),
+                           int(frame), po, 1 if oon else 0)
+        return (out, total) if want_rays else out
 
     def draw_aovs(self, frame: int, num_frames: int, width: int, height: int, albedo=None, normal=None, ids=None,
                   flags: int = 0, rows: Optional[Tuple[int, int, int, int]] = None, stream: int = 0, want_rays: bool = True):
@@ -307,13 +330,10 @@ class Context:
         Buffers hold width x height pixels (numRows with a packed row region), all host or all device; rows = (row0,
         numRows, rowStep, packed). Returns the rays traced (one per sample) if want_rays, else None."""
         row0, nrows, step, packed = rows if rows is not None else (0, height, 1, 0)
-        (pa, pn, pi), on_dev, _keep = _aov_ptrs("draw_aovs", albedo, normal, ids, (nrows if packed else height) * width)
-        total = ctypes.c_longlong(0)
-        rc = self._L.tpt_draw_aovs(self._h, frame, num_frames, width, height, row0, nrows, step, packed, pa, pn, pi,
-                                   1 if on_dev else 0, flags, ctypes.byref(total) if want_rays else None,
-                                   ctypes.c_void_p(stream) if stream else None)
-        self._check(rc, "tpt_draw_aovs")
-        return int(total.value) if want_rays else None
+        (pa, pn, pi), on_dev, _keep = _buffer_ptrs("draw_aovs", _aovs(albedo, normal, ids), (nrows if packed else height) * width)
+        total = self._call("tpt_draw_aovs", want_rays, stream, frame, num_frames, width, height, row0, nrows, step, packed,
+                           pa, pn, pi, 1 if on_dev else 0, flags)
+        return total if want_rays else None
 
     def trace_aovs(self, rays, albedo=None, normal=None, ids=None, n=None, stream: int = 0, want_rays: bool = True):
         """tpt_trace_aovs: first-hit AOVs of caller rays {o.xyz, d.xyz} (buffers as for trace_rays). albedo and normal
@@ -321,33 +341,14 @@ class Context:
         of them may be omitted, and without all three they are allocated, (N, 4), (N, 4) and (N,), of the kind of `rays`
         (a DevicePtr gets CUDA tensors). Returns ((albedo, normal, ids), rays traced), or the tuple alone when want_rays
         is False."""
-        if isinstance(rays, DevicePtr):
-            if n is None:
-                raise TptError("trace_aovs: a DevicePtr needs n")
-            raddr, ron, keep = rays.addr, True, rays
-        else:
-            if tuple(rays.shape[1:]) != (6,) or len(rays.shape) != 2:
-                raise TptError("trace_aovs: rays must have shape (N, 6)")
-            if n is not None and int(n) != rays.shape[0]:
-                raise TptError("trace_aovs: n does not match rays")
-            n = rays.shape[0]
-            raddr, ron, keep = _as_ptr(rays)
-        n = int(n)
+        n = _entries("trace_aovs", "rays", rays, n, (6,))
+        raddr, ron, _keep = _as_ptr(rays)
         if albedo is None and normal is None and ids is None:
-            if isinstance(rays, np.ndarray):
-                albedo, normal, ids = np.empty((n, 4), np.float32), np.empty((n, 4), np.float32), np.empty(n, np.int32)
-            else:
-                import torch
-                dev = rays.device if hasattr(rays, "device") else torch.device("cuda", self.device)
-                albedo = torch.empty((n, 4), dtype=torch.float32, device=dev)
-                normal = torch.empty((n, 4), dtype=torch.float32, device=dev)
-                ids = torch.empty(n, dtype=torch.int32, device=dev)
-        (pa, pn, pi), oon, _keep = _aov_ptrs("trace_aovs", albedo, normal, ids, n)
-        total = ctypes.c_longlong(0)
-        rc = self._L.tpt_trace_aovs(self._h, ctypes.c_void_p(raddr), 1 if ron else 0, n, pa, pn, pi, 1 if oon else 0,
-                                    ctypes.byref(total) if want_rays else None, ctypes.c_void_p(stream) if stream else None)
-        self._check(rc, "tpt_trace_aovs")
-        return ((albedo, normal, ids), int(total.value)) if want_rays else (albedo, normal, ids)
+            albedo, normal, ids = _alloc_like(rays, self.device, [((n, 4), "float32"), ((n, 4), "float32"), (n, "int32")])
+        (pa, pn, pi), oon, _keep_out = _buffer_ptrs("trace_aovs", _aovs(albedo, normal, ids), n)
+        total = self._call("tpt_trace_aovs", want_rays, stream, ctypes.c_void_p(raddr), 1 if ron else 0, n, pa, pn, pi,
+                           1 if oon else 0)
+        return ((albedo, normal, ids), total) if want_rays else (albedo, normal, ids)
 
     def draw_samples(self, frame: int, width: int, height: int, pixels=None, spp: Optional[int] = None, sum4=None,
                      sq4=None, stream: int = 0, want_rays: bool = True, n=None):
@@ -367,31 +368,20 @@ class Context:
         if pixels is None:
             if n is not None and int(n) != numpix:
                 raise TptError("draw_samples: without pixels n must be width * height")
-            n, paddr, pon, kind = numpix, None, None, None
-        elif isinstance(pixels, DevicePtr):
-            if n is None:
-                raise TptError("draw_samples: a DevicePtr needs n")
-            paddr, pon, kind = pixels.addr, True, None
+            n = numpix
         else:
-            if len(pixels.shape) != 1:
-                raise TptError("draw_samples: pixels must have shape (N,)")
-            if n is not None and int(n) != pixels.shape[0]:
-                raise TptError("draw_samples: n does not match pixels")
-            n = pixels.shape[0]
-            paddr, pon, _keep = _as_ptr(pixels, "int32")
-            kind = pixels
-        n = int(n)
+            n = _entries("draw_samples", "pixels", pixels, n, ())
         if n < 0:
             raise TptError("draw_samples: n < 0")
         if sum4 is None and sq4 is not None:
             raise TptError("draw_samples: sq4 needs sum4")
         alloc_dev = None
         if sum4 is None:
-            if isinstance(kind, np.ndarray):
+            if isinstance(pixels, np.ndarray):
                 sum4, sq4 = np.zeros((n, 4), np.float32), np.zeros((n, 4), np.float32)
             else:
                 import torch
-                alloc_dev = kind.device if kind is not None else torch.device("cuda", self.device)
+                alloc_dev = pixels.device if hasattr(pixels, "device") else torch.device("cuda", self.device)
         # Torch CUDA tensors are written and read on torch's streams, which the library does not know: without an
         # explicit stream the call runs on torch's current stream of their device, after the torch work that filled
         # them (and the zeroing of outputs allocated here) and before the torch work that reads the sums.
@@ -408,29 +398,11 @@ class Context:
             with on:
                 sum4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
                 sq4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
-        # empty buffers have no data pointer; the library reads none of an empty list's, but NULL means "no list"
-        if paddr == 0 and n == 0:
-            paddr = ctypes.addressof(_NO_ENTRIES)
-        ptrs, kinds, keep = [], set() if pon is None else {pon}, []
-        for name, buf in (("sum4", sum4), ("sq4", sq4)):
-            if buf is None:
-                ptrs.append(None)
-                continue
-            if not isinstance(buf, DevicePtr) and _numel(buf) != n * 4:
-                raise TptError(f"draw_samples: {name} must hold {n} x 4 float32 values, not {_numel(buf)}")
-            addr, on_dev, k = _as_ptr(buf)
-            if addr == 0 and n == 0:
-                addr = ctypes.addressof(_NO_ENTRIES)
-            ptrs.append(ctypes.c_void_p(addr)); kinds.add(on_dev); keep.append(k)
-        if len(kinds) > 1:
-            raise TptError("draw_samples: pixels, sum4 and sq4 must be all host or all device buffers")
-        total = ctypes.c_longlong(0)
-        rc = self._L.tpt_draw_samples(self._h, int(frame), int(width), int(height),
-                                      None if paddr is None else ctypes.c_void_p(paddr), n, spp, ptrs[0], ptrs[1],
-                                      1 if kinds.pop() else 0, ctypes.byref(total) if want_rays else None,
-                                      ctypes.c_void_p(stream) if stream else None)
-        self._check(rc, "tpt_draw_samples")
-        return ((sum4, sq4), int(total.value)) if want_rays else (sum4, sq4)
+        (pp, ps, pq), on_dev, _keep = _buffer_ptrs(
+            "draw_samples", [("pixels", pixels, "int32", 1), ("sum4", sum4, "float32", 4), ("sq4", sq4, "float32", 4)], n)
+        total = self._call("tpt_draw_samples", want_rays, stream, int(frame), int(width), int(height), pp, n, spp, ps, pq,
+                           1 if on_dev else 0)
+        return ((sum4, sq4), total) if want_rays else (sum4, sq4)
 
     def render_adaptive(self, width: int, height: int, base_spp: int = 4, max_spp: int = 64, rel_err: float = 0.05,
                         frame: int = 0):

@@ -9,9 +9,14 @@
 #include <string>
 #include <vector>
 #include <string.h>
+#include <stdarg.h>
 #include <stdio.h>
 
 using namespace tpt;
+
+// Device staging allocations of host buffers (tpt_context::staging). kStageImage holds tpt_draw's image, the input of
+// tpt_tonemap_rgba8, tpt_trace_rays' out4 and tpt_draw_samples' sum4; the others hold the buffers they are named after.
+enum Staging { kStageImage, kStageRays, kStageAlbedo, kStageNormal, kStageIds, kStagePixels, kStageSq4, kNumStaging };
 
 struct tpt_context
 {
@@ -74,13 +79,7 @@ struct tpt_context
     size_t maxScratchBytes = (size_t)8 << 30;
 
     // buffers
-    float* dImage = nullptr; size_t imageCap = 0;      // staging image for host-pointer draws (and host tpt_trace_rays outputs)
-    float* dRays = nullptr; size_t raysCap = 0;        // staging of host tpt_trace_rays / tpt_trace_aovs inputs
-    float* dAovAlbedo = nullptr; size_t aovAlbedoCap = 0;   // staging of host AOV outputs (tpt_draw_aovs, tpt_trace_aovs)
-    float* dAovNormal = nullptr; size_t aovNormalCap = 0;
-    int* dAovIds = nullptr; size_t aovIdsCap = 0;
-    int* dPixels = nullptr; size_t pixelsCap = 0;      // staging of host tpt_draw_samples lists (sum4 goes through dImage)
-    float* dSq4 = nullptr; size_t sq4Cap = 0;
+    struct { void* ptr = nullptr; size_t cap = 0; } staging[kNumStaging];   // grown by ensure, see Staging
     unsigned long long* dBadPixel = nullptr;           // tpt_draw_samples' index check, and its page-locked copy
     unsigned long long* hBadPixel = nullptr;
     float* dScratch = nullptr; size_t scratchCap = 0;  // exact mode per-frame colours
@@ -128,6 +127,15 @@ static int fail_msg(tpt_context* ctx, const char* msg)
 {
     if (ctx) ctx->lastError = msg;
     return (int)cudaErrorInvalidValue;
+}
+__attribute__((format(printf, 2, 3))) static int fail_msgf(tpt_context* ctx, const char* fmt, ...)
+{
+    char msg[256];
+    va_list args;
+    va_start(args, fmt);
+    vsnprintf(msg, sizeof(msg), fmt, args);
+    va_end(args);
+    return fail_msg(ctx, msg);
 }
 #define CK(call, what) do { cudaError_t _e = (call); if (_e != cudaSuccess) return fail(ctx, _e, what); } while (0)
 
@@ -234,7 +242,8 @@ void tpt_destroy(tpt_context* ctx)
     cudaSetDevice(ctx->device);
     cudaDeviceSynchronize();
     if (ctx->registeredPtr) cudaHostUnregister(ctx->registeredPtr);
-    cudaFree(ctx->dImage); cudaFree(ctx->dRays); cudaFree(ctx->dAovAlbedo); cudaFree(ctx->dAovNormal); cudaFree(ctx->dAovIds); cudaFree(ctx->dPixels); cudaFree(ctx->dSq4); cudaFree(ctx->dBadPixel); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
+    for (auto& s : ctx->staging) cudaFree(s.ptr);
+    cudaFree(ctx->dBadPixel); cudaFree(ctx->dScratch); cudaFree(ctx->dRayCounters); cudaFree(ctx->dLook); cudaFree(ctx->dLookRays);
     cudaFree(ctx->dAccum); cudaFree(ctx->dWork);
     for (int i = 0; i < 2; ++i)
     {
@@ -476,6 +485,38 @@ static int finish_call(tpt_context* ctx, cudaStream_t stream, int n, bool hostBu
     return 0;
 }
 
+// A call with nothing to trace: no launch, no rays (none in each of its `numFrames` frames either).
+static int empty_call(tpt_context* ctx, long long* outRayCount, long long* outPerFrame = nullptr, int numFrames = 0)
+{
+    if (outRayCount) *outRayCount = 0;
+    if (outPerFrame) for (int i = 0; i < numFrames; ++i) outPerFrame[i] = 0;
+    ctx->lastLaunches = 0;
+    return 0;
+}
+
+// The work-counter slot of the next launch sequence: the ring leaves the slots of the calls still in flight alone.
+static unsigned int* next_work_counter(tpt_context* ctx)
+{
+    return ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+}
+
+// Parameters of a draw of the rows y_i = row0 + i*rowStep (or the packed band) of a width x height image through the
+// context's camera; the rest is zero.
+static DrawParams image_params(const tpt_context* ctx, int width, int height, int row0, int numRows, int rowStep, int packed,
+                               int spp, unsigned flags)
+{
+    DrawParams p;
+    memset(&p, 0, sizeof(p));
+    p.cam = ctx->cam;
+    p.width = width; p.height = height;
+    p.row0 = row0; p.numRows = numRows; p.rowStep = rowStep; p.packed = packed ? 1 : 0;
+    p.spp = spp;
+    p.flags = flags;
+    p.invWidth = 1.0f / (float)width;     // Test.cpp:270-271
+    p.invHeight = 1.0f / (float)height;
+    return p;
+}
+
 int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
              int row0, int numRows, int rowStep, int packed,
              float* backbuffer, int bufferOnDevice, unsigned testFlags, int mode,
@@ -488,14 +529,8 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode != TPT_MODE_EXACT && mode != TPT_MODE_FAST && mode != TPT_MODE_REFGPU && mode != TPT_MODE_REFGPU_FAST)
         return fail_msg(ctx, "tpt_draw: unknown mode");
     const bool refgpu = mode == TPT_MODE_REFGPU || mode == TPT_MODE_REFGPU_FAST;
-    if (numRows == 0)
-    {
-        // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
-        if (outRayCount) *outRayCount = 0;
-        if (outRaysPerFrame) for (int i = 0; i < numFrames; ++i) outRaysPerFrame[i] = 0;
-        ctx->lastLaunches = 0;
-        return 0;
-    }
+    // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
+    if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
     cudaStream_t stream;
     SceneDev scene;
@@ -544,9 +579,10 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     }
     if (!bufferOnDevice && !zeroCopy)
     {
-        int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, bufBytes, "cudaMalloc image");
+        auto& st = ctx->staging[kStageImage];
+        int r = ensure(ctx, &st.ptr, &st.cap, bufBytes, "cudaMalloc image");
         if (r) return r;
-        dImage = ctx->dImage;
+        dImage = (float*)st.ptr;
         // `prev` is an input of the blend (Test.cpp:293). Exact mode always uploads it (NaN/Inf * 0 and the
         // untouched alpha are part of bit parity). Fast mode uploads it only when prev has a non-zero weight;
         // otherwise the kernel writes alpha = 0, which is what every reference shell's zero-initialised buffer
@@ -572,17 +608,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode == TPT_MODE_FAST && framesPerLaunch > 256) framesPerLaunch = 256;
 
     if (int r = start_kernels(ctx, stream, numFrames)) return r;
-    DrawParams p;
-    memset(&p, 0, sizeof(p));
-    p.cam = ctx->cam;
-    p.width = width; p.height = height;
-    p.row0 = row0; p.numRows = numRows; p.rowStep = rowStep; p.packed = packed ? 1 : 0;
-    p.spp = ctx->spp;
-    p.flags = testFlags;
-    p.invWidth = 1.0f / (float)width;     // Test.cpp:270-271
-    p.invHeight = 1.0f / (float)height;
+    DrawParams p = image_params(ctx, width, height, row0, numRows, rowStep, packed, ctx->spp, testFlags);
     p.image = dImage;
-    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    p.workCounter = next_work_counter(ctx);
     // alpha is never written by the reference (Maths.h:38). When `prev` has zero weight the fast kernels keep the alpha
     // that is in the buffer, unless the staging image was not uploaded (host buffer) or the caller waived it.
     p.zeroAlpha = (ctx->fastAlphaZero || (!bufferOnDevice && !needPrev)) ? 1 : 0;     // (zero-copy: never reads host memory)
@@ -737,25 +765,90 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
 }
 
-// A device buffer of tpt_trace_rays (or the AOV calls, named by fn) must be addressable by the context's device: its own
-// memory, or mapped host memory.
-static int check_device_buffer(tpt_context* ctx, const void* ptr, const char* name, const char* fn = "tpt_trace_rays")
+} // extern "C" (the caller-buffer helpers below are templates, which cannot have C linkage)
+
+// A row region of a draw's image: rows y_i = row0 + i*rowStep (or the packed band) of `width` pixels, see copy_rows.
+struct RowRegion { int width, row0, numRows, rowStep, packed; };
+
+enum { kCopyUp = 1, kCopyDown = 2 };
+
+// One caller buffer of tpt_trace_rays, tpt_trace_aovs, tpt_draw_aovs or tpt_draw_samples. A null `ptr` is a buffer the
+// caller left out: it is neither checked nor staged.
+struct CallerBuffer
+{
+    const char* name;                   // as the error texts name it
+    void* ptr;                          // the caller's
+    bool onDevice;                      // device memory (or mapped host memory); otherwise staged
+    int align;                          // bytes a device pointer must be aligned to
+    size_t bytes;                       // the whole buffer: the size of its staging allocation
+    Staging staging;                    // the allocation a host buffer is staged through
+    int copy;                           // kCopyUp: a host buffer is uploaded before the kernels, kCopyDown: downloaded after
+    const RowRegion* rows = nullptr;    // a draw buffer: only the region's rows of pixBytes-byte pixels are copied
+    size_t pixBytes = 16;
+    void* dev = nullptr;                // what the kernels use, set by stage_in
+};
+
+// A device buffer must be addressable by the context's device: its own memory, or mapped host memory.
+static int check_device_buffer(tpt_context* ctx, const char* fn, const void* ptr, const char* name)
 {
     cudaPointerAttributes attr;
-    char msg[160];
     if (cudaPointerGetAttributes(&attr, ptr) != cudaSuccess || attr.type == cudaMemoryTypeUnregistered)
     {
         (void)cudaGetLastError();
-        snprintf(msg, sizeof(msg), "%s: device %s is not CUDA memory", fn, name);
-        return fail_msg(ctx, msg);
+        return fail_msgf(ctx, "%s: device %s is not CUDA memory", fn, name);
     }
     if ((attr.type == cudaMemoryTypeDevice || attr.type == cudaMemoryTypeManaged) && attr.device != ctx->device)
+        return fail_msgf(ctx, "%s: device %s lives on device %d, the context on device %d", fn, name, attr.device, ctx->device);
+    return 0;
+}
+
+// The device buffers of call `fn`: all aligned, then each addressable by the context's device.
+template <int N>
+static int check_buffers(tpt_context* ctx, const char* fn, const CallerBuffer (&bufs)[N])
+{
+    for (const CallerBuffer& b : bufs)
+        if (b.ptr && b.onDevice && ((uintptr_t)b.ptr & (uintptr_t)(b.align - 1)))
+            return fail_msgf(ctx, "%s: device %s is not %d-byte aligned", fn, b.name, b.align);
+    for (const CallerBuffer& b : bufs)
+        if (b.ptr && b.onDevice)
+            if (int r = check_device_buffer(ctx, fn, b.ptr, b.name)) return r;
+    return 0;
+}
+
+static cudaError_t copy_buffer(const CallerBuffer& b, void* dst, const void* src, cudaMemcpyKind kind, cudaStream_t stream)
+{
+    if (!b.rows) return cudaMemcpyAsync(dst, src, b.bytes, kind, stream);
+    const RowRegion& r = *b.rows;
+    return copy_rows(dst, src, r.width, r.row0, r.numRows, r.rowStep, r.packed, kind, stream, b.pixBytes);
+}
+
+// Gives every buffer the pointer its kernels use: a host buffer's staging allocation, grown to the buffer's size and
+// uploaded when the record says so.
+template <int N>
+static int stage_in(tpt_context* ctx, cudaStream_t stream, CallerBuffer (&bufs)[N])
+{
+    for (CallerBuffer& b : bufs)
     {
-        snprintf(msg, sizeof(msg), "%s: device %s lives on device %d, the context on device %d", fn, name, attr.device, ctx->device);
-        return fail_msg(ctx, msg);
+        b.dev = b.ptr;
+        if (!b.ptr || b.onDevice) continue;
+        auto& st = ctx->staging[b.staging];
+        if (int r = ensure(ctx, &st.ptr, &st.cap, b.bytes, b.name)) return r;
+        b.dev = st.ptr;
+        if (b.copy & kCopyUp) CK(copy_buffer(b, b.dev, b.ptr, cudaMemcpyHostToDevice, stream), b.name);
     }
     return 0;
 }
+
+// Copies the host buffers the record says so back from their staging allocations.
+template <int N>
+static int stage_out(tpt_context* ctx, cudaStream_t stream, const CallerBuffer (&bufs)[N])
+{
+    for (const CallerBuffer& b : bufs)
+        if (b.ptr && !b.onDevice && (b.copy & kCopyDown)) CK(copy_buffer(b, b.ptr, b.dev, cudaMemcpyDeviceToHost, stream), b.name);
+    return 0;
+}
+
+extern "C" {
 
 int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
                    float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
@@ -767,94 +860,30 @@ int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     if (spp < 1) return fail_msg(ctx, "tpt_trace_rays: spp < 1");
     // the sample stream of (ray i, sample s) is i * spp + s in 32 bits, and so is the ray index
     if (n > (1LL << 32) / spp || n > 0xffffffffLL) return fail_msg(ctx, "tpt_trace_rays: n * spp > 2^32 (32-bit sample streams)");
-    if (raysOnDevice && ((uintptr_t)rays6 & 3)) return fail_msg(ctx, "tpt_trace_rays: device rays6 is not 4-byte aligned");
-    if (outOnDevice && ((uintptr_t)out4 & 15)) return fail_msg(ctx, "tpt_trace_rays: device out4 is not 16-byte aligned");
-    if (raysOnDevice) { if (int r = check_device_buffer(ctx, rays6, "rays6")) return r; }
-    if (outOnDevice) { if (int r = check_device_buffer(ctx, out4, "out4")) return r; }
-    if (n == 0)
-    {
-        if (outRayCount) *outRayCount = 0;
-        ctx->lastLaunches = 0;
-        return 0;
-    }
+    CallerBuffer bufs[] = {{"rays6", (void*)rays6, raysOnDevice != 0, 4, (size_t)n * 24, kStageRays, kCopyUp},
+                           {"out4", out4, outOnDevice != 0, 16, (size_t)n * 16, kStageImage, kCopyDown}};
+    if (int r = check_buffers(ctx, "tpt_trace_rays", bufs)) return r;
+    if (n == 0) return empty_call(ctx, outRayCount);
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    const float* dRays = rays6;
-    float* dOut = out4;
-    if (!raysOnDevice)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dRays, &ctx->raysCap, (size_t)n * 24, "cudaMalloc rays")) return r;
-        CK(cudaMemcpyAsync(ctx->dRays, rays6, (size_t)n * 24, cudaMemcpyHostToDevice, stream), "H2D rays");
-        dRays = ctx->dRays;
-    }
-    if (!outOnDevice)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, (size_t)n * 16, "cudaMalloc ray outputs")) return r;
-        dOut = ctx->dImage;
-    }
+    if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
     DrawParams p;
     memset(&p, 0, sizeof(p));
     p.spp = spp;
     p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
-    p.image = dOut;
+    p.image = (float*)bufs[1].dev;
     p.rayCounter = ctx->dRayCounters;
-    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
-    p.rays = dRays;
+    p.workCounter = next_work_counter(ctx);
+    p.rays = (const float*)bufs[0].dev;
     p.numRays = (uint32_t)n;
     cudaError_t e = launch_fast_rays(p, scene, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
-    if (!outOnDevice) CK(cudaMemcpyAsync(out4, dOut, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H ray outputs");
+    if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
-}
-
-// Outputs of tpt_draw_aovs / tpt_trace_aovs (fn): at least one buffer; device buffers aligned (float4 outputs to 16 bytes,
-// ids to 4) and addressable by the context's device.
-static int check_aov_outputs(tpt_context* ctx, const char* fn, const float* albedo4, const float* normal4, const int* ids, int onDevice)
-{
-    char msg[160];
-    if (!albedo4 && !normal4 && !ids)
-    {
-        snprintf(msg, sizeof(msg), "%s: albedo4, normal4 and ids are all null", fn);
-        return fail_msg(ctx, msg);
-    }
-    if (!onDevice) return 0;
-    const struct { const void* ptr; const char* name; int align; } outs[3] = {{albedo4, "albedo4", 16}, {normal4, "normal4", 16}, {ids, "ids", 4}};
-    for (const auto& o : outs)
-    {
-        if (!o.ptr) continue;
-        if ((uintptr_t)o.ptr & (uintptr_t)(o.align - 1))
-        {
-            snprintf(msg, sizeof(msg), "%s: device %s is not %d-byte aligned", fn, o.name, o.align);
-            return fail_msg(ctx, msg);
-        }
-        if (int r = check_device_buffer(ctx, o.ptr, o.name, fn)) return r;
-    }
-    return 0;
-}
-
-// Host AOV outputs of `pixels` pixels: each given buffer is replaced by the context's staging buffer for it.
-static int stage_aov_outputs(tpt_context* ctx, size_t pixels, float*& albedo4, float*& normal4, int*& ids)
-{
-    if (albedo4)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dAovAlbedo, &ctx->aovAlbedoCap, pixels * 16, "cudaMalloc AOV albedo4")) return r;
-        albedo4 = ctx->dAovAlbedo;
-    }
-    if (normal4)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dAovNormal, &ctx->aovNormalCap, pixels * 16, "cudaMalloc AOV normal4")) return r;
-        normal4 = ctx->dAovNormal;
-    }
-    if (ids)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dAovIds, &ctx->aovIdsCap, pixels * 4, "cudaMalloc AOV ids")) return r;
-        ids = ctx->dAovIds;
-    }
-    return 0;
 }
 
 int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
@@ -867,56 +896,33 @@ int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, in
     if (width <= 0 || height <= 0 || numFrames <= 0 || frameCount < 0 || numRows < 0 || rowStep <= 0 || row0 < 0)
         return fail_msg(ctx, "tpt_draw_aovs: bad arguments");
     if (numFrames > 256) return fail_msg(ctx, "tpt_draw_aovs: numFrames > 256");
-    if (int r = check_aov_outputs(ctx, "tpt_draw_aovs", albedo4, normal4, ids, buffersOnDevice)) return r;
-    if (numRows == 0)
-    {
-        if (outRayCount) *outRayCount = 0;
-        ctx->lastLaunches = 0;
-        return 0;
-    }
+    if (!albedo4 && !normal4 && !ids) return fail_msg(ctx, "tpt_draw_aovs: albedo4, normal4 and ids are all null");
+    const RowRegion rows = {width, row0, numRows, rowStep, packed};
+    const size_t bufPix = (packed ? (size_t)numRows : (size_t)height) * width;
+    // the float4 outputs are `prev` of the blend when it has weight; ids are not blended
+    const int prev = prev_weight(frameCount, numFrames, testFlags) != 0.0f ? kCopyUp : 0;
+    const bool dev = buffersOnDevice != 0;
+    CallerBuffer bufs[] = {{"albedo4", albedo4, dev, 16, bufPix * 16, kStageAlbedo, prev | kCopyDown, &rows},
+                           {"normal4", normal4, dev, 16, bufPix * 16, kStageNormal, prev | kCopyDown, &rows},
+                           {"ids", ids, dev, 4, bufPix * 4, kStageIds, kCopyDown, &rows, 4}};
+    if (int r = check_buffers(ctx, "tpt_draw_aovs", bufs)) return r;
+    if (numRows == 0) return empty_call(ctx, outRayCount);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw_aovs: rows outside the image");
     if ((long long)numRows * width > 0xffffffe0LL) return fail_msg(ctx, "tpt_draw_aovs: more than 2^32 - 32 pixels");
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-
-    float* dAlbedo = albedo4;
-    float* dNormal = normal4;
-    int* dIds = ids;
-    if (!buffersOnDevice)
-    {
-        const size_t bufPix = (packed ? (size_t)numRows : (size_t)height) * width;
-        if (int r = stage_aov_outputs(ctx, bufPix, dAlbedo, dNormal, dIds)) return r;
-        // the float4 outputs are `prev` of the blend when it has weight; ids are not blended
-        if (prev_weight(frameCount, numFrames, testFlags) != 0.0f)
-        {
-            if (albedo4) CK(copy_rows(dAlbedo, albedo4, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream), "H2D albedo4");
-            if (normal4) CK(copy_rows(dNormal, normal4, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream), "H2D normal4");
-        }
-    }
+    if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
-    DrawParams p;
-    memset(&p, 0, sizeof(p));
-    p.cam = ctx->cam;
-    p.width = width; p.height = height;
-    p.row0 = row0; p.numRows = numRows; p.rowStep = rowStep; p.packed = packed ? 1 : 0;
+    DrawParams p = image_params(ctx, width, height, row0, numRows, rowStep, packed, ctx->spp, testFlags);
     p.frame0 = frameCount; p.numFrames = numFrames;
-    p.spp = ctx->spp;
-    p.flags = testFlags;
-    p.invWidth = 1.0f / (float)width;
-    p.invHeight = 1.0f / (float)height;
     p.rayCounter = ctx->dRayCounters;
-    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
-    cudaError_t e = launch_fast_aovs(p, scene, false, dAlbedo, dNormal, dIds, ctx->numSMs, stream);
+    p.workCounter = next_work_counter(ctx);
+    cudaError_t e = launch_fast_aovs(p, scene, false, (float*)bufs[0].dev, (float*)bufs[1].dev, (int*)bufs[2].dev, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
-    if (!buffersOnDevice)
-    {
-        if (albedo4) CK(copy_rows(albedo4, dAlbedo, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream), "D2H albedo4");
-        if (normal4) CK(copy_rows(normal4, dNormal, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream), "D2H normal4");
-        if (ids) CK(copy_rows(ids, dIds, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream, 4), "D2H ids");
-    }
+    if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !buffersOnDevice, outRayCount, nullptr);
 }
 
@@ -929,48 +935,32 @@ int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     if (!rays6) return fail_msg(ctx, "tpt_trace_aovs: null rays6");
     if (n < 0) return fail_msg(ctx, "tpt_trace_aovs: n < 0");
     if (n > 0xffffffffLL) return fail_msg(ctx, "tpt_trace_aovs: n > 2^32 - 1 (32-bit ray indices)");
-    if (raysOnDevice && ((uintptr_t)rays6 & 3)) return fail_msg(ctx, "tpt_trace_aovs: device rays6 is not 4-byte aligned");
-    if (int r = check_aov_outputs(ctx, "tpt_trace_aovs", albedo4, normal4, ids, outOnDevice)) return r;
-    if (raysOnDevice) { if (int r = check_device_buffer(ctx, rays6, "rays6", "tpt_trace_aovs")) return r; }
-    if (n == 0)
-    {
-        if (outRayCount) *outRayCount = 0;
-        ctx->lastLaunches = 0;
-        return 0;
-    }
+    if (!albedo4 && !normal4 && !ids) return fail_msg(ctx, "tpt_trace_aovs: albedo4, normal4 and ids are all null");
+    const bool dev = outOnDevice != 0;
+    CallerBuffer bufs[] = {{"rays6", (void*)rays6, raysOnDevice != 0, 4, (size_t)n * 24, kStageRays, kCopyUp},
+                           {"albedo4", albedo4, dev, 16, (size_t)n * 16, kStageAlbedo, kCopyDown},
+                           {"normal4", normal4, dev, 16, (size_t)n * 16, kStageNormal, kCopyDown},
+                           {"ids", ids, dev, 4, (size_t)n * 4, kStageIds, kCopyDown}};
+    if (int r = check_buffers(ctx, "tpt_trace_aovs", bufs)) return r;
+    if (n == 0) return empty_call(ctx, outRayCount);
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    const float* dRays = rays6;
-    if (!raysOnDevice)
-    {
-        if (int r = ensure(ctx, (void**)&ctx->dRays, &ctx->raysCap, (size_t)n * 24, "cudaMalloc rays")) return r;
-        CK(cudaMemcpyAsync(ctx->dRays, rays6, (size_t)n * 24, cudaMemcpyHostToDevice, stream), "H2D rays");
-        dRays = ctx->dRays;
-    }
-    float* dAlbedo = albedo4;
-    float* dNormal = normal4;
-    int* dIds = ids;
-    if (!outOnDevice) { if (int r = stage_aov_outputs(ctx, (size_t)n, dAlbedo, dNormal, dIds)) return r; }
+    if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
     DrawParams p;
     memset(&p, 0, sizeof(p));
     p.spp = 1;
     p.numFrames = 1;
     p.rayCounter = ctx->dRayCounters;
-    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
-    p.rays = dRays;
+    p.workCounter = next_work_counter(ctx);
+    p.rays = (const float*)bufs[0].dev;
     p.numRays = (uint32_t)n;
-    cudaError_t e = launch_fast_aovs(p, scene, true, dAlbedo, dNormal, dIds, ctx->numSMs, stream);
+    cudaError_t e = launch_fast_aovs(p, scene, true, (float*)bufs[1].dev, (float*)bufs[2].dev, (int*)bufs[3].dev, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
-    if (!outOnDevice)
-    {
-        if (albedo4) CK(cudaMemcpyAsync(albedo4, dAlbedo, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H albedo4");
-        if (normal4) CK(cudaMemcpyAsync(normal4, dNormal, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H normal4");
-        if (ids) CK(cudaMemcpyAsync(ids, dIds, (size_t)n * 4, cudaMemcpyDeviceToHost, stream), "D2H ids");
-    }
+    if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
 }
 
@@ -989,25 +979,17 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
     if (numPix > (1LL << 32) / spp) return fail_msg(ctx, "tpt_draw_samples: width * height * spp > 2^32 (32-bit sample streams)");
     if (!sum4) return fail_msg(ctx, "tpt_draw_samples: null sum4");
     if (!pixels && n != numPix) return fail_msg(ctx, "tpt_draw_samples: without a pixel list n must be width * height");
-    if (n == 0)
-    {
-        // an empty list: nothing to trace, no buffer is read
-        if (outRayCount) *outRayCount = 0;
-        ctx->lastLaunches = 0;
-        return 0;
-    }
+    // an empty list: nothing to trace, no buffer is read
+    if (n == 0) return empty_call(ctx, outRayCount);
     const long long slab = fast_slab_pixels();
     if (n > 0xffffffffLL || (n + slab - 1) / slab * spp > 0x7fffffffLL)
         return fail_msg(ctx, "tpt_draw_samples: n * spp too large (2^31 slabs of 64 entries x one sample)");
-    if (buffersOnDevice)
-    {
-        if (pixels && ((uintptr_t)pixels & 3)) return fail_msg(ctx, "tpt_draw_samples: device pixels is not 4-byte aligned");
-        if ((uintptr_t)sum4 & 15) return fail_msg(ctx, "tpt_draw_samples: device sum4 is not 16-byte aligned");
-        if (sq4 && ((uintptr_t)sq4 & 15)) return fail_msg(ctx, "tpt_draw_samples: device sq4 is not 16-byte aligned");
-        if (pixels) { if (int r = check_device_buffer(ctx, pixels, "pixels", "tpt_draw_samples")) return r; }
-        if (int r = check_device_buffer(ctx, sum4, "sum4", "tpt_draw_samples")) return r;
-        if (sq4) { if (int r = check_device_buffer(ctx, sq4, "sq4", "tpt_draw_samples")) return r; }
-    }
+    // the outputs accumulate: host sums go up and come back
+    const bool dev = buffersOnDevice != 0;
+    CallerBuffer bufs[] = {{"pixels", (void*)pixels, dev, 4, (size_t)n * 4, kStagePixels, kCopyUp},
+                           {"sum4", sum4, dev, 16, (size_t)n * 16, kStageImage, kCopyUp | kCopyDown},
+                           {"sq4", sq4, dev, 16, (size_t)n * 16, kStageSq4, kCopyUp | kCopyDown}};
+    if (int r = check_buffers(ctx, "tpt_draw_samples", bufs)) return r;
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
@@ -1016,63 +998,27 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
         CK(cudaMalloc(&ctx->dBadPixel, sizeof(unsigned long long)), "cudaMalloc index check");
         CK(cudaMallocHost(&ctx->hBadPixel, sizeof(unsigned long long)), "cudaMallocHost index check");
     }
-    const int* dPixels = pixels;
-    float* dSum = sum4;
-    float* dSq = sq4;
-    if (!buffersOnDevice)
-    {
-        // the outputs accumulate: host sums go up and come back
-        if (pixels)
-        {
-            if (int r = ensure(ctx, (void**)&ctx->dPixels, &ctx->pixelsCap, (size_t)n * 4, "cudaMalloc pixels")) return r;
-            CK(cudaMemcpyAsync(ctx->dPixels, pixels, (size_t)n * 4, cudaMemcpyHostToDevice, stream), "H2D pixels");
-            dPixels = ctx->dPixels;
-        }
-        if (int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, (size_t)n * 16, "cudaMalloc sum4")) return r;
-        CK(cudaMemcpyAsync(ctx->dImage, sum4, (size_t)n * 16, cudaMemcpyHostToDevice, stream), "H2D sum4");
-        dSum = ctx->dImage;
-        if (sq4)
-        {
-            if (int r = ensure(ctx, (void**)&ctx->dSq4, &ctx->sq4Cap, (size_t)n * 16, "cudaMalloc sq4")) return r;
-            CK(cudaMemcpyAsync(ctx->dSq4, sq4, (size_t)n * 16, cudaMemcpyHostToDevice, stream), "H2D sq4");
-            dSq = ctx->dSq4;
-        }
-    }
+    if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
-    DrawParams p;
-    memset(&p, 0, sizeof(p));
-    p.cam = ctx->cam;
-    p.width = width; p.height = height;
-    p.row0 = 0; p.numRows = height; p.rowStep = 1;
+    DrawParams p = image_params(ctx, width, height, 0, height, 1, 0, spp, 0);
     p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
-    p.spp = spp;
-    p.invWidth = 1.0f / (float)width;
-    p.invHeight = 1.0f / (float)height;
-    p.image = dSum;
-    p.sq4 = dSq;
-    p.pixels = dPixels;
+    p.image = (float*)bufs[1].dev;
+    p.sq4 = (float*)bufs[2].dev;
+    p.pixels = (const int*)bufs[0].dev;
     p.numRays = (uint32_t)n;
     p.rayCounter = ctx->dRayCounters;
-    p.workCounter = ctx->dWork + (size_t)(ctx->workSlot++ % tpt_context::kWorkSlots) * 32;
+    p.workCounter = next_work_counter(ctx);
     cudaError_t e = launch_fast_samples(p, scene, ctx->dBadPixel, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     ctx->lastLaunches += fast_samples_launches(p);
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (pixels) CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream), "D2H index check");
-    if (!buffersOnDevice)
-    {
-        CK(cudaMemcpyAsync(sum4, dSum, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H sum4");
-        if (sq4) CK(cudaMemcpyAsync(sq4, dSq, (size_t)n * 16, cudaMemcpyDeviceToHost, stream), "D2H sq4");
-    }
+    if (int r = stage_out(ctx, stream, bufs)) return r;
     // a pixel list makes the call synchronous: its index check is the call's result
     if (int r = finish_call(ctx, stream, 1, !buffersOnDevice || pixels, outRayCount, nullptr)) return r;
     if (pixels && *ctx->hBadPixel != ~0ull)
-    {
-        char msg[200];
-        snprintf(msg, sizeof(msg), "tpt_draw_samples: pixels[%llu] = %d is outside the %d x %d image (nothing was traced)",
-                 *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, width, height);
-        return fail_msg(ctx, msg);
-    }
+        return fail_msgf(ctx, "tpt_draw_samples: pixels[%llu] = %d is outside the %d x %d image (nothing was traced)",
+                         *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, width, height);
     return 0;
 }
 
@@ -1112,10 +1058,11 @@ int tpt_tonemap_rgba8(tpt_context* ctx, const float* image, int imageOnDevice, i
     const float* dIn = image;
     if (!imageOnDevice)
     {
-        int r = ensure(ctx, (void**)&ctx->dImage, &ctx->imageCap, inBytes, "cudaMalloc image");
+        auto& st = ctx->staging[kStageImage];
+        int r = ensure(ctx, &st.ptr, &st.cap, inBytes, "cudaMalloc image");
         if (r) return r;
-        CK(cudaMemcpyAsync(ctx->dImage, image, inBytes, cudaMemcpyHostToDevice, stream), "H2D image");
-        dIn = ctx->dImage;
+        CK(cudaMemcpyAsync(st.ptr, image, inBytes, cudaMemcpyHostToDevice, stream), "H2D image");
+        dIn = (const float*)st.ptr;
     }
     unsigned char* dOut = dst;
     if (!dstOnDevice)
