@@ -117,6 +117,36 @@ __device__ __forceinline__ float4 blend_prev(const DrawParams& p, const float* p
     return make_float4(ax, ay, az, p.zeroAlpha ? 0.0f : __ldg(px + 3));
 }
 
+// Pixel (x, row ri) of the draw's region: image row y = row0 + ri * rowStep, and the pixel's float4 offset in the caller's
+// buffer (row ri of a packed band, row y otherwise).
+struct RegionPixel { int x, y; size_t off; };
+__device__ __forceinline__ RegionPixel region_pixel(const DrawParams& p, int ri, int x)
+{
+    const int y = p.row0 + ri * p.rowStep;
+    return {x, y, (size_t)(p.packed ? ri : y) * p.width + x};
+}
+// Pixel i of the region, counted row-major over its numRows rows; the division is done in i's type.
+template <class I>
+__device__ __forceinline__ RegionPixel region_pixel(const DrawParams& p, I i)
+{
+    const int ri = (int)(i / (I)p.width);
+    return region_pixel(p, ri, (int)(i - (I)ri * (I)p.width));
+}
+
+// A finished tile of region pixels [pix0, pix0 + tilePix) whose radiance sits in acc[3 i ..]: prev * wPrev + acc with one
+// coalesced 128-bit store per pixel (a 128-bit load of prev when it has weight), the accumulators zeroed for the next
+// tile. The CTA's `stride` threads share the loop.
+template <class I, class N>
+__device__ __forceinline__ void write_tile(const DrawParams& p, float* acc, I pix0, N tilePix, float wPrev, N stride)
+{
+    for (N i = threadIdx.x; i < tilePix; i += stride)
+    {
+        float* px = p.image + region_pixel(p, pix0 + (I)i).off * 4;
+        st_stream_f4(px, blend_prev(p, px, wPrev, acc[i * 3 + 0], acc[i * 3 + 1], acc[i * 3 + 2]));
+        acc[i * 3 + 0] = 0.0f; acc[i * 3 + 1] = 0.0f; acc[i * 3 + 2] = 0.0f;
+    }
+}
+
 // ---- variant 0 ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kFastThreads)
 k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes)
@@ -139,7 +169,7 @@ k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
     unsigned rc = 0;
     if (x < p.width && ri < p.numRows)
     {
-        const int y = p.row0 + ri * p.rowStep;
+        const int y = region_pixel(p, ri, x).y;
         SerialHitter<false> hitter;
         V3 acc = v3(0, 0, 0);
         const float invSpp = 1.0f / (float)p.spp;
@@ -154,7 +184,7 @@ k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             }
             acc = acc + col * (invSpp * sW[fi]);
         }
-        float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
+        float* px = p.image + region_pixel(p, ri, x).off * 4;
         st_stream_f4(px, blend_prev(p, px, sWPrev, acc.x, acc.y, acc.z));
     }
     flush_ray_count(p.rayCounter, rc, lane);
@@ -234,12 +264,10 @@ k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlo
                         // samples of one pixel sit in adjacent lanes: coherent primary rays
                         const int pixIn = task / S, sIdx = task % S;
                         const int fi = sIdx / p.spp;
-                        const long long gp = pix0 + pixIn;
-                        const int ri = (int)(gp / p.width), x = (int)(gp % p.width);
-                        const int y = p.row0 + ri * p.rowStep;
-                        st.rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + (uint32_t)(sIdx % p.spp),
+                        const RegionPixel q = region_pixel(p, pix0 + pixIn);
+                        st.rng = pixel_seed((uint32_t)(q.y * p.width + q.x) * (uint32_t)p.spp + (uint32_t)(sIdx % p.spp),
                                             (uint32_t)(p.frame0 + fi));
-                        Ray r = fast_camera_ray(p, x, y, st.rng);
+                        Ray r = fast_camera_ray(p, q.x, q.y, st.rng);
                         st.o = r.orig; st.d = r.dir;
                         st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
                         st.pix = pixIn; st.weight = invSpp * sW[fi];
@@ -352,18 +380,9 @@ k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlo
             }
         }
 
-        // ---- tile done: coalesced 128-bit write-out (+ 128-bit read of prev when accumulating)
+        // ---- tile done
         __syncthreads();
-        const float wPrev = sWPrev;
-        for (int i = threadIdx.x; i < tilePix; i += kFastThreads)
-        {
-            const long long gp = pix0 + i;
-            const int ri = (int)(gp / p.width), x = (int)(gp % p.width);
-            const int y = p.row0 + ri * p.rowStep;
-            float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
-            st_stream_f4(px, blend_prev(p, px, wPrev, sAcc[i * 3 + 0], sAcc[i * 3 + 1], sAcc[i * 3 + 2]));
-            sAcc[i * 3 + 0] = 0.0f; sAcc[i * 3 + 1] = 0.0f; sAcc[i * 3 + 2] = 0.0f;
-        }
+        write_tile(p, sAcc, pix0, tilePix, sWPrev, kFastThreads);
     }
     flush_ray_count(p.rayCounter, rc, lane);
 }
@@ -398,9 +417,7 @@ __global__ void k_prepare_image(DrawParams p, float wPrev)
     const long long idx = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     const long long n = (long long)p.numRows * p.width;
     if (idx >= n) return;
-    const int ri = (int)(idx / p.width), x = (int)(idx % p.width);
-    const int y = p.row0 + ri * p.rowStep;
-    float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
+    float* px = p.image + region_pixel(p, idx).off * 4;
     float4 v = blend_prev(p, px, wPrev, 0.0f, 0.0f, 0.0f);
     *reinterpret_cast<float4*>(px) = v;   // stays in L2 for the reductions that follow
 }
@@ -420,10 +437,10 @@ __device__ __forceinline__ void generate_slab_rays(const DrawParams& p, float4 (
     {
         int x = x0 + (int)q, ri = ri0;
         while (x >= p.width) { x -= p.width; ++ri; }
-        const int y = p.row0 + ri * p.rowStep;
-        uint32_t rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + sample, frame);
-        Ray r = fast_camera_ray(p, x, y, rng);
-        const uint32_t tag = tileBase < 0 ? (uint32_t)((p.packed ? ri : y) * p.width + x) : (uint32_t)tileBase + q;
+        const RegionPixel pix = region_pixel(p, ri, x);
+        uint32_t rng = pixel_seed((uint32_t)(pix.y * p.width + x) * (uint32_t)p.spp + sample, frame);
+        Ray r = fast_camera_ray(p, x, pix.y, rng);
+        const uint32_t tag = tileBase < 0 ? (uint32_t)pix.off : (uint32_t)tileBase + q;
         rays[q][0] = make_float4(r.orig.x, r.orig.y, r.orig.z, __uint_as_float(rng));
         rays[q][1] = make_float4(r.dir.x, r.dir.y, r.dir.z, __uint_as_float(tag));
     }
@@ -512,6 +529,53 @@ struct QPath
     bool doMaterialE;
     bool active;
 };
+
+// A new path from a ray-buffer entry {origin.xyz, rng state} {direction.xyz, tag}. The caller decodes the tag into
+// pixOff and weight.
+__device__ __forceinline__ void begin_path(QPath& st, float4 e0, float4 e1)
+{
+    st.o = v3(e0.x, e0.y, e0.z); st.d = v3(e1.x, e1.y, e1.z);
+    st.rng = __float_as_uint(e0.w);
+    st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
+    st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
+}
+
+// Ray regeneration of the warp-dealt kernels (slab, tile and group queues): the idle lanes take entries [cur, end) of
+// the warp's ray buffer in lane-rank order, the cursor being warp-uniform. When the buffer is used up, refill(p) fetches
+// the next batch and returns kDealRefilled (cur and end reset, the buffer written between two __syncwarp), kDealBlocked
+// (nothing can be fetched this round; the warp traces what it has) or kDealExhausted (the work counter ran out: set
+// `exhausted`, no more fetches). start(tag) decodes an entry's tag for the lane that took it.
+// (p is handed to refill rather than captured: a lambda holding the address of the body's by-value DrawParams made
+// the compiler load every field into registers at kernel entry, +1 register and up to 8 B of spills.)
+enum DealResult { kDealRefilled, kDealBlocked, kDealExhausted };
+template <class Refill, class Start>
+__device__ __forceinline__ void deal_paths(const DrawParams& p, QPath& st, const float4 (*rays)[2], uint32_t& cur, uint32_t& end,
+                                           bool& exhausted, int lane, Refill&& refill, Start&& start)
+{
+    const unsigned ltMask = (1u << lane) - 1u;
+    unsigned need = __ballot_sync(0xffffffffu, !st.active);
+    while (need && !exhausted)
+    {
+        if (cur >= end)
+        {
+            const DealResult r = refill(p);
+            if (r == kDealExhausted) { exhausted = true; break; }
+            if (r == kDealBlocked) break;
+        }
+        const uint32_t avail = end - cur;
+        const uint32_t rank = (uint32_t)__popc(need & ltMask);
+        if (!st.active && rank < avail)
+        {
+            const float4 e0 = rays[cur + rank][0];
+            const float4 e1 = rays[cur + rank][1];
+            begin_path(st, e0, e1);
+            start(__float_as_uint(e1.w));
+        }
+        const uint32_t n = (uint32_t)__popc(need);
+        cur += n < avail ? n : avail;
+        need = __ballot_sync(0xffffffffu, !st.active);
+    }
+}
 
 // Fast-mode sweep in expanded form: with od = o.d, oo = o.o and K = |s|^2 - r^2 (per sphere, computed once per CTA in
 // double precision) nb = s.d - od and c = K + oo - 2 s.o, i.e. 8 instead of 10 FP32 issue slots per (ray, sphere):
@@ -1044,16 +1108,13 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     SceneView sc = make_view<THREADS == 128>(smem, blob, L, stagedBytes, count, nLights);
     const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
-    const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = SRC != kSrcCamera ? p.numRays : (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
-    
+
     unsigned rc = 0;
 
     // warp-uniform slab cursor
     uint32_t slabCur = 0, slabEnd = 0;
-    int slabX0 = 0, slabRi0 = 0;
-    uint32_t slabSample = 0, slabFrame = 0;
     float slabW = 0.0f;
     bool exhausted = false;
     // progress reporting for host-buffer draws (bandDone != nullptr): slabs are dealt in pixel order, so the image
@@ -1071,59 +1132,36 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     st.active = false;
     for (;;)
     {
-        // ---- regeneration
-        unsigned need = __ballot_sync(0xffffffffu, !st.active);
-        while (need && !exhausted)
-        {
-            if (slabCur >= slabEnd)
-            {
-                uint32_t slab = 0;
-                if (lane == 0) slab = atomicAdd(p.workCounter, 1u);
-                slab = __shfl_sync(0xffffffffu, slab, 0);
-                if (slab >= numSlabs) { exhausted = true; break; }
-                uint32_t mtile = slab / S;
-                const uint32_t s = slab - mtile * S;
-                // progress mode: walk the image from its LAST macro-tile to its first. Row 0 is the bottom of the image
-                // (ground, light sampling: the expensive pixels); starting with the cheap upper rows makes pixels
-                // complete early at a high rate, so most of the D2H runs under the expensive rows' tracing.
-                if (bandDone) mtile = (numSlabs / S) - 1u - mtile;
-                const uint32_t pix0 = mtile * kSlabPix;
-                slabEnd = regionPix - pix0 < (uint32_t)kSlabPix ? regionPix - pix0 : (uint32_t)kSlabPix;
-                slabCur = 0;
-                if constexpr (SRC == kSrcCamera)
-                {
-                    slabRi0 = (int)(pix0 / (uint32_t)p.width);
-                    slabX0 = (int)(pix0 - (uint32_t)slabRi0 * (uint32_t)p.width);
-                }
-                const uint32_t fi = s / (uint32_t)p.spp;
-                slabSample = s - fi * (uint32_t)p.spp;
-                slabFrame = (uint32_t)p.frame0 + fi;
-                slabW = invSpp * sW[fi];
-                slabBand = bandDone ? mtile / mtilesPerBand : 0u;
-                __syncwarp();       // every lane has popped what it needed from the previous slab
-                if constexpr (SRC == kSrcRays) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
-                else if constexpr (SRC == kSrcPixels) generate_list_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, slabSample, slabFrame);
-                else generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, slabX0, slabRi0, slabSample, slabFrame, -1);
-                __syncwarp();
-            }
-            const uint32_t avail = slabEnd - slabCur;
-            const uint32_t rank = (uint32_t)__popc(need & ltMask);
-            if (!st.active && rank < avail)
-            {
-                const float4 e0 = sRays[threadIdx.x >> 5][slabCur + rank][0];
-                const float4 e1 = sRays[threadIdx.x >> 5][slabCur + rank][1];
-                st.o = v3(e0.x, e0.y, e0.z); st.d = v3(e1.x, e1.y, e1.z);
-                st.rng = __float_as_uint(e0.w);
-                st.pixOff = __float_as_uint(e1.w);
-                st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
-                st.weight = slabW;
-                myBand = slabBand;
-                st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
-            }
-            const uint32_t n = (uint32_t)__popc(need);
-            slabCur += n < avail ? n : avail;
-            need = __ballot_sync(0xffffffffu, !st.active);
-        }
+        // a slab from the global counter: its rays into the warp's buffer, tag = image float4 offset (camera rays) or entry.
+        // (Defined inside the loop: defined above it, the 768-thread KFORM 0 k_fast_samples instances took one more register.)
+        auto refill = [&](const DrawParams& p) {
+            uint32_t slab = 0;
+            if (lane == 0) slab = atomicAdd(p.workCounter, 1u);
+            slab = __shfl_sync(0xffffffffu, slab, 0);
+            if (slab >= numSlabs) return kDealExhausted;
+            uint32_t mtile = slab / S;
+            const uint32_t s = slab - mtile * S;
+            // progress mode: walk the image from its LAST macro-tile to its first. Row 0 is the bottom of the image
+            // (ground, light sampling: the expensive pixels); starting with the cheap upper rows makes pixels
+            // complete early at a high rate, so most of the D2H runs under the expensive rows' tracing.
+            if (bandDone) mtile = (numSlabs / S) - 1u - mtile;
+            const uint32_t pix0 = mtile * kSlabPix;
+            slabEnd = regionPix - pix0 < (uint32_t)kSlabPix ? regionPix - pix0 : (uint32_t)kSlabPix;
+            slabCur = 0;
+            const int ri0 = (int)(pix0 / (uint32_t)p.width), x0 = (int)(pix0 - (uint32_t)ri0 * (uint32_t)p.width);
+            const uint32_t fi = s / (uint32_t)p.spp;
+            const uint32_t sample = s - fi * (uint32_t)p.spp, frame = (uint32_t)p.frame0 + fi;
+            slabW = invSpp * sW[fi];
+            slabBand = bandDone ? mtile / mtilesPerBand : 0u;
+            __syncwarp();       // every lane has popped what it needed from the previous slab
+            if constexpr (SRC == kSrcRays) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, sample, frame);
+            else if constexpr (SRC == kSrcPixels) generate_list_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, sample, frame);
+            else generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, x0, ri0, sample, frame, -1);
+            __syncwarp();
+            return kDealRefilled;
+        };
+        deal_paths(p, st, sRays[threadIdx.x >> 5], slabCur, slabEnd, exhausted, lane, refill,
+                   [&](uint32_t tag) { st.pixOff = tag; st.weight = slabW; myBand = slabBand; });
         if (!__any_sync(0xffffffffu, st.active)) break;
 #if TPT_TRACE_WARPS
         if (!trReady) trReady = gtimer();
@@ -1258,12 +1296,10 @@ __device__ __forceinline__ void generate_group_rays(const DrawParams& p, float4 
     {
         const uint32_t sl = npix == (uint32_t)kGroupPix ? q >> 4 : q / npix;
         const uint32_t px = q - sl * npix;
-        const uint32_t gp = pix0 + px;
-        const int ri = (int)(gp / (uint32_t)p.width), x = (int)(gp - (uint32_t)ri * (uint32_t)p.width);
-        const int y = p.row0 + ri * p.rowStep;
+        const RegionPixel g = region_pixel(p, pix0 + px);
         const uint32_t s = s0 + sl, fi = s / (uint32_t)p.spp, ss = s - fi * (uint32_t)p.spp;
-        uint32_t rng = pixel_seed((uint32_t)(y * p.width + x) * (uint32_t)p.spp + ss, (uint32_t)p.frame0 + fi);
-        Ray r = fast_camera_ray(p, x, y, rng);
+        uint32_t rng = pixel_seed((uint32_t)(g.y * p.width + g.x) * (uint32_t)p.spp + ss, (uint32_t)p.frame0 + fi);
+        Ray r = fast_camera_ray(p, g.x, g.y, rng);
         rays[q][0] = make_float4(r.orig.x, r.orig.y, r.orig.z, __uint_as_float(rng));
         rays[q][1] = make_float4(r.dir.x, r.dir.y, r.dir.z, __uint_as_float(px | (slot << 4) | (fi << 8)));
     }
@@ -1289,7 +1325,6 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     SceneView sc = make_view<ALLS>(smem, blob, L, stagedBytes, count, nLights);     // ALLS: whole blob staged -> LDS for every section
     const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
     unsigned rc = 0;
@@ -1300,53 +1335,37 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     uint32_t grpPix0 = 0, grpNpix = 0, curSlot = 0, groupsOpened = 0;
     bool exhausted = false;
 
+    // the next chunk of up to 4 sample indices of the current group, opening a new group when it has none left
+    auto refill = [&](const DrawParams& p) {
+        if (sNext >= S)
+        {
+            const uint32_t slot = groupsOpened % (uint32_t)kGroupOpen;
+            if (sRemain[warp][slot] != 0) return kDealBlocked;     // that slot's group still has paths in flight: trace them first
+            uint32_t g = 0;
+            if (lane == 0) g = atomicAdd(p.workCounter, 1u);
+            g = __shfl_sync(0xffffffffu, g, 0);
+            if (g >= numGroups) return kDealExhausted;
+            grpPix0 = g * (uint32_t)kGroupPix;
+            grpNpix = regionPix - grpPix0 < (uint32_t)kGroupPix ? regionPix - grpPix0 : (uint32_t)kGroupPix;
+            curSlot = slot; ++groupsOpened; sNext = 0;
+            if (lane == 0) { sRemain[warp][slot] = (int)(grpNpix * S); sGrpPix0[warp][slot] = grpPix0; }
+        }
+        const uint32_t ns = S - sNext < 4u ? S - sNext : 4u;
+        __syncwarp();       // every lane has popped what it needed from the previous chunk
+        generate_group_rays(p, sRays[warp], lane, grpNpix, ns, grpPix0, sNext, curSlot);
+        __syncwarp();
+        chunkCur = 0; chunkEnd = grpNpix * ns; sNext += ns;
+        return kDealRefilled;
+    };
+
     QPath st;
     st.active = false;
     for (;;)
     {
-        // ---- regeneration
-        unsigned need = __ballot_sync(0xffffffffu, !st.active);
-        while (need && !exhausted)
-        {
-            if (chunkCur >= chunkEnd)
-            {
-                if (sNext >= S)
-                {
-                    const uint32_t slot = groupsOpened % (uint32_t)kGroupOpen;
-                    if (sRemain[warp][slot] != 0) break;        // that slot's group still has paths in flight: trace them first
-                    uint32_t g = 0;
-                    if (lane == 0) g = atomicAdd(p.workCounter, 1u);
-                    g = __shfl_sync(0xffffffffu, g, 0);
-                    if (g >= numGroups) { exhausted = true; break; }
-                    grpPix0 = g * (uint32_t)kGroupPix;
-                    grpNpix = regionPix - grpPix0 < (uint32_t)kGroupPix ? regionPix - grpPix0 : (uint32_t)kGroupPix;
-                    curSlot = slot; ++groupsOpened; sNext = 0;
-                    if (lane == 0) { sRemain[warp][slot] = (int)(grpNpix * S); sGrpPix0[warp][slot] = grpPix0; }
-                }
-                const uint32_t ns = S - sNext < 4u ? S - sNext : 4u;
-                __syncwarp();       // every lane has popped what it needed from the previous chunk
-                generate_group_rays(p, sRays[warp], lane, grpNpix, ns, grpPix0, sNext, curSlot);
-                __syncwarp();
-                chunkCur = 0; chunkEnd = grpNpix * ns; sNext += ns;
-            }
-            const uint32_t avail = chunkEnd - chunkCur;
-            const uint32_t rank = (uint32_t)__popc(need & ltMask);
-            if (!st.active && rank < avail)
-            {
-                const float4 e0 = sRays[warp][chunkCur + rank][0];
-                const float4 e1 = sRays[warp][chunkCur + rank][1];
-                st.o = v3(e0.x, e0.y, e0.z); st.d = v3(e1.x, e1.y, e1.z);
-                st.rng = __float_as_uint(e0.w);
-                const uint32_t tag = __float_as_uint(e1.w);
-                st.pixOff = tag & 0xffu;                         // px | slot << 4
-                st.weight = invSpp * sW[tag >> 8];
-                st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
-                st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
-            }
-            const uint32_t n = (uint32_t)__popc(need);
-            chunkCur += n < avail ? n : avail;
-            need = __ballot_sync(0xffffffffu, !st.active);
-        }
+        deal_paths(p, st, sRays[warp], chunkCur, chunkEnd, exhausted, lane, refill, [&](uint32_t tag) {
+            st.pixOff = tag & 0xffu;                         // px | slot << 4
+            st.weight = invSpp * sW[tag >> 8];
+        });
         if (!__any_sync(0xffffffffu, st.active)) break;
 
         bool lastOfGroup = false;
@@ -1370,10 +1389,7 @@ fast_group_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             const uint32_t npix = regionPix - pix0 < (uint32_t)kGroupPix ? regionPix - pix0 : (uint32_t)kGroupPix;
             if ((uint32_t)lane < npix)
             {
-                const uint32_t gp = pix0 + (uint32_t)lane;
-                const int ri = (int)(gp / (uint32_t)p.width), x = (int)(gp - (uint32_t)ri * (uint32_t)p.width);
-                const int y = p.row0 + ri * p.rowStep;
-                float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
+                float* px = p.image + region_pixel(p, pix0 + (uint32_t)lane).off * 4;
                 const float4 a = sAcc[warp][slot][lane];
                 st_stream_f4(px, blend_prev(p, px, wPrev, a.x, a.y, a.z));
                 sAcc[warp][slot][lane] = make_float4(0, 0, 0, 0);
@@ -1427,7 +1443,6 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
     const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
     const int lane = threadIdx.x & 31;
-    const unsigned ltMask = (1u << lane) - 1u;
     const uint32_t regionPix = (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
     unsigned rc = 0;
@@ -1444,56 +1459,34 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
         const uint32_t slabsPerSample = (tilePix + kSlabPix - 1) / kSlabPix;
         const uint32_t tileSlabs = slabsPerSample * S;
 
-        uint32_t slabCur = 0, slabEnd = 0, slabQ0 = 0;
-        int slabX0 = 0, slabRi0 = 0;
-        uint32_t slabSample = 0, slabFrame = 0;
+        uint32_t slabCur = 0, slabEnd = 0;
         float slabW = 0.0f;
         bool exhausted = false;
+        // a slab of the tile from the CTA's counter, tag = pixel index inside the tile
+        auto refill = [&](const DrawParams& p) {
+            uint32_t slab = 0;
+            if (lane == 0) slab = atomicAdd(&sSlab, 1u);
+            slab = __shfl_sync(0xffffffffu, slab, 0);
+            if (slab >= tileSlabs) return kDealExhausted;
+            const uint32_t s = slab / slabsPerSample, g = slab - s * slabsPerSample;   // sample-major inside the tile
+            const uint32_t q0 = g * kSlabPix;
+            slabEnd = tilePix - q0 < (uint32_t)kSlabPix ? tilePix - q0 : (uint32_t)kSlabPix;
+            slabCur = 0;
+            const uint32_t pix0 = tilePix0 + q0;
+            const int ri0 = (int)(pix0 / (uint32_t)p.width), x0 = (int)(pix0 - (uint32_t)ri0 * (uint32_t)p.width);
+            const uint32_t fi = s / (uint32_t)p.spp;
+            slabW = invSpp * sW[fi];
+            __syncwarp();
+            generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, x0, ri0, s - fi * (uint32_t)p.spp, (uint32_t)p.frame0 + fi, (int)q0);
+            __syncwarp();
+            return kDealRefilled;
+        };
         QPath st;
         st.active = false;
         for (;;)
         {
-            unsigned need = __ballot_sync(0xffffffffu, !st.active);
-            while (need && !exhausted)
-            {
-                if (slabCur >= slabEnd)
-                {
-                    uint32_t slab = 0;
-                    if (lane == 0) slab = atomicAdd(&sSlab, 1u);
-                    slab = __shfl_sync(0xffffffffu, slab, 0);
-                    if (slab >= tileSlabs) { exhausted = true; break; }
-                    const uint32_t s = slab / slabsPerSample, g = slab - s * slabsPerSample;   // sample-major inside the tile
-                    slabQ0 = g * kSlabPix;
-                    slabEnd = tilePix - slabQ0 < (uint32_t)kSlabPix ? tilePix - slabQ0 : (uint32_t)kSlabPix;
-                    slabCur = 0;
-                    const uint32_t pix0 = tilePix0 + slabQ0;
-                    slabRi0 = (int)(pix0 / (uint32_t)p.width);
-                    slabX0 = (int)(pix0 - (uint32_t)slabRi0 * (uint32_t)p.width);
-                    const uint32_t fi = s / (uint32_t)p.spp;
-                    slabSample = s - fi * (uint32_t)p.spp;
-                    slabFrame = (uint32_t)p.frame0 + fi;
-                    slabW = invSpp * sW[fi];
-                    __syncwarp();
-                    generate_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, slabX0, slabRi0, slabSample, slabFrame, (int)slabQ0);
-                    __syncwarp();
-                }
-                const uint32_t avail = slabEnd - slabCur;
-                const uint32_t rank = (uint32_t)__popc(need & ltMask);
-                if (!st.active && rank < avail)
-                {
-                    const float4 e0 = sRays[threadIdx.x >> 5][slabCur + rank][0];
-                    const float4 e1 = sRays[threadIdx.x >> 5][slabCur + rank][1];
-                    st.o = v3(e0.x, e0.y, e0.z); st.d = v3(e1.x, e1.y, e1.z);
-                    st.rng = __float_as_uint(e0.w);
-                    st.pixOff = __float_as_uint(e1.w);      // pixel index inside the tile
-                    st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
-                    st.weight = slabW;
-                    st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
-                }
-                const uint32_t n = (uint32_t)__popc(need);
-                slabCur += n < avail ? n : avail;
-                need = __ballot_sync(0xffffffffu, !st.active);
-            }
+            deal_paths(p, st, sRays[threadIdx.x >> 5], slabCur, slabEnd, exhausted, lane, refill,
+                       [&](uint32_t tag) { st.pixOff = tag; st.weight = slabW; });
             if (!__any_sync(0xffffffffu, st.active)) break;
             if (path_step<kLsRuntime>(sc, st, rc, hitter))
             {
@@ -1504,17 +1497,9 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
             }
         }
 
-        // ---- tile finished: coalesced 128-bit write-out (possibly into a peer GPU's memory)
+        // ---- tile finished (the stores may go to a peer GPU's memory)
         __syncthreads();
-        for (uint32_t i = threadIdx.x; i < tilePix; i += kQueueThreads)
-        {
-            const uint32_t gp = tilePix0 + i;
-            const int ri = (int)(gp / (uint32_t)p.width), x = (int)(gp - (uint32_t)ri * (uint32_t)p.width);
-            const int y = p.row0 + ri * p.rowStep;
-            float* px = p.image + ((size_t)(p.packed ? ri : y) * p.width + x) * 4;
-            st_stream_f4(px, blend_prev(p, px, wPrev, sAcc[i * 3 + 0], sAcc[i * 3 + 1], sAcc[i * 3 + 2]));
-            sAcc[i * 3 + 0] = 0.0f; sAcc[i * 3 + 1] = 0.0f; sAcc[i * 3 + 2] = 0.0f;
-        }
+        write_tile(p, sAcc, tilePix0, tilePix, wPrev, (uint32_t)kQueueThreads);
     }
     flush_ray_count(p.rayCounter, rc, lane);
 }
@@ -2138,8 +2123,8 @@ k_fast_aov(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout
         }
         else
         {
-            const int ri = (int)(i / (uint32_t)p.width), x = (int)(i - (uint32_t)ri * (uint32_t)p.width);
-            const int y = p.row0 + ri * p.rowStep;
+            const RegionPixel q = region_pixel(p, i);
+            const int x = q.x, y = q.y;
             for (int fi = 0; fi < p.numFrames; ++fi)
             {
                 AovSample fs{v3(0, 0, 0), v3(0, 0, 0), 0.0f, 0.0f};
@@ -2157,7 +2142,7 @@ k_fast_aov(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout
                 acc.albedo = acc.albedo + fs.albedo * w; acc.normal = acc.normal + fs.normal * w;
                 acc.cov += fs.cov * w; acc.t += fs.t * w;
             }
-            off = (size_t)(p.packed ? ri : y) * p.width + x;
+            off = q.off;
         }
         float4 va = make_float4(acc.albedo.x, acc.albedo.y, acc.albedo.z, acc.cov);
         float4 vn = make_float4(acc.normal.x, acc.normal.y, acc.normal.z, acc.t);
