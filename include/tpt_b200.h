@@ -80,8 +80,10 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * the next), "host_progress" (default 1: with fast variant 3/4 a single kernel publishes per-band completion counters and the
  * copy stream waits on them with cuStreamWaitValue32, "progress_bands" bands, default 4; 0 falls back to host_bands),
  * "fast_kform" (fast kernels' sphere sweep: 0 reference form, 1 expanded form, 2 (default) expanded form on a pair-interleaved
- * sphere array, one 128-bit shared load per coordinate of two spheres; 1 and 2 only when the scene passes the gate in
- * tpt_set_scene — a scene that fails it gets, with 2, the packed sweep made conservative by a folded-in error bound
+ * sphere array, one 128-bit shared load per coordinate of two spheres — the slab queue of a scene of at most 64 padded
+ * spheres takes that array in its kernel parameters instead, so its first pass reads the spheres as constant operands;
+ * 3 as 2 but with the array always in shared memory, for A/B comparisons; 1, 2 and 3 only when the scene passes the gate in
+ * tpt_set_scene — a scene that fails it gets, with 2 or 3, the packed sweep made conservative by a folded-in error bound
  * plus reference-form hit decisions, and the reference form otherwise; per context), "fast_alpha_zero" (default 0; 1: fast-mode draws whose `prev` has zero weight write
  * alpha = 0 instead of keeping the buffer's alpha — saves the read over NVLink when the buffer is a peer GPU's),
  * "exact_lookahead" (default 0; L > 1: an exact-mode draw of ONE frame that misses the cache traces frames [f, f+L) in a
@@ -258,7 +260,8 @@ int tpt_ipc_close(tpt_context* ctx, void* devPtr);
 int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long long n);
 /* Diagnostic used by the parity tests: nearest hit (HitWorld, Test.cpp:85-106) of n host rays {o.xyz, d.xyz} in the
  * current scene with one sweep form of the fast kernels (kform 0 reference form, 1 expanded, 2 expanded on packed pairs,
- * 3 conservative packed pass + reference-form decisions), tMin/tMax as Trace uses them. outId -1 = miss. */
+ * 3 conservative packed pass + reference-form decisions, 4 expanded on packed pairs read from the kernel parameters: scenes
+ * of at most 64 padded spheres only), tMin/tMax as Trace uses them. outId -1 = miss. */
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays6, int* outId, float* outT, long long n);
 /* Diagnostic: device timestamps (ms since the start of the last progress-mode host draw) of the trace kernel's end,
  * each band copy's end and the draw's end. Returns minus the number of entries written. */

@@ -518,8 +518,7 @@ struct QPath
     V3 nextDir;
     V3 thrAlb;
     V3 nl;
-    V3 pend;
-    V3 albedo;
+    float pend;       // m * omega / pi of the shadow ray in flight: it adds thrAlb * E_light * pend when it hits its light
     uint32_t rng;
     uint32_t pixOff;  // float4 index of the pixel in the image buffer
     float weight;
@@ -667,19 +666,43 @@ __device__ __forceinline__ void build_sphK(const SceneView& sc, float4* sphInSme
 //   2 LOP3 + 2 SHF (sign bits into the candidate mask).
 // -c and discr are the exact negations/equals of FastHitterK's c and discr (same products, IEEE negation symmetry), so pass
 // 2 — unchanged, on the {s, K} array — sees the same candidates it would have computed itself.
-// Packed-pair pass 1 shared by FastHitterK2 / FastHitterK2C: spheres [s0, s0+G) = G/2 pairs of the pair array at shared
-// address sphP; shifts G rejection signs into `neg` (sphere s0 ends up at the highest of the G new bits).
+// Where pass 1 reads the pair array from: shared memory at address sphP (two LDS.128 per pair), or the kernel parameter
+// (ParamPairs, sweep form 4), where every index is a compile-time constant: ptxas (12.9, sm_90a) then loads the values into
+// uniform registers (ULDC.64, two per instruction) that the FFMAs read, with no vector register and no shared-memory
+// latency per value. kOneChunk: the scene has at most 64 padded spheres, so the sweep is a single chunk at base 0.
+struct SmemPairs
+{
+    static constexpr bool kOneChunk = false;
+    uint32_t sphP;
+    __device__ __forceinline__ void load(int pair, float& x0, float& x1, float& y0, float& y1, float& z0, float& z1, float& k0, float& k1) const
+    {
+        const uint32_t a = sphP + (uint32_t)pair * 32u;
+        asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(x0), "=f"(x1), "=f"(y0), "=f"(y1) : "r"(a));
+        asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(z0), "=f"(z1), "=f"(k0), "=f"(k1) : "r"(a + 16u));
+    }
+};
+struct ParamPairsRef
+{
+    static constexpr bool kOneChunk = true;
+    const ParamPairs* pp;       // the kernel's __grid_constant__ parameter
+    __device__ __forceinline__ void load(int pair, float& x0, float& x1, float& y0, float& y1, float& z0, float& z1, float& k0, float& k1) const
+    {
+        const float* f = pp->f + pair * 8;
+        x0 = f[0]; x1 = f[1]; y0 = f[2]; y1 = f[3]; z0 = f[4]; z1 = f[5]; k0 = f[6]; k1 = f[7];
+    }
+};
+
+// Packed-pair pass 1 shared by FastHitterK2 / FastHitterKC / FastHitterK2C: spheres [s0, s0+G) = G/2 pairs of the pair
+// array; shifts G rejection signs into `neg` (sphere s0 ends up at the highest of the G new bits).
 struct SweepConsts { float DX, DY, DZ, NOD, BX, BY, BZ, NOO; };
-template <int G>
-__device__ __forceinline__ void sweep_full(uint32_t sphP, int s0, uint32_t& neg, const SweepConsts& c)
+template <int G, class P>
+__device__ __forceinline__ void sweep_full(const P& pairs, int s0, uint32_t& neg, const SweepConsts& c)
 {
 #pragma unroll
     for (int j = 0; j < G; j += 2)
     {
         float x0, x1, y0, y1, z0, z1, k0, k1;
-        const uint32_t a = sphP + (uint32_t)((s0 + j) >> 1) * 32u;
-        asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(x0), "=f"(x1), "=f"(y0), "=f"(y1) : "r"(a));
-        asm("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(z0), "=f"(z1), "=f"(k0), "=f"(k1) : "r"(a + 16u));
+        pairs.load((s0 + j) >> 1, x0, x1, y0, y1, z0, z1, k0, k1);
         const float nb0 = fmaf(x0, c.DX, fmaf(y0, c.DY, fmaf(z0, c.DZ, c.NOD)));
         const float nb1 = fmaf(x1, c.DX, fmaf(y1, c.DY, fmaf(z1, c.DZ, c.NOD)));
         const float negc0 = fmaf(x0, c.BX, fmaf(y0, c.BY, fmaf(z0, c.BZ, __fadd_rn(k0, c.NOO))));
@@ -695,40 +718,44 @@ __device__ __forceinline__ void sweep_full(uint32_t sphP, int s0, uint32_t& neg,
 // The straight-line group between two (warp-uniform) bounds checks is the instruction scheduler's window: a group of 16
 // spheres keeps sixteen independent chains in flight. Counts that are not a multiple of the group fall through to halved
 // groups, down to 4.
-template <int G>
-__device__ __forceinline__ void sweep_upto(uint32_t sphP, int s0, int left, uint32_t& neg, const SweepConsts& c)
+template <int G, class P>
+__device__ __forceinline__ void sweep_upto(const P& pairs, int s0, int left, uint32_t& neg, const SweepConsts& c)
 {
-    if (left >= G) sweep_full<G>(sphP, s0, neg, c);
+    if (left >= G) sweep_full<G>(pairs, s0, neg, c);
     else if constexpr (G > 4)
     {
         if (left > 0)
         {
-            sweep_upto<G / 2>(sphP, s0, left, neg, c);
-            sweep_upto<G / 2>(sphP, s0 + G / 2, left - G / 2, neg, c);
+            sweep_upto<G / 2>(pairs, s0, left, neg, c);
+            sweep_upto<G / 2>(pairs, s0 + G / 2, left - G / 2, neg, c);
         }
     }
 }
 // 64 spheres [base, base+n) -> candidate mask, sphere base + J <-> bit 63 - J (n a multiple of 4, 4 <= n <= 64)
-__device__ __forceinline__ unsigned long long sweep_chunk64(uint32_t sphP, int base, int n, const SweepConsts& c)
+template <class P>
+__device__ __forceinline__ unsigned long long sweep_chunk64(const P& pairs, int base, int n, const SweepConsts& c)
 {
     const int n0 = n < 32 ? n : 32, n1 = n - n0;
     uint32_t neg0 = 0, neg1 = 0;
 #pragma unroll
-    for (int k = 0; k < 32; k += TPT_P1_GROUP) sweep_upto<TPT_P1_GROUP>(sphP, base + k, n0 - k, neg0, c);
+    for (int k = 0; k < 32; k += TPT_P1_GROUP) sweep_upto<TPT_P1_GROUP>(pairs, base + k, n0 - k, neg0, c);
     if (n1 > 0)
     {
 #pragma unroll
-        for (int k = 0; k < 32; k += TPT_P1_GROUP) sweep_upto<TPT_P1_GROUP>(sphP, base + 32 + k, n1 - k, neg1, c);
+        for (int k = 0; k < 32; k += TPT_P1_GROUP) sweep_upto<TPT_P1_GROUP>(pairs, base + 32 + k, n1 - k, neg1, c);
     }
     // left-align: after n shifts sphere j of the round sits at bit n-1-j
     const uint32_t c0 = ~neg0 << (32 - n0);
     const uint32_t c1 = n1 > 0 ? ~neg1 << (32 - n1) : 0u;
     return ((unsigned long long)c0 << 32) | c1;
 }
-struct FastHitterK2
+// FastHitterK2: pass 1 on the pair array in shared memory; FastHitterKC: on the pair array in the kernel parameter (scenes
+// of at most 64 padded spheres). Same values in the same operations: ids and distances are bit-identical.
+template <class P>
+struct FastHitterK2T
 {
     uint32_t sphK;      // shared-memory address of {sx, sy, sz, K}[simdCount]         (pass 2)
-    uint32_t sphP;      // shared-memory address of the pair array, 32 B per pair       (pass 1)
+    P pairs;            // the pair array, 32 B per pair                                (pass 1)
     int simdCount;
     __device__ __forceinline__ float4 ld(int i) const
     {
@@ -747,9 +774,9 @@ struct FastHitterK2
         float bestT = tMax;
         int bestId = -1;
         // chunks of 64 spheres: pass 1 fills a 64-bit candidate mask (sphere base + J <-> bit 63 - J), pass 2 walks it
-        for (int base = 0; base < simdCount; base += 64)
+        for (int base = 0; base < (P::kOneChunk ? 1 : simdCount); base += 64)
         {
-            unsigned long long cand = sweep_chunk64(sphP, base, simdCount - base < 64 ? simdCount - base : 64, C);
+            unsigned long long cand = sweep_chunk64(pairs, base, simdCount - base < 64 ? simdCount - base : 64, C);
             // pass 2, two candidates per trip (independent LDS.128 / 9 FMA / MUFU chains); ascending sphere order as before
             while (cand)
             {
@@ -776,6 +803,8 @@ struct FastHitterK2
         return bestId;
     }
 };
+using FastHitterK2 = FastHitterK2T<SmemPairs>;
+using FastHitterKC = FastHitterK2T<ParamPairsRef>;
 
 // Conservative form for scenes the expanded form is NOT accurate enough for (centres far from the origin: the gate in
 // tpt_set_scene fails, e.g. the 4096-sphere stress scene): pass 1 is the packed expanded-form sweep with an error bound
@@ -804,7 +833,7 @@ struct FastHitterK2C
         int bestId = -1;
         for (int base = 0; base < simdCount; base += 64)
         {
-            unsigned long long cand = sweep_chunk64(sphP, base, simdCount - base < 64 ? simdCount - base : 64, C);
+            unsigned long long cand = sweep_chunk64(SmemPairs{sphP}, base, simdCount - base < 64 ? simdCount - base : 64, C);
             // pass 2 on the untouched {s, r^2} array in the reference form (Maths.cpp:97-102), two candidates per trip
             while (cand)
             {
@@ -885,14 +914,17 @@ __host__ __device__ inline FastSmem fast_smem(uint32_t stagedBytes, uint32_t pai
 //   1  expanded form: {s, r^2} rewritten to {s, K} in place (FastHitterK)
 //   2  expanded form on the pair array, built from {s, K} (FastHitterK2)
 //   3  conservative pair array built from {s, r^2}, which stays for the reference-form pass 2 (FastHitterK2C)
+//   4  form 2 with the pair array in the kernel parameter pp (FastHitterKC; at most kParamPairSpheres padded spheres),
+//      no pair array in shared memory; pass 2 on {s, K} as in form 2
 // The sweep's loads are plain (schedulable) asm: their addresses are made opaque AFTER the barrier so that none of them
 // can be hoisted above the rewrite of the sphere array or the construction of the pair array.
 template <int KFORM>
-__device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char* smem, const SceneBlobLayout& L, uint32_t stagedBytes)
+__device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char* smem, const SceneBlobLayout& L, uint32_t stagedBytes,
+                                              const ParamPairs* pp = nullptr)
 {
     float4* sph = reinterpret_cast<float4*>(smem + L.offSph);
     float4* pairs = reinterpret_cast<float4*>(smem + fast_smem(stagedBytes).pairs);
-    if constexpr (KFORM == 1 || KFORM == 2) build_sphK(sc, sph);
+    if constexpr (KFORM == 1 || KFORM == 2 || KFORM == 4) build_sphK(sc, sph);
     __syncthreads();
     if constexpr (KFORM == 0) return SerialHitter<false>();
     else if constexpr (KFORM == 1)
@@ -905,8 +937,14 @@ __device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char
     {
         build_sph_pairs(sc, sph, pairs);
         __syncthreads();
-        FastHitterK2 h; h.sphK = sc.sphShared; h.sphP = smem_u32(pairs); h.simdCount = sc.simdCount;
-        asm volatile("" : "+r"(h.sphK), "+r"(h.sphP));
+        FastHitterK2 h; h.sphK = sc.sphShared; h.pairs.sphP = smem_u32(pairs); h.simdCount = sc.simdCount;
+        asm volatile("" : "+r"(h.sphK), "+r"(h.pairs.sphP));
+        return h;
+    }
+    else if constexpr (KFORM == 4)
+    {
+        FastHitterKC h; h.sphK = sc.sphShared; h.pairs.pp = pp; h.simdCount = sc.simdCount;
+        asm volatile("" : "+r"(h.sphK));
         return h;
     }
     else
@@ -922,7 +960,7 @@ __device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char
 // Light-sampling mode of path_step, fixed at compile time per kernel instance:
 //   kLsOn       explicit light sampling (DO_LIGHT_SAMPLING 1); the scene flag is not looked at
 //   kLsOff      DO_LIGHT_SAMPLING 0: a Lambert vertex bounces at once and adds its emission; no shadow rays, so the
-//               light-sampling block and the QPath fields it keeps (nextDir, thrAlb, nl, pend, albedo) are dead code
+//               light-sampling block and the QPath fields it keeps (nextDir, thrAlb, nl, pend) are dead code
 //   kLsRuntime  either, from the scene flag (warp-uniform): the kernels that have no kLsOff twin
 enum { kLsOn = 0, kLsOff = 1, kLsRuntime = 2 };
 
@@ -970,7 +1008,6 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     V3 target = normal + RandomUnitVector<false>(st.rng);
                     st.nextDir = M<false>::normalize(target);
                     st.thrAlb = st.thr * mat.albedo;
-                    st.albedo = mat.albedo;
                     st.nl = dot(normal, st.d) < 0.0f ? normal : neg(normal);
                     st.mid = mid;
                     st.o = pos;
@@ -1010,7 +1047,8 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         else
         {
             const int j = st.kind - 1;
-            if (id == sc.lights[j].id) st.col = st.col + st.pend;
+            const LightRec& Lj = sc.lights[j];
+            if (id == Lj.id) st.col = st.col + (st.thrAlb * v3(Lj.ex, Lj.ey, Lj.ez)) * st.pend;
             wantLight = true; lightFrom = j + 1;
         }
     }
@@ -1044,7 +1082,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
             float dl = dot(l, st.nl);
             float m = (0.0f < dl) ? dl : 0.0f;
-            st.pend = st.thr * ((st.albedo * v3(Lr.ex, Lr.ey, Lr.ez)) * (m * omega * (1.0f / TPT_PI)));
+            st.pend = m * omega * (1.0f / TPT_PI);
             st.d = l;
             st.kind = 1 + j;
         }
@@ -1085,7 +1123,7 @@ template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = f
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-                uint32_t raysOffset)
+                uint32_t raysOffset, const ParamPairs& pp)
 {
     // a pixel list with an index outside the image traces nothing (the call reports the index)
     if constexpr (SRC == kSrcPixels)
@@ -1106,7 +1144,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     // the 128-thread instances are only launched for scenes whose whole blob is staged (launch_fast): their view points into
     // shared memory for every section, so materials, lights and 1/r load with LDS instead of generic LD
     SceneView sc = make_view<THREADS == 128>(smem, blob, L, stagedBytes, count, nLights);
-    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes, &pp);
     const int lane = threadIdx.x & 31;
     const uint32_t regionPix = SRC != kSrcCamera ? p.numRays : (uint32_t)((long long)p.numRows * p.width);
     const float invSpp = 1.0f / (float)p.spp;
@@ -1206,9 +1244,9 @@ template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
              uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-             uint32_t raysOffset)
+             uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOn>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // DO_LIGHT_SAMPLING 0 (scene flag kSceneNoLightSampling): the same kernel without the light-sampling half of the state
@@ -1217,9 +1255,9 @@ template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                      uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-                     uint32_t raysOffset)
+                     uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOff>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_trace_rays: the slab queue on caller rays (RAYS = true), with the same launch shapes as k_fast_queue and the
@@ -1228,18 +1266,18 @@ template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-            uint32_t raysOffset)
+            uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-                    uint32_t raysOffset)
+                    uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_draw_samples: the slab queue on a pixel list (SRC = kSrcPixels), per-entry sums and, with MOMENTS, sums of squares.
@@ -1248,20 +1286,20 @@ template <int THREADS, int MINB, int KFORM, bool MOMENTS>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_samples(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
-               uint32_t raysOffset)
+               uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
     fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
-                                                                 mtilesPerBand, raysOffset);
+                                                                 mtilesPerBand, raysOffset, pp);
 }
 
 template <int THREADS, int MINB, int KFORM, bool MOMENTS>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                        uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone,
-                       uint32_t mtilesPerBand, uint32_t raysOffset)
+                       uint32_t mtilesPerBand, uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
     fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
-                                                                  mtilesPerBand, raysOffset);
+                                                                  mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_draw_samples' index check: the smallest (entry << 32 | index) of the entries whose index lies outside [0, numPix)
@@ -1832,20 +1870,23 @@ namespace tpt {
 // sc.kformOk, the scene passes the expanded form's accuracy gate (tpt_set_scene; never with fast_kform 0).
 // The families differ on purpose:
 //   slab queue (variants 3/4/9, and tpt_draw's automatic variant): the pair array where the blob, the pairs and 24
-//     camera-ray buffers fit in 200 KB, else form 1. A scene that fails the gate runs the conservative form 3 when
-//     fast_kform is 2 and the pairs fit, else form 0.
+//     camera-ray buffers fit in 200 KB, else form 1; pick_queue turns form 2 into form 4 (pair array in the kernel
+//     parameter) for scenes of at most 64 padded spheres when fast_kform is 2. A scene that fails the gate runs the
+//     conservative form 3 when fast_kform is 2 or 3 and the pairs fit, else form 0.
 //   group and tile queue (variants 8 and 5): the pair array up to 1024 spheres, else form 1. No form 3: a scene that
 //     fails the gate runs form 0.
 //   reference-GPU native instance: form 2 under the group rule but only when fast_kform is 2, else its own
 //     reference-form setup (RgSetupPlain); never form 1 or 3.
 static uint32_t simd_count(const SceneDev& sc) { return (uint32_t)((sc.count + 3) / 4 * 4); }
+// bytes of the pair array a sweep form keeps in shared memory (forms 2 and 3; form 4 has it in the kernel parameter)
+static uint32_t smem_pair_bytes(const SceneDev& sc, int kform) { return kform == 2 || kform == 3 ? simd_count(sc) * 16 : 0; }
 
 int fast_queue_kform(const SceneDev& sc)
 {
     const bool pairsFit = fast_smem(sc.stagedBytes, simd_count(sc) * 16, 24 * 2048).bytes <= 200 * 1024;
     if (sc.kformMode == 0) return 0;
     if (sc.kformOk) return (sc.kformMode == 1 || !pairsFit) ? 1 : 2;
-    return (sc.kformMode == 2 && pairsFit) ? 3 : 0;
+    return (sc.kformMode >= 2 && pairsFit) ? 3 : 0;
 }
 static int fast_group_kform(const SceneDev& sc)
 {
@@ -1853,7 +1894,7 @@ static int fast_group_kform(const SceneDev& sc)
 }
 static int refgpu_fast_kform(const SceneDev& sc)
 {
-    return sc.kformOk && sc.kformMode == 2 && simd_count(sc) <= 1024 ? 2 : 0;
+    return sc.kformOk && sc.kformMode >= 2 && simd_count(sc) <= 1024 ? 2 : 0;
 }
 
 // Runtime sweep form -> kernel instance: f(std::integral_constant<int, kform>) for kform in [1, KMAX], f(<0>) otherwise.
@@ -1917,7 +1958,8 @@ struct QueuePick
 // The slab-queue instance for `samples` samples of each of `regionPix` pixels, rays or list entries (variants 3/4/9;
 // tpt_trace_rays and tpt_draw_samples take variant 3's choice). Small scenes: 128-thread CTAs, 6 (variant 4: 7, at 72 registers) per SM; scenes whose arrays
 // fill most of an SM's shared memory: ONE 768-thread CTA per SM (24 warps share one copy of the geometry instead of 2 CTAs
-// x 4 warps with a copy each). Long launches (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80;
+// x 4 warps with a copy each). Long launches (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80
+// (the same rule for form 4: at 720p x 4 spp its 8-CTA instance is 3 % slower than the 6-CTA one);
 // short ones keep 6, where a warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant
 // 9 forces the 8-CTA instance (A/B runs).
 template <int SRC, bool MOMENTS = false>
@@ -1925,11 +1967,22 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
 {
     QueuePick q;
     q.kform = fast_queue_kform(sc);
-    const bool big = fast_smem(sc.stagedBytes, q.kform >= 2 ? simd_count(sc) * 16 : 0, 4 * 2048).bytes > 36 * 1024 ||
+    // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
+    // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2)
+    if (q.kform == 2 && sc.kformMode == 2 && simd_count(sc) <= (uint32_t)kParamPairSpheres && SRC != kSrcPixels &&
+        !(SRC == kSrcCamera && variant == 4))
+        q.kform = 4;
+    const bool big = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, q.kform), 4 * 2048).bytes > 36 * 1024 ||
                      sc.stagedBytes != sc.layout.totalBytes;
     const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
     q.threads = big ? TPT_BIG_THREADS : 128;
     if (big) q.kern = queue_kernel<SRC, MOMENTS, TPT_BIG_THREADS, 1>(sc, q.kform);
+    else if (q.kform == 4)
+    {
+        if constexpr (SRC != kSrcPixels)
+            q.kern = variant == 9 || (variant == 3 && slabsPerWarp >= 48) ? queue_instance<SRC, MOMENTS, 128, 8, 4>(sc)
+                                                                          : queue_instance<SRC, MOMENTS, 128, 6, 4>(sc);
+    }
     else if (q.kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) q.kern = queue_instance<SRC, MOMENTS, 128, 8, 2>(sc);
     else if (SRC == kSrcCamera && variant == 4) q.kern = queue_kernel<kSrcCamera, false, 128, 7>(sc, q.kform);
     else q.kern = queue_kernel<SRC, MOMENTS, 128, TPT_QUEUE_MINB>(sc, q.kform);
@@ -1945,7 +1998,7 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
 {
     const QueueKernel kern = q.kern;
     const int threads = q.threads;
-    const FastSmem lay = fast_smem(sc.stagedBytes, q.kform >= 2 ? simd_count(sc) * 16 : 0, (uint32_t)(threads / 32) * kSlabPix * 32, true);
+    const FastSmem lay = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, q.kform), (uint32_t)(threads / 32) * kSlabPix * 32, true);
     const uint32_t S = (uint32_t)(p.spp * p.numFrames);
     const long long slabs = ((regionPix + kSlabPix - 1) / kSlabPix) * S;
     if (slabs > 0x7fffffffLL) return cudaErrorInvalidValue;
@@ -1982,7 +2035,8 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
     }
 #endif
     kern<<<(unsigned)grid, threads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                          (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers);
+                                                          (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers,
+                                                          sc.pairs);
 #if TPT_TRACE_WARPS
     if (const char* tf = getenv("TPT_TRACE_FILE"))
     {
@@ -2000,13 +2054,14 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
 template <int KFORM>
 __global__ void __launch_bounds__(256)
 k_debug_hit(const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes,
-            const float* __restrict__ rays, int* __restrict__ outId, float* __restrict__ outT, long long n)
+            const float* __restrict__ rays, int* __restrict__ outId, float* __restrict__ outT, long long n,
+            const __grid_constant__ ParamPairs pp)
 {
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     stage_blob(smem, blob, stagedBytes, &bar);
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes);
+    const auto hitter = prepare_sweep<KFORM>(sc, smem, L, stagedBytes, &pp);
     for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
     {
         const V3 o{rays[6 * i], rays[6 * i + 1], rays[6 * i + 2]}, d{rays[6 * i + 3], rays[6 * i + 4], rays[6 * i + 5]};
@@ -2018,13 +2073,13 @@ k_debug_hit(const unsigned char* __restrict__ blob, SceneBlobLayout L, int count
 
 cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, int* dId, float* dT, long long n, int numSMs, cudaStream_t stream)
 {
-    auto kern = for_kform<3>(kform, [](auto K) { return k_debug_hit<decltype(K)::value>; });
+    auto kern = for_kform<4>(kform, [](auto K) { return k_debug_hit<decltype(K)::value>; });
     // the blob padded to 128 B even without a pair array: the end of the (possibly empty) pair array
-    const size_t dyn = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0).buffers;
+    const size_t dyn = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, kform)).buffers;
     if (dyn > 200 * 1024) return cudaErrorInvalidValue;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
     if (e != cudaSuccess) return e;
-    kern<<<numSMs, 256, dyn, stream>>>(sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, dRays, dId, dT, n);
+    kern<<<numSMs, 256, dyn, stream>>>(sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, dRays, dId, dT, n, sc.pairs);
     return cudaGetLastError();
 }
 
@@ -2178,7 +2233,7 @@ cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays,
     auto kern = rays ? for_kform<3>(kform, [](auto K) { return k_fast_aov<true, decltype(K)::value>; })
                      : for_kform<3>(kform, [](auto K) { return k_fast_aov<false, decltype(K)::value>; });
     // [staged blob | pair array (forms 2/3)], nothing behind it
-    const size_t dyn = fast_smem(sc.stagedBytes, kform >= 2 ? simd_count(sc) * 16 : 0).buffers;
+    const size_t dyn = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, kform)).buffers;
     const long long n = rays ? (long long)p.numRays : (long long)p.numRows * p.width;
     const long long chunks = (n + 31) / 32;
     long long grid = 0;

@@ -11,9 +11,12 @@ struct SceneDev
     SceneBlobLayout layout;
     int count, nLights;
     uint32_t stagedBytes;        // prefix of the blob every CTA stages into shared memory via TMA
-    int kformMode;               // fast kernels: 2 = expanded form on the pair array where it fits, 1 = expanded form, scalar
+    int kformMode;               // fast kernels: 2 = expanded form on the pair array where it fits (kernel parameter up to
+                                 // kParamPairSpheres, else shared memory), 3 = the same always in shared memory (A/B),
+                                 // 1 = expanded form, scalar
     bool kformOk;                // every sphere satisfies |c|^2 <= 128 + 2 r^2: the expanded-form sweep of the fast kernels
                                  // then rounds no worse than the reference form (see FastHitterK)
+    ParamPairs pairs;            // pass-1 operands of sweep form 4 (all zero for scenes of more than kParamPairSpheres)
 };
 
 // lanes: 0 = choose from the number of (frame,row) chains; 1, 2, 8, 9, 32 or 64..71 to force (see tpt_exact.cu).

@@ -84,6 +84,25 @@ inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int
     }
 }
 
+// ParamPairs of a packed scene of at most kParamPairSpheres padded spheres, bit-identical to the pair array the kernels
+// build in shared memory (build_sphK, build_sph_pairs): K = |s|^2 - r^2 in double (the float products are exact in
+// double, so contraction cannot change it) rounded to float, padded spheres K = 1e30; unused entries zero.
+inline void build_param_pairs(const std::vector<unsigned char>& blob, const SceneBlobLayout& L, int count, ParamPairs& pp)
+{
+    memset(&pp, 0, sizeof(pp));
+    const int simdCount = (count + 3) / 4 * 4;
+    if (simdCount > kParamPairSpheres) return;
+    const Q4* sph = (const Q4*)(blob.data() + L.offSph);
+    for (int i = 0; i < simdCount; ++i)
+    {
+        const Q4 s = sph[i];
+        const double K = (double)s.x * s.x + (double)s.y * s.y + (double)s.z * s.z - (double)s.w;
+        float* f = pp.f + (i >> 1) * 8 + (i & 1);
+        f[0] = s.x; f[2] = s.y; f[4] = s.z;
+        f[6] = -(i < count ? (float)K : 1.0e30f);
+    }
+}
+
 inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlobLayout& L, int count, int nLights)
 {
     SceneView v;

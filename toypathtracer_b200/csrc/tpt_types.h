@@ -72,6 +72,13 @@ enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u };
 // keeps the light table either way, so toggling the switch uploads the same bytes.
 inline int sampled_lights(uint32_t sceneFlags, int nLights) { return (sceneFlags & kSceneNoLightSampling) ? 0 : nLights; }
 
+// The fast slab queue's pass-1 operands for scenes of at most kParamPairSpheres padded spheres (sweep form 4): the pair
+// array of the expanded form, pair p = spheres 2p, 2p+1 as f[8p ..] = {x0, x1, y0, y1, z0, z1, -K0, -K1}, built on the
+// host (build_param_pairs) and passed by value in a __grid_constant__ kernel parameter, so that pass 1 reads the sphere
+// values from the constant bank into uniform registers instead of from shared memory into vector registers.
+constexpr int kParamPairSpheres = 64;
+struct ParamPairs { float f[kParamPairSpheres * 4]; };
+
 struct DrawParams
 {
     Camera88 cam;
