@@ -263,6 +263,17 @@ int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long l
  * 3 conservative packed pass + reference-form decisions, 4 expanded on packed pairs read from the kernel parameters: scenes
  * of at most 64 padded spheres only), tMin/tMax as Trace uses them. outId -1 = miss. */
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays6, int* outId, float* outT, long long n);
+/* Diagnostic: the mangled names of the trace kernels (path tracing and first-hit AOV kernels, not the helpers that clear,
+ * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_draw_samples, tpt_draw_aovs or
+ * tpt_trace_aovs launched, in launch order, separated by '\n' and NUL-terminated in buf[cap].
+ *   - The record is per host thread, not per context: a call on another thread, or on another context from this
+ *     thread, replaces it.
+ *   - A call resets it when it starts launching (an empty call too). A call refused before that leaves the previous
+ *     record; a call that fails after it holds the launches made before the failure.
+ *   - Only the first 16 launches are named. The return value counts all of them, so a result above 16 means the list
+ *     was cut off (long multi-launch draws, e.g. exact mode split over many frame batches).
+ * Returns that count, or minus an error code (buffer too small, CUDA error). */
+int tpt_debug_last_kernels(tpt_context* ctx, char* buf, int cap);
 /* Diagnostic: device timestamps (ms since the start of the last progress-mode host draw) of the trace kernel's end,
  * each band copy's end and the draw's end. Returns minus the number of entries written. */
 int tpt_debug_timeline(tpt_context* ctx, float* outMs, int capacity);

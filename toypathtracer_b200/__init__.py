@@ -75,6 +75,7 @@ def _load_lib():
     L.tpt_tonemap_rgba8.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci, ci, ci, vp]; L.tpt_tonemap_rgba8.restype = ci
     L.tpt_debug_libm.argtypes = [vp, ci, vp, vp, cll]; L.tpt_debug_libm.restype = ci
     L.tpt_debug_hit.argtypes = [vp, ci, vp, vp, vp, cll]; L.tpt_debug_hit.restype = ci
+    L.tpt_debug_last_kernels.argtypes = [vp, ctypes.c_char_p, ci]; L.tpt_debug_last_kernels.restype = ci
     L.tpt_trace_rays.argtypes = [vp, vp, ci, cll, ci, ci, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_rays.restype = ci
     L.tpt_draw_aovs.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, ci, cu, ctypes.POINTER(cll), vp]
     L.tpt_draw_aovs.restype = ci
@@ -191,6 +192,68 @@ def _torch_stream(dev) -> int:
     stream, so torch's legacy default stream is passed as cudaStreamLegacy)."""
     import torch
     return torch.cuda.current_stream(dev).cuda_stream or _CUDA_STREAM_LEGACY
+
+
+def kernel_signature(mangled: str) -> str:
+    """A kernel's mangled name as its template instance, the namespace and parameter list dropped:
+    '_ZN3tpt12k_fast_queueILi128ELi6ELi4EEEv...' -> 'k_fast_queue<128, 6, 4>', '_ZN3tpt8k_refgpuILb0ENS_9RgSetupK2EEEv...'
+    -> 'k_refgpu<false, RgSetupK2>'. Decodes the part of the Itanium C++ ABI mangling the library's kernels use (nested
+    names, substitutions, integer and bool literals, class template arguments), so no demangler is needed."""
+    s = mangled
+    if not s.startswith("_Z"):
+        return s
+    pos = 2
+
+    def source():                       # <length><identifier>
+        nonlocal pos
+        i = pos
+        while s[pos].isdigit():
+            pos += 1
+        n = int(s[i:pos])
+        pos += n
+        return s[pos - n:pos]
+
+    def targs():                        # I <arg>+ E
+        nonlocal pos
+        pos += 1
+        out = []
+        while s[pos] != "E":
+            if s[pos] == "L":           # L <type> <value> E
+                t = s[pos + 1]
+                j = s.index("E", pos)
+                v = s[pos + 2:j]
+                pos = j + 1
+                out.append(("true" if v == "1" else "false") if t == "b" else ("-" + v[1:] if v.startswith("n") else v))
+            else:
+                out.append(name())
+        pos += 1
+        return "<" + ", ".join(out) + ">"
+
+    def name():
+        nonlocal pos
+        nested = s[pos] == "N"
+        if nested:
+            pos += 1
+        out = ""
+        while True:
+            c = s[pos]
+            if c == "I":
+                out += targs()
+            elif c == "S":              # a substitution (here: the namespace seen before)
+                pos = s.index("_", pos) + 1
+            elif c.isdigit():
+                part = source()
+                if part != "tpt":
+                    out += ("::" if out else "") + part
+            else:
+                break
+            if not nested and s[pos] != "I":
+                break
+        if nested:
+            pos += 1                    # E
+        return out
+
+    return name()
 
 
 LUMA = (0.2126, 0.7152, 0.0722)    # Rec. 709 luminance weights of the adaptive stopping rule
@@ -491,6 +554,17 @@ class Context:
         t = np.empty(len(rays), np.float32)
         self._check(self._L.tpt_debug_hit(self._h, kform, rays.ctypes.data, ids.ctypes.data, t.ctypes.data, len(rays)), "tpt_debug_hit")
         return ids, t
+
+    def last_kernels(self):
+        """Trace kernels the calling thread's most recent draw / trace_rays / draw_samples / AOV call launched, as
+        readable template instances (kernel_signature), in launch order. The library names the first 16 launches; past
+        that the list ends with "... N more launches" (see tpt_debug_last_kernels)."""
+        buf = ctypes.create_string_buffer(4096)
+        n = self._L.tpt_debug_last_kernels(self._h, buf, len(buf))
+        if n < 0:
+            self._check(-n, "tpt_debug_last_kernels")
+        names = [kernel_signature(s) for s in buf.value.decode().split("\n")] if n else []
+        return names + ([f"... {n - len(names)} more launches"] if n > len(names) else [])
 
     def tonemap_srgb8(self, image, width: int, height: int) -> np.ndarray:
         addr, on_dev, _keep = _as_ptr(image)

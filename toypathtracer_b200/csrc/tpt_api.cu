@@ -14,6 +14,8 @@
 
 using namespace tpt;
 
+thread_local KernelRecord tpt::t_lastKernels = {};
+
 // Device staging allocations of host buffers (tpt_context::staging). kStageImage holds tpt_draw's image, the input of
 // tpt_tonemap_rgba8, tpt_trace_rays' out4 and tpt_draw_samples' sum4; the others hold the buffers they are named after.
 enum Staging { kStageImage, kStageRays, kStageAlbedo, kStageNormal, kStageIds, kStagePixels, kStageSq4, kNumStaging };
@@ -444,6 +446,7 @@ static int start_kernels(tpt_context* ctx, cudaStream_t stream, int n)
     }
     CK(cudaMemsetAsync(ctx->dRayCounters, 0, (size_t)n * sizeof(unsigned long long), stream), "zero counters");
     ctx->lastLaunches = 0;
+    clear_kernels();
     CK(cudaEventRecord(ctx->evStart, stream), "event record");
     return 0;
 }
@@ -496,6 +499,7 @@ static int empty_call(tpt_context* ctx, long long* outRayCount, long long* outPe
     if (outRayCount) *outRayCount = 0;
     if (outPerFrame) for (int i = 0; i < numFrames; ++i) outPerFrame[i] = 0;
     ctx->lastLaunches = 0;
+    clear_kernels();
     return 0;
 }
 
@@ -1196,6 +1200,27 @@ int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays, int* outId, fl
     cudaFree(dRays); cudaFree(dT); cudaFree(dId);
     if (e != cudaSuccess) return fail(ctx, e, "tpt_debug_hit");
     return 0;
+}
+
+int tpt_debug_last_kernels(tpt_context* ctx, char* buf, int cap)
+{
+    if (!ctx || !buf || cap < 1) return -(int)cudaErrorInvalidValue;
+    if (cudaError_t e = cudaSetDevice(ctx->device)) return -fail(ctx, e, "cudaSetDevice");
+    int len = 0;
+    buf[0] = '\0';
+    const int kept = t_lastKernels.n < KernelRecord::kCap ? t_lastKernels.n : KernelRecord::kCap;
+    for (int i = 0; i < kept; ++i)
+    {
+        const char* name = nullptr;
+        cudaError_t e = cudaFuncGetName(&name, t_lastKernels.fn[i]);
+        if (e != cudaSuccess) return -fail(ctx, e, "tpt_debug_last_kernels");
+        const int need = (int)strlen(name) + (i ? 1 : 0);
+        if (len + need + 1 > cap) return -fail_msg(ctx, "tpt_debug_last_kernels: buffer too small");
+        if (i) buf[len++] = '\n';
+        memcpy(buf + len, name, strlen(name) + 1);
+        len += (int)strlen(name);
+    }
+    return t_lastKernels.n;
 }
 
 } // extern "C"

@@ -2034,6 +2034,7 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
         cudaMemsetAsync(dTrace, 0, traceWords * 8, stream);
     }
 #endif
+    note_kernel((const void*)kern);
     kern<<<(unsigned)grid, threads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
                                                           (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers,
                                                           sc.pairs);
@@ -2239,6 +2240,7 @@ cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays,
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, kAovThreads, dyn, numSMs, (chunks + kAovThreads / 32 - 1) / (kAovThreads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
+    note_kernel((const void*)kern);
     kern<<<(unsigned)grid, kAovThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, (uint32_t)chunks,
                                                        rays ? 0.0f : prev_weight(p.frame0, p.numFrames, p.flags), albedo4, normal4, ids);
     return cudaGetLastError();
@@ -2262,6 +2264,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         e = cudaFuncSetAttribute(k_fast_mega, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
         if (e != cudaSuccess) return e;
         const int tilesX = (p.width + 15) / 16, tilesY = (p.numRows + 15) / 16;
+        note_kernel((const void*)k_fast_mega);
         k_fast_mega<<<tilesX * tilesY, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
         return cudaGetLastError();
     }
@@ -2271,6 +2274,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         const int numTiles = (int)((regionPix + kTilePix - 1) / kTilePix);
         e = persistent_grid(kern, kFastThreads, sc.stagedBytes, numSMs, numTiles, p, stream, grid);
         if (e != cudaSuccess) return e;
+        note_kernel((const void*)kern);
         kern<<<(unsigned)grid, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, numTiles);
         return cudaGetLastError();
     }
@@ -2293,6 +2297,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         if (groups > 0x7fffffffLL) return cudaErrorInvalidValue;
         e = persistent_grid(kern, kQueueThreads, dyn, numSMs, (groups + kQueueThreads / 32 - 1) / (kQueueThreads / 32), p, stream, grid);
         if (e != cudaSuccess) return e;
+        note_kernel((const void*)kern);
         kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
                                                                (uint32_t)groups, S, prev_weight(p.frame0, p.numFrames, p.flags));
         return cudaGetLastError();
@@ -2313,6 +2318,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         wa.S = S;
         wa.totalPaths = (uint32_t)total;
         wa.divS = make_fastdiv(wa.S); wa.divW = make_fastdiv((uint32_t)p.width); wa.divSpp = make_fastdiv((uint32_t)p.spp);
+        note_kernel((const void*)kern);
         kern<<<(unsigned)grid, kWaveThreads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, lay.buffers, wa);
         return cudaGetLastError();
     }
@@ -2332,6 +2338,7 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         while (tileQPix > (uint32_t)kSlabPix && (regionPix + tileQPix - 1) / tileQPix < 8 * grid && tileQPix * S > 2048) tileQPix -= kSlabPix;
         const long long tiles = (regionPix + tileQPix - 1) / tileQPix;
         if (grid > tiles) grid = tiles;
+        note_kernel((const void*)kern);
         kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
                                                                (uint32_t)tiles, S, prev_weight(p.frame0, p.numFrames, p.flags), tileQPix);
         return cudaGetLastError();

@@ -62,6 +62,23 @@ bool fast_variant_writes_final_pixels(int variant);   // the trace kernel stores
 // weight of `prev` when frames [frame0, frame0 + numFrames) are blended into it: the product of their lerp_fac
 float prev_weight(int frame0, int numFrames, unsigned flags);
 
+// Diagnostic (tpt_debug_last_kernels): the trace kernels the calling thread's current library call launched, as the
+// function pointers its launch sites passed to note_kernel. start_kernels clears the record; a launch only stores a pointer.
+// n counts every launch; the first kCap are kept (tpt_debug_last_kernels reports the count, so a cut-off list shows).
+struct KernelRecord
+{
+    static constexpr int kCap = 16;
+    const void* fn[kCap];
+    int n;
+};
+extern thread_local KernelRecord t_lastKernels;
+inline void clear_kernels() { t_lastKernels.n = 0; }
+inline void note_kernel(const void* fn)
+{
+    if (t_lastKernels.n < KernelRecord::kCap) t_lastKernels.fn[t_lastKernels.n] = fn;
+    ++t_lastKernels.n;
+}
+
 // Launch set-up of a persistent kernel: allows `dyn` bytes of dynamic shared memory, sizes the grid to the CTAs that stay
 // resident on numSMs SMs (at least one per SM) but no more than `ctasNeeded`, and zeroes the work counter.
 template <class Kernel>
