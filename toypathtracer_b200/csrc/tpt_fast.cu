@@ -3,14 +3,20 @@
 // contraction and fast intrinsics allowed. Results agree with the reference statistically (same expectation,
 // same rays/sample), not bitwise — bitwise parity is the exact mode's job (tpt_exact.cu).
 //
-// variant 0  "megakernel": one thread per pixel, loops over frames x spp (what the reference's own GPU shaders
-//            do, Cpp/Windows/ComputeShader.hlsl:353-395). Baseline for the persistent design.
-// variant 1  "persistent wavefront": one CTA per SM slot, resident for the whole draw. The CTA pulls tiles of
-//            TILE_PIX pixels from a global counter; inside a tile every lane runs a path state machine and
-//            refills itself with the next (pixel, sample) from a warp-aggregated shared counter as soon as its
-//            path ends (ray regeneration), so the ray-vs-all-spheres sweep — 85 % of the instructions — always
-//            runs with full warps. Radiance is accumulated per pixel in shared memory; finished tiles are
-//            written with coalesced 128-bit stores (and 128-bit loads of `prev` when accumulating).
+// The estimator is written once, as path_step (one step of a per-lane path state machine on a QPath): every variant and
+// entry point shades with it, and the block wavefront (variants 6/7) calls its pieces phase by phase. The variants differ
+// in how they deal work and write pixels:
+// variant 0  "megakernel": one thread per pixel, loops over frames x spp with one stream per pixel and frame (what
+//            the reference's own GPU shaders do, Cpp/Windows/ComputeShader.hlsl:353-395). Baseline for the
+//            persistent design.
+// variant 1  "persistent wavefront" (variant 2: the same kernel at 3 instead of 2 CTAs per SM): one CTA per SM
+//            slot, resident for the whole draw. The CTA pulls tiles of
+//            kTilePix pixels from a global counter; inside a tile every lane runs a path and refills itself with the
+//            next (pixel, sample) from a warp-aggregated shared counter as soon as its path ends (ray regeneration),
+//            so the ray-vs-all-spheres sweep — 85 % of the instructions — always runs with full warps. Radiance is
+//            accumulated per pixel in shared memory; finished tiles are written with coalesced 128-bit stores (and
+//            128-bit loads of `prev` when accumulating).
+// variants 3-9: see their sections below.
 #include <climits>
 #include <cstdio>
 #include <cstdlib>
@@ -146,247 +152,6 @@ __device__ __forceinline__ void write_tile(const DrawParams& p, float* acc, I pi
         acc[i * 3 + 0] = 0.0f; acc[i * 3 + 1] = 0.0f; acc[i * 3 + 2] = 0.0f;
     }
 }
-
-// ---- variant 0 ------------------------------------------------------------------------------------------------
-__global__ void __launch_bounds__(kFastThreads)
-k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes)
-{
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t bar;
-    __shared__ float sW[kMaxFramesPerDraw];
-    __shared__ float sWPrev;
-    stage_blob(smem, blob, stagedBytes, &bar);
-    if (threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); sWPrev = wp; }
-    __syncthreads();
-    SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-
-    // 16x16 pixel block, each warp an 8x4 patch
-    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-    const int tilesX = (p.width + 15) / 16;
-    const int tx = blockIdx.x % tilesX, ty = blockIdx.x / tilesX;
-    const int x = tx * 16 + (warp & 1) * 8 + (lane & 7);
-    const int ri = ty * 16 + (warp >> 1) * 4 + (lane >> 3);
-    unsigned rc = 0;
-    if (x < p.width && ri < p.numRows)
-    {
-        const int y = region_pixel(p, ri, x).y;
-        SerialHitter<false> hitter;
-        V3 acc = v3(0, 0, 0);
-        const float invSpp = 1.0f / (float)p.spp;
-        for (int fi = 0; fi < p.numFrames; ++fi)
-        {
-            uint32_t state = pixel_seed((uint32_t)(y * p.width + x), (uint32_t)(p.frame0 + fi));
-            V3 col = v3(0, 0, 0);
-            for (int s = 0; s < p.spp; ++s)
-            {
-                Ray r = fast_camera_ray(p, x, y, state);
-                col = col + trace_fast(sc, r, state, rc, hitter);
-            }
-            acc = acc + col * (invSpp * sW[fi]);
-        }
-        float* px = p.image + region_pixel(p, ri, x).off * 4;
-        st_stream_f4(px, blend_prev(p, px, sWPrev, acc.x, acc.y, acc.z));
-    }
-    flush_ray_count(p.rayCounter, rc, lane);
-}
-
-// ---- variant 1 ------------------------------------------------------------------------------------------------
-struct PathState
-{
-    V3 o, d;          // ray to intersect next
-    V3 thr, col;      // throughput before the current vertex, radiance so far
-    V3 nextDir;       // Lambert bounce direction, pending while shadow rays are in flight
-    V3 thrAlb;        // thr * albedo at the pending Lambert vertex
-    V3 nl;            // shading normal facing the incoming ray (Test.cpp:129)
-    V3 pend;          // radiance the in-flight shadow ray carries if it reaches its light
-    V3 albedo;
-    uint32_t rng;
-    int pix;          // pixel index inside the tile
-    float weight;
-    int kind;         // 0: path ray, 1+j: shadow ray towards light j
-    int depth;
-    int mid;          // sphere id of the pending Lambert vertex (skip-self test, Test.cpp:100)
-    bool doMaterialE;
-    bool active;
-};
-
-template <int MINB>
-__global__ void __launch_bounds__(kFastThreads, MINB)
-k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
-                  uint32_t stagedBytes, int numTiles)
-{
-    extern __shared__ __align__(128) unsigned char smem[];
-    __shared__ uint64_t bar;
-    __shared__ float sW[kMaxFramesPerDraw];
-    __shared__ float sWPrev;
-    __shared__ float sAcc[kTilePix * 3];
-    __shared__ int sTile;
-    __shared__ int sTask;
-    stage_blob(smem, blob, stagedBytes, &bar);
-    if (threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); sWPrev = wp; }
-    for (int i = threadIdx.x; i < kTilePix * 3; i += kFastThreads) sAcc[i] = 0.0f;
-    SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    const int lane = threadIdx.x & 31;
-    const long long regionPix = (long long)p.numRows * p.width;
-    const int S = p.spp * p.numFrames;          // samples per pixel in this draw
-    const float invSpp = 1.0f / (float)p.spp;
-    SerialHitter<false> hitter;
-    unsigned rc = 0;
-
-    for (;;)
-    {
-        __syncthreads(); // sAcc zeroed / previous tile written
-        if (threadIdx.x == 0) { sTile = (int)atomicAdd(p.workCounter, 1u); sTask = 0; }
-        __syncthreads();
-        const int tile = sTile;
-        if (tile >= numTiles) break;
-        const long long pix0 = (long long)tile * kTilePix;
-        const int tilePix = (int)(regionPix - pix0 < kTilePix ? regionPix - pix0 : kTilePix);
-        const int tileTasks = tilePix * S;
-
-        PathState st;
-        st.active = false;
-        for (;;)
-        {
-            // ---- regeneration: lanes without a path take the next (pixel, sample) of the tile
-            unsigned need = __ballot_sync(0xffffffffu, !st.active);
-            if (need)
-            {
-                int base = 0;
-                const int leader = __ffs(need) - 1;
-                if (lane == leader) base = atomicAdd(&sTask, __popc(need));
-                base = __shfl_sync(0xffffffffu, base, leader);
-                if (!st.active)
-                {
-                    const int task = base + __popc(need & ((1u << lane) - 1u));
-                    if (task < tileTasks)
-                    {
-                        // samples of one pixel sit in adjacent lanes: coherent primary rays
-                        const int pixIn = task / S, sIdx = task % S;
-                        const int fi = sIdx / p.spp;
-                        const RegionPixel q = region_pixel(p, pix0 + pixIn);
-                        st.rng = pixel_seed((uint32_t)(q.y * p.width + q.x) * (uint32_t)p.spp + (uint32_t)(sIdx % p.spp),
-                                            (uint32_t)(p.frame0 + fi));
-                        Ray r = fast_camera_ray(p, q.x, q.y, st.rng);
-                        st.o = r.orig; st.d = r.dir;
-                        st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
-                        st.pix = pixIn; st.weight = invSpp * sW[fi];
-                        st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
-                    }
-                }
-            }
-            if (!__any_sync(0xffffffffu, st.active)) break;
-
-            // ---- intersect: every active lane sweeps all spheres (shared-memory broadcast reads)
-            float t = TPT_MAX_T;
-            int id = -1;
-            if (st.active) { id = hitter.hit(sc, st.o, st.d, TPT_MIN_T, TPT_MAX_T, t); ++rc; }
-
-            // ---- shade
-            bool wantLight = false;   // lane must pick its next shadow ray (or resume the path)
-            int lightFrom = 0;
-            bool finished = false;
-            if (st.active)
-            {
-                if (st.kind == 0)
-                {
-                    if (id < 0) { st.col = st.col + st.thr * sky(st.d, sc); finished = true; }
-                    else
-                    {
-                        Q4 s = ld_sph(sc, id);
-                        V3 pos = st.o + st.d * t;
-                        V3 normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];
-                        const int mid = id < sc.count ? id : sc.count;
-                        Mat mat = load_mat(sc, mid);
-                        if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
-                        else if (mat.type == kLambert)
-                        {
-                            if (st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
-                            V3 target = normal + RandomUnitVector<false>(st.rng);
-                            st.nextDir = M<false>::normalize(target);
-                            st.thrAlb = st.thr * mat.albedo;
-                            st.albedo = mat.albedo;
-                            st.nl = dot(normal, st.d) < 0.0f ? normal : neg(normal);
-                            st.mid = mid;
-                            st.o = pos;
-                            wantLight = true; lightFrom = 0;
-                        }
-                        else
-                        {
-                            V3 att, outDir;
-                            bool ok = scatter_specular<false>(mat, st.d, pos, normal, st.rng, att, outDir);
-                            if (!ok) { st.col = st.col + st.thr * mat.emissive; finished = true; }
-                            else
-                            {
-                                if (st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
-                                st.doMaterialE = true;
-                                st.thr = st.thr * att;
-                                st.o = pos; st.d = outDir; ++st.depth;
-                            }
-                        }
-                    }
-                }
-                else
-                {
-                    const int j = st.kind - 1;
-                    if (id == sc.lights[j].id) st.col = st.col + st.pend;
-                    wantLight = true; lightFrom = j + 1;
-                }
-            }
-            // Lambert vertices and returning shadow rays converge here: next light sample or resume the path
-            if (wantLight)
-            {
-                int j = lightFrom;
-                while (j < sc.nLights && sc.lights[j].id == st.mid) ++j;
-                if (j < sc.nLights)
-                {
-                    const LightRec Lr = sc.lights[j];
-                    // sample_light (Test.cpp:104-131) with the facing normal already resolved
-                    V3 scn = v3(Lr.cx, Lr.cy, Lr.cz);
-                    V3 sw = M<false>::normalize(scn - st.o);
-                    V3 su = M<false>::normalize(cross(fabsf(sw.x) > 0.01f ? v3(0, 1, 0) : v3(1, 0, 0), sw));
-                    V3 sv = cross(sw, su);
-                    V3 pc = st.o - scn;
-                    float cosAMax = M<false>::sqrt_(1.0f - __fdividef(Lr.radius * Lr.radius, dot(pc, pc)));
-                    float eps1 = RandomFloat01(st.rng), eps2 = RandomFloat01(st.rng);
-                    float cosA = 1.0f - eps1 + eps1 * cosAMax;
-                    float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
-                    float phi = 2.0f * TPT_PI * eps2;
-                    float sp, cp;
-                    __sincosf(phi, &sp, &cp);
-                    V3 l = su * (cp * sinA) + sv * (sp * sinA) + sw * cosA;
-                    float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
-                    float dl = dot(l, st.nl);
-                    float m = (0.0f < dl) ? dl : 0.0f;
-                    st.pend = st.thr * ((st.albedo * v3(Lr.ex, Lr.ey, Lr.ez)) * (m * omega * (1.0f / TPT_PI)));
-                    st.d = l;
-                    st.kind = 1 + j;
-                }
-                else
-                {
-                    st.d = st.nextDir;
-                    st.thr = st.thrAlb;
-                    st.kind = 0;
-                    st.doMaterialE = emission_after_lambert(sc);
-                    ++st.depth;
-                }
-            }
-            if (finished)
-            {
-                atomicAdd(&sAcc[st.pix * 3 + 0], st.col.x * st.weight);
-                atomicAdd(&sAcc[st.pix * 3 + 1], st.col.y * st.weight);
-                atomicAdd(&sAcc[st.pix * 3 + 2], st.col.z * st.weight);
-                st.active = false;
-            }
-        }
-
-        // ---- tile done
-        __syncthreads();
-        write_tile(p, sAcc, pix0, tilePix, sWPrev, kFastThreads);
-    }
-    flush_ray_count(p.rayCounter, rc, lane);
-}
-
 
 // ---- variant 3 ------------------------------------------------------------------------------------------------
 // "persistent queue": no tiles, no block barriers after the prologue. Every WARP pulls slabs of kSlabPix pixels x
@@ -529,14 +294,19 @@ struct QPath
     bool active;
 };
 
+// A new path along camera ray r, its stream continuing from rng. The caller sets pixOff and weight.
+__device__ __forceinline__ void begin_path(QPath& st, const Ray& r, uint32_t rng)
+{
+    st.o = r.orig; st.d = r.dir;
+    st.rng = rng;
+    st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
+    st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
+}
 // A new path from a ray-buffer entry {origin.xyz, rng state} {direction.xyz, tag}. The caller decodes the tag into
 // pixOff and weight.
 __device__ __forceinline__ void begin_path(QPath& st, float4 e0, float4 e1)
 {
-    st.o = v3(e0.x, e0.y, e0.z); st.d = v3(e1.x, e1.y, e1.z);
-    st.rng = __float_as_uint(e0.w);
-    st.thr = v3(1, 1, 1); st.col = v3(0, 0, 0);
-    st.kind = 0; st.depth = 0; st.doMaterialE = true; st.active = true;
+    begin_path(st, Ray{v3(e0.x, e0.y, e0.z), v3(e1.x, e1.y, e1.z)}, __float_as_uint(e0.w));
 }
 
 // Ray regeneration of the warp-dealt kernels (slab, tile and group queues): the idle lanes take entries [cur, end) of
@@ -964,7 +734,55 @@ __device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char
 //   kLsRuntime  either, from the scene flag (warp-uniform): the kernels that have no kLsOff twin
 enum { kLsOn = 0, kLsOff = 1, kLsRuntime = 2 };
 
-// One iteration of the per-lane path state machine shared by the queue kernels: intersect the lane's current ray
+// The first light from index j on that a Lambert vertex on sphere `mid` samples: a light never samples itself (Test.cpp:100).
+__device__ __forceinline__ int next_light(const SceneView& sc, int j, int mid)
+{
+    while (j < sc.nLights && sc.lights[j].id == mid) ++j;
+    return j;
+}
+
+// The shadow ray from o towards light Lr (Test.cpp:104-131, the facing normal nl already resolved): a direction l drawn
+// uniformly in the cone the light subtends, and the returned weight m * omega / pi. The ray adds thrAlb * E_light * weight
+// when it reaches its light.
+__device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l)
+{
+    V3 scn = v3(Lr.cx, Lr.cy, Lr.cz);
+    V3 pc = scn - o;
+    float d2 = dot(pc, pc);
+    float inv = __frsqrt_rn(d2);          // d2 is a squared distance between distinct spheres: never denormal
+    V3 sw = pc * inv;
+    // any orthonormal (su, sv) around sw gives the same cone-sample distribution (phi is uniform): use the
+    // branch-free basis of Duff et al. 2017 instead of normalize(cross(up, sw)), cross(sw, su) (Test.cpp:108-109)
+    const float sgn = copysignf(1.0f, sw.z);
+    const float oa = __fdividef(-1.0f, sgn + sw.z);      // |sgn + sw.z| in [1, 2]: MUFU.RCP + FMUL instead of the IEEE sequence
+    const float ob = sw.x * sw.y * oa;
+    V3 su = v3(1.0f + sgn * sw.x * sw.x * oa, sgn * ob, -sgn * sw.x);
+    V3 sv = v3(ob, sgn + sw.y * sw.y * oa, -sw.y);
+    float cosAMax = M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
+    float eps1 = RandomFloat01(rng), eps2 = RandomFloat01(rng);
+    float cosA = 1.0f - eps1 + eps1 * cosAMax;
+    float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
+    float phi = 2.0f * TPT_PI * eps2;
+    float sp, cp;
+    __sincosf(phi, &sp, &cp);
+    l = su * (cp * sinA) + sv * (sp * sinA) + sw * cosA;
+    float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
+    float dl = dot(l, nl);
+    float m = (0.0f < dl) ? dl : 0.0f;
+    return m * omega * (1.0f / TPT_PI);
+}
+
+// Metal bounce direction (Test.cpp:137-150); the path goes on when dot(result, normal) > 0. With roughness == 0 the
+// unit-sphere sample has zero weight, so the fast mode skips drawing it (the exact mode must draw it: it advances the
+// shared RNG stream).
+__device__ __forceinline__ V3 metal_dir(V3 d, V3 normal, float roughness, uint32_t& rng)
+{
+    V3 refl = reflect(d, normal);
+    if (roughness != 0.0f) refl = refl + roughness * fast_in_unit_sphere(rng);
+    return M<false>::normalize(refl);
+}
+
+// One iteration of the per-lane path state machine every fast kernel shades with: intersect the lane's current ray
 // (path or shadow) against all spheres, then shade. Returns true when the lane's path has ended (st.col is final).
 template <int LS, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
@@ -1015,11 +833,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 }
                 else if (opaque_int(mtype) == kMetal)
                 {
-                    // Test.cpp:137-150; with roughness == 0 the unit-sphere sample has zero weight, so the fast
-                    // mode skips drawing it (the exact mode must draw it: it advances the shared RNG stream)
-                    V3 refl = reflect(st.d, normal);
-                    if (mat.roughness != 0.0f) refl = refl + mat.roughness * fast_in_unit_sphere(st.rng);
-                    V3 outDir = M<false>::normalize(refl);
+                    V3 outDir = metal_dir(st.d, normal, mat.roughness, st.rng);
                     if (dot(outDir, normal) > 0.0f)
                     {
                         if (LS == kLsOff || st.doMaterialE) st.col = st.col + st.thr * mat.emissive;
@@ -1054,36 +868,10 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
     }
     if (LS != kLsOff && wantLight)
     {
-        int j = lightFrom;
-        while (j < sc.nLights && sc.lights[j].id == st.mid) ++j;
+        const int j = next_light(sc, lightFrom, st.mid);
         if (j < sc.nLights)
         {
-            const LightRec Lr = sc.lights[j];
-            V3 scn = v3(Lr.cx, Lr.cy, Lr.cz);
-            V3 pc = scn - st.o;
-            float d2 = dot(pc, pc);
-            float inv = __frsqrt_rn(d2);          // d2 is a squared distance between distinct spheres: never denormal
-            V3 sw = pc * inv;
-            // any orthonormal (su, sv) around sw gives the same cone-sample distribution (phi is uniform): use the
-            // branch-free basis of Duff et al. 2017 instead of normalize(cross(up, sw)), cross(sw, su) (Test.cpp:108-109)
-            const float sgn = copysignf(1.0f, sw.z);
-            const float oa = __fdividef(-1.0f, sgn + sw.z);      // |sgn + sw.z| in [1, 2]: MUFU.RCP + FMUL instead of the IEEE sequence
-            const float ob = sw.x * sw.y * oa;
-            V3 su = v3(1.0f + sgn * sw.x * sw.x * oa, sgn * ob, -sgn * sw.x);
-            V3 sv = v3(ob, sgn + sw.y * sw.y * oa, -sw.y);
-            float cosAMax = M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
-            float eps1 = RandomFloat01(st.rng), eps2 = RandomFloat01(st.rng);
-            float cosA = 1.0f - eps1 + eps1 * cosAMax;
-            float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
-            float phi = 2.0f * TPT_PI * eps2;
-            float sp, cp;
-            __sincosf(phi, &sp, &cp);
-            V3 l = su * (cp * sinA) + sv * (sp * sinA) + sw * cosA;
-            float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
-            float dl = dot(l, st.nl);
-            float m = (0.0f < dl) ? dl : 0.0f;
-            st.pend = m * omega * (1.0f / TPT_PI);
-            st.d = l;
+            st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
             st.kind = 1 + j;
         }
         else
@@ -1096,6 +884,137 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         }
     }
     return finished;
+}
+
+// ---- variant 0 ------------------------------------------------------------------------------------------------
+__global__ void __launch_bounds__(kFastThreads)
+k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes)
+{
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ uint64_t bar;
+    __shared__ float sW[kMaxFramesPerDraw];
+    __shared__ float sWPrev;
+    stage_blob(smem, blob, stagedBytes, &bar);
+    if (threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); sWPrev = wp; }
+    __syncthreads();
+    SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
+
+    // 16x16 pixel block, each warp an 8x4 patch
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int tilesX = (p.width + 15) / 16;
+    const int tx = blockIdx.x % tilesX, ty = blockIdx.x / tilesX;
+    const int x = tx * 16 + (warp & 1) * 8 + (lane & 7);
+    const int ri = ty * 16 + (warp >> 1) * 4 + (lane >> 3);
+    unsigned rc = 0;
+    if (x < p.width && ri < p.numRows)
+    {
+        const int y = region_pixel(p, ri, x).y;
+        SerialHitter<false> hitter;
+        V3 acc = v3(0, 0, 0);
+        const float invSpp = 1.0f / (float)p.spp;
+        for (int fi = 0; fi < p.numFrames; ++fi)
+        {
+            // one stream per pixel and frame, carried across the pixel's samples
+            uint32_t state = pixel_seed((uint32_t)(y * p.width + x), (uint32_t)(p.frame0 + fi));
+            V3 col = v3(0, 0, 0);
+            for (int s = 0; s < p.spp; ++s)
+            {
+                QPath st;
+                const Ray r = fast_camera_ray(p, x, y, state);
+                begin_path(st, r, state);
+                while (!path_step<kLsRuntime>(sc, st, rc, hitter)) {}
+                state = st.rng;
+                col = col + st.col;
+            }
+            acc = acc + col * (invSpp * sW[fi]);
+        }
+        float* px = p.image + region_pixel(p, ri, x).off * 4;
+        st_stream_f4(px, blend_prev(p, px, sWPrev, acc.x, acc.y, acc.z));
+    }
+    flush_ray_count(p.rayCounter, rc, lane);
+}
+
+// ---- variant 1 ------------------------------------------------------------------------------------------------
+template <int MINB>
+__global__ void __launch_bounds__(kFastThreads, MINB)
+k_fast_persistent(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
+                  uint32_t stagedBytes, int numTiles)
+{
+    extern __shared__ __align__(128) unsigned char smem[];
+    __shared__ uint64_t bar;
+    __shared__ float sW[kMaxFramesPerDraw];
+    __shared__ float sWPrev;
+    __shared__ float sAcc[kTilePix * 3];
+    __shared__ int sTile;
+    __shared__ int sTask;
+    stage_blob(smem, blob, stagedBytes, &bar);
+    if (threadIdx.x == 0) { float wp; blend_weights(p, sW, wp); sWPrev = wp; }
+    for (int i = threadIdx.x; i < kTilePix * 3; i += kFastThreads) sAcc[i] = 0.0f;
+    SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
+    const int lane = threadIdx.x & 31;
+    const long long regionPix = (long long)p.numRows * p.width;
+    const int S = p.spp * p.numFrames;          // samples per pixel in this draw
+    const float invSpp = 1.0f / (float)p.spp;
+    SerialHitter<false> hitter;
+    unsigned rc = 0;
+
+    for (;;)
+    {
+        __syncthreads(); // sAcc zeroed / previous tile written
+        if (threadIdx.x == 0) { sTile = (int)atomicAdd(p.workCounter, 1u); sTask = 0; }
+        __syncthreads();
+        const int tile = sTile;
+        if (tile >= numTiles) break;
+        const long long pix0 = (long long)tile * kTilePix;
+        const int tilePix = (int)(regionPix - pix0 < kTilePix ? regionPix - pix0 : kTilePix);
+        const int tileTasks = tilePix * S;
+
+        QPath st;
+        st.active = false;
+        for (;;)
+        {
+            // ---- regeneration: lanes without a path take the next (pixel, sample) of the tile
+            unsigned need = __ballot_sync(0xffffffffu, !st.active);
+            if (need)
+            {
+                int base = 0;
+                const int leader = __ffs(need) - 1;
+                if (lane == leader) base = atomicAdd(&sTask, __popc(need));
+                base = __shfl_sync(0xffffffffu, base, leader);
+                if (!st.active)
+                {
+                    const int task = base + __popc(need & ((1u << lane) - 1u));
+                    if (task < tileTasks)
+                    {
+                        // samples of one pixel sit in adjacent lanes: coherent primary rays
+                        const int pixIn = task / S, sIdx = task % S;
+                        const int fi = sIdx / p.spp;
+                        const RegionPixel q = region_pixel(p, pix0 + pixIn);
+                        uint32_t rng = pixel_seed((uint32_t)(q.y * p.width + q.x) * (uint32_t)p.spp + (uint32_t)(sIdx % p.spp),
+                                                  (uint32_t)(p.frame0 + fi));
+                        const Ray r = fast_camera_ray(p, q.x, q.y, rng);
+                        begin_path(st, r, rng);
+                        st.pixOff = (uint32_t)pixIn;        // pixel index inside the tile
+                        st.weight = invSpp * sW[fi];
+                    }
+                }
+            }
+            if (!__any_sync(0xffffffffu, st.active)) break;
+
+            if (path_step<kLsRuntime>(sc, st, rc, hitter))
+            {
+                atomicAdd(&sAcc[st.pixOff * 3 + 0], st.col.x * st.weight);
+                atomicAdd(&sAcc[st.pixOff * 3 + 1], st.col.y * st.weight);
+                atomicAdd(&sAcc[st.pixOff * 3 + 2], st.col.z * st.weight);
+                st.active = false;
+            }
+        }
+
+        // ---- tile done
+        __syncthreads();
+        write_tile(p, sAcc, pix0, tilePix, sWPrev, kFastThreads);
+    }
+    flush_ray_count(p.rayCounter, rc, lane);
 }
 
 // Diagnostic build (-DTPT_TRACE_WARPS=1, tools/warp_trace.py): every warp of k_fast_queue records global-timer stamps (entry,
@@ -1544,7 +1463,7 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
 
 // ---- variant 6 ------------------------------------------------------------------------------------------------
 // "block wavefront": the persistent design of the north star taken literally. A CTA keeps kWaveSlots path slots in
-// SHARED memory (11 float4 per slot) and runs every iteration in three phases separated by block barriers:
+// SHARED memory (9 float4 per slot) and runs every iteration in three phases separated by block barriers:
 //   sweep     thread i regenerates slot i if it is free (next path of the CTA's chunk) and intersects slot i's
 //             ray (path or shadow) against all spheres -> every lane has a ray, no divergence outside pass 2;
 //   sort      the slot is classified {miss, lambert, metal, dielectric, shadow-return, terminal} and appended to
@@ -1553,12 +1472,14 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
 //             material type (Scatter(), Test.cpp:83-193, without divergence); Lambert vertices and returning
 //             shadow rays append themselves to the light list, processed the same way in a third phase
 //             (explicit light sampling, Test.cpp:96-133).
-// Radiance leaves through the same 128-bit vector reductions as variant 3.
+// The shading is path_step's, phase by phase: the same metal bounce, light choice and light-cone sample, and the same
+// scalar shadow-ray weight. Radiance leaves through the same 128-bit vector reductions as variant 3.
 constexpr int kWaveThreads = 256;
 constexpr int kWaveSlots = 256;        // one slot per thread
-constexpr int kWaveFields = 11;
+constexpr int kWaveFields = 9;
 constexpr int kWaveChunk = 4096;       // paths taken from the global counter at a time
-enum { WF_O = 0, WF_D, WF_THR, WF_COL, WF_NEXT, WF_THRALB, WF_NL, WF_ALB, WF_PEND, WF_POS, WF_NRM };
+// WF_NL.w: the weight m * omega / pi of the slot's shadow ray in flight (QPath::pend)
+enum { WF_O = 0, WF_D, WF_THR, WF_COL, WF_NEXT, WF_THRALB, WF_NL, WF_POS, WF_NRM };
 enum { WT_MISS = 0, WT_LAMBERT, WT_METAL, WT_DIEL, WT_SHADOW, WT_TERMINAL, WT_COUNT };
 // a slot's state word (WF_D.w): bits 0-15 kind (0 path ray, 1 + j shadow ray of light j, kKindFree), bits 16-23 depth,
 // bit 24 doMaterialE. The launcher refuses nLights >= kKindFree.
@@ -1642,9 +1563,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                         const uint32_t fi = fdiv(s, wa.divSpp), ss = s - fi * (uint32_t)p.spp;
                         const int y = p.row0 + (int)ri * p.rowStep;
                         uint32_t rng = pixel_seed((uint32_t)(y * p.width + (int)x) * (uint32_t)p.spp + ss, (uint32_t)p.frame0 + fi);
-                        float u = ((float)x + RandomFloat01(rng)) * p.invWidth;
-                        float v = ((float)y + RandomFloat01(rng)) * p.invHeight;
-                        Ray r = fast_get_ray(p.cam, u, v, rng);
+                        Ray r = fast_camera_ray(p, (int)x, y, rng);
                         kind = 0; misc = 0 | (0 << 16) | (1 << 24);
                         fd = make_float4(r.dir.x, r.dir.y, r.dir.z, __int_as_float(misc));
                         WFLD(WF_O, tid) = make_float4(r.orig.x, r.orig.y, r.orig.z, 0.0f);
@@ -1724,7 +1643,12 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                     {
                         const int j = (m2 & 0xffff) - 1;
                         const int hid = __float_as_int(WFLD(WF_POS, slot).w);
-                        if (hid == sc.lights[j].id) { const float4 pe = WFLD(WF_PEND, slot); col = col + v3(pe.x, pe.y, pe.z); }
+                        const LightRec& Lj = sc.lights[j];
+                        if (hid == Lj.id)
+                        {
+                            const float4 ta = WFLD(WF_THRALB, slot);
+                            col = col + (v3(ta.x, ta.y, ta.z) * v3(Lj.ex, Lj.ey, Lj.ez)) * WFLD(WF_NL, slot).w;
+                        }
                         wantLight = true;   // next light index = j + 1, kept in kind
                     }
                     else
@@ -1744,7 +1668,6 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                             WFLD(WF_NEXT, slot) = make_float4(nextDir.x, nextDir.y, nextDir.z, WFLD(WF_NEXT, slot).w);
                             WFLD(WF_THRALB, slot) = make_float4(thrAlb.x, thrAlb.y, thrAlb.z, __int_as_float(mid));
                             WFLD(WF_NL, slot) = make_float4(nl.x, nl.y, nl.z, 0.0f);
-                            WFLD(WF_ALB, slot) = make_float4(mat.albedo.x, mat.albedo.y, mat.albedo.z, 0.0f);
                             WFLD(WF_O, slot) = make_float4(pos.x, pos.y, pos.z, 0.0f);
                             m2 = (m2 & ~0xffff) | 0;    // kind := "before light 0" (light phase advances it)
                             wantLight = true;
@@ -1755,9 +1678,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                             bool ok;
                             if (T == WT_METAL)
                             {
-                                V3 refl = reflect(d, normal);
-                                if (mat.roughness != 0.0f) refl = refl + mat.roughness * fast_in_unit_sphere(rng);
-                                outDir = M<false>::normalize(refl);
+                                outDir = metal_dir(d, normal, mat.roughness, rng);
                                 att = mat.albedo;
                                 ok = dot(outDir, normal) > 0.0f;
                             }
@@ -1809,36 +1730,16 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                     float4 fdd = WFLD(WF_D, slot);
                     int m2 = __float_as_int(fdd.w);
                     const float4 fta = WFLD(WF_THRALB, slot);
-                    const int mid = __float_as_int(fta.w);
-                    int j = m2 & 0xffff;               // kind k = shadow ray of light k-1 just returned -> next is light k
-                    while (j < sc.nLights && sc.lights[j].id == mid) ++j;
+                    // kind k = shadow ray of light k-1 just returned -> next is light k
+                    const int j = next_light(sc, m2 & 0xffff, __float_as_int(fta.w));
                     if (j < sc.nLights)
                     {
-                        const LightRec Lr = sc.lights[j];
-                        const float4 fo = WFLD(WF_O, slot), fnl = WFLD(WF_NL, slot), fal = WFLD(WF_ALB, slot);
-                        float4 fthr = WFLD(WF_THR, slot);
-                        uint32_t rng = __float_as_uint(fthr.w);
-                        const V3 o = v3(fo.x, fo.y, fo.z);
-                        V3 pc = v3(Lr.cx, Lr.cy, Lr.cz) - o;
-                        float d2 = dot(pc, pc);
-                        float inv = rsqrtf(d2);
-                        V3 sw = pc * inv;
-                        V3 su = M<false>::normalize(cross(fabsf(sw.x) > 0.01f ? v3(0, 1, 0) : v3(1, 0, 0), sw));
-                        V3 sv = cross(sw, su);
-                        float cosAMax = M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
-                        float eps1 = RandomFloat01(rng), eps2 = RandomFloat01(rng);
-                        float cosA = 1.0f - eps1 + eps1 * cosAMax;
-                        float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
-                        float sp, cp;
-                        __sincosf(2.0f * TPT_PI * eps2, &sp, &cp);
-                        V3 l = su * (cp * sinA) + sv * (sp * sinA) + sw * cosA;
-                        float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
-                        float dl = dot(l, v3(fnl.x, fnl.y, fnl.z));
-                        float m = (0.0f < dl) ? dl : 0.0f;
-                        V3 pend = v3(fthr.x, fthr.y, fthr.z) * ((v3(fal.x, fal.y, fal.z) * v3(Lr.ex, Lr.ey, Lr.ez)) * (m * omega * (1.0f / TPT_PI)));
-                        WFLD(WF_PEND, slot) = make_float4(pend.x, pend.y, pend.z, 0.0f);
-                        fthr.w = __uint_as_float(rng);
-                        WFLD(WF_THR, slot) = fthr;
+                        const float4 fo = WFLD(WF_O, slot), fnl = WFLD(WF_NL, slot);
+                        uint32_t rng = __float_as_uint(WFLD(WF_THR, slot).w);
+                        V3 l;
+                        const float pend = sample_light_cone(sc.lights[j], v3(fo.x, fo.y, fo.z), v3(fnl.x, fnl.y, fnl.z), rng, l);
+                        WFLD(WF_NL, slot).w = pend;
+                        WFLD(WF_THR, slot).w = __uint_as_float(rng);
                         m2 = (m2 & ~0xffff) | (1 + j);
                         WFLD(WF_D, slot) = make_float4(l.x, l.y, l.z, __int_as_float(m2));
                     }

@@ -559,58 +559,6 @@ TPT_HD V3 trace_exact(const SceneView& sc, Ray r, uint32_t& state, unsigned& ray
     return result;
 }
 
-// Same estimator, front-to-back accumulation, no stack (fast mode).
-template <class Hitter>
-TPT_HD V3 trace_fast(const SceneView& sc, Ray r, uint32_t& state, unsigned& rayCount, const Hitter& hitter)
-{
-    V3 col = v3(0, 0, 0), thr = v3(1, 1, 1);
-    bool doMaterialE = true;
-    for (int depth = 0;; ++depth)
-    {
-        ++rayCount;
-        float t;
-        int id = hitter.hit(sc, r.orig, r.dir, TPT_MIN_T, TPT_MAX_T, t);
-        if (id < 0) { col = col + thr * sky(r.dir, sc); break; }
-        Q4 s = ld_sph(sc, id);
-        V3 pos = r.orig + r.dir * t;
-        V3 normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];
-        int mid = id < sc.count ? id : sc.count;
-        Mat mat = load_mat(sc, mid);
-        if (depth >= TPT_MAX_DEPTH) { col = col + thr * mat.emissive; break; }
-        V3 attenuation, outDir;
-        if (mat.type == kLambert)
-        {
-            V3 target = pos + normal + RandomUnitVector<false>(state);
-            outDir = M<false>::normalize(target - pos);
-            attenuation = mat.albedo;
-            if (doMaterialE) col = col + thr * mat.emissive;
-            for (int j = 0; j < sc.nLights; ++j)
-            {
-                const LightRec L = sc.lights[j];
-                if (L.id == mid) continue;
-                V3 l, contrib;
-                sample_light<false>(L, pos, normal, r.dir, mat.albedo, state, l, contrib);
-                ++rayCount;
-                float ts;
-                int hid = hitter.hit(sc, pos, l, TPT_MIN_T, TPT_MAX_T, ts);
-                if (hid == L.id) col = col + thr * contrib;
-            }
-            doMaterialE = emission_after_lambert(sc);
-        }
-        else
-        {
-            bool ok = scatter_specular<false>(mat, r.dir, pos, normal, state, attenuation, outDir);
-            if (!ok) { col = col + thr * mat.emissive; break; }   // Test.cpp:218-221: full matE
-            if (doMaterialE) col = col + thr * mat.emissive;
-            doMaterialE = true;
-        }
-        thr = thr * attenuation;
-        r.orig = pos;
-        r.dir = outDir;
-    }
-    return col;
-}
-
 // Test.cpp:272-276
 TPT_HD float lerp_fac(int frameCount, unsigned flags)
 {
