@@ -77,7 +77,7 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * time it is seen so both copies run at full PCIe rate; only safe when the buffer outlives the context, as a
  * reference shell's does; default 0 — buffers that are already pinned are detected by CUDA on their own), "host_bands" (1..8, default 3:
  * host-buffer fast draws are split into row bands on separate streams so the D2H of one band overlaps the tracing of
- * the next), "host_progress" (default 1: with fast variant 3/4 a single kernel publishes per-band completion counters and the
+ * the next), "host_progress" (default 1: with fast variant 3/4/9 a single kernel publishes per-band completion counters and the
  * copy stream waits on them with cuStreamWaitValue32, "progress_bands" bands, default 4; 0 falls back to host_bands),
  * "fast_kform" (fast kernels' sphere sweep: 0 reference form, 1 expanded form, 2 (default) expanded form on a pair-interleaved
  * sphere array, one 128-bit shared load per coordinate of two spheres — the slab queue of a scene of at most 64 padded

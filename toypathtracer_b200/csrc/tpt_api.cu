@@ -51,8 +51,7 @@ struct tpt_context
     int spp = 4;
 
     // options
-    int fastVariant = -1;     // -1 = auto: 3 (slab queue + L2 reductions; 7 = material-sorted block wavefront from 1024 spheres) for device buffers, 8 (warp-owned groups, direct coalesced
-                              // write-out) when a host-buffer draw can store straight into page-locked memory
+    int fastVariant = -1;     // -1 = auto (fast_auto_variant)
     int fastKForm = 2;        // 0: reference-form sweep, 1: expanded form, 2: expanded form on the pair array (slab queue: in the
                               // kernel parameter for scenes of <= 64 padded spheres), 3: as 2 with the pair array always in
                               // shared memory (A/B); gated per scene by kformOk
@@ -103,7 +102,7 @@ struct tpt_context
     cudaEvent_t bandEvent[kMaxBands] = {};
     cudaEvent_t forkEvent = nullptr;
 
-    // progress-triggered D2H (fast variant 3/4): the trace kernel publishes per-band completion counters, the copy
+    // progress-triggered D2H (fast variants 3/4/9): the trace kernel publishes per-band completion counters, the copy
     // stream waits on them with stream memory operations and copies a band while later bands are still being traced
     typedef CUresult (*WaitValue32Fn)(CUstream, CUdeviceptr, cuuint32_t, unsigned int);
     WaitValue32Fn waitValue32 = nullptr;
@@ -395,20 +394,6 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     return fail_msg(ctx, "tpt_set_option: unknown key");
 }
 
-// Copies the rows y_i = row0 + i*rowStep (or the packed band) of an image of pixBytes-byte pixels (float4 by default)
-// between host and device.
-static cudaError_t copy_rows(void* dstBase, const void* srcBase, int width, int row0, int numRows, int rowStep, int packed,
-                             cudaMemcpyKind kind, cudaStream_t stream, size_t pixBytes = 16)
-{
-    char* dst = (char*)dstBase;
-    const char* src = (const char*)srcBase;
-    const size_t rowBytes = (size_t)width * pixBytes;
-    if (packed) return cudaMemcpyAsync(dst, src, rowBytes * numRows, kind, stream);
-    const size_t off = (size_t)row0 * rowBytes;
-    if (rowStep == 1) return cudaMemcpyAsync(dst + off, src + off, rowBytes * numRows, kind, stream);
-    return cudaMemcpy2DAsync(dst + off, rowBytes * rowStep, src + off, rowBytes * rowStep, rowBytes, numRows, kind, stream);
-}
-
 static int ensure(tpt_context* ctx, void** p, size_t* cap, size_t bytes, const char* what)
 {
     if (bytes <= *cap) return 0;
@@ -464,9 +449,10 @@ static int finish_kernels(tpt_context* ctx, cudaStream_t stream, int n, bool wan
         CK(cudaMallocHost(&ctx->hPinned, (size_t)n * sizeof(unsigned long long)), "cudaMallocHost");
         ctx->hPinnedCap = n;
     }
+    note_launch();
     k_accumulate_rays<<<1, 1, 0, stream>>>(ctx->dRayCounters, n, ctx->dAccum, wantCounts ? ctx->hPinned : nullptr);
     CK(cudaGetLastError(), "accumulate launch");
-    ctx->lastLaunches += 1;
+    ctx->lastLaunches = t_lastKernels.launches;
     return 0;
 }
 
@@ -526,263 +512,15 @@ static DrawParams image_params(const tpt_context* ctx, int width, int height, in
     return p;
 }
 
-int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
-             int row0, int numRows, int rowStep, int packed,
-             float* backbuffer, int bufferOnDevice, unsigned testFlags, int mode,
-             long long* outRayCount, long long* outRaysPerFrame, void* cudaStreamArg)
-{
-    if (!ctx) return (int)cudaErrorInvalidValue;
-    if (!ctx->haveScene) return fail_msg(ctx, "tpt_draw: no scene (call tpt_set_scene after UpdateTest)");
-    if (!backbuffer || width <= 0 || height <= 0 || numFrames <= 0 || frameCount < 0 || numRows < 0 || rowStep <= 0 || row0 < 0)
-        return fail_msg(ctx, "tpt_draw: bad arguments");
-    if (mode != TPT_MODE_EXACT && mode != TPT_MODE_FAST && mode != TPT_MODE_REFGPU && mode != TPT_MODE_REFGPU_FAST)
-        return fail_msg(ctx, "tpt_draw: unknown mode");
-    const bool refgpu = mode == TPT_MODE_REFGPU || mode == TPT_MODE_REFGPU_FAST;
-    // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
-    if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
-    if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
-    cudaStream_t stream;
-    SceneDev scene;
-    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-
-    const size_t bufRows = packed ? (size_t)numRows : (size_t)height;
-    const size_t bufBytes = bufRows * width * 4 * sizeof(float);
-    float* dImage = backbuffer;
-    bool needPrev = true;
-    bool zeroCopy = false;
-    if (!bufferOnDevice && ctx->registerHost && (ctx->registeredPtr != backbuffer || ctx->registeredBytes != bufBytes))
-    {
-        if (ctx->registeredPtr) { cudaHostUnregister(ctx->registeredPtr); ctx->registeredPtr = nullptr; }
-        // page-lock (and map) the caller's buffer once: copies run at full PCIe rate and the kernels can store into it
-        // directly; failure is not fatal
-        if (cudaHostRegister(backbuffer, bufBytes, cudaHostRegisterMapped) == cudaSuccess)
-        {
-            ctx->registeredPtr = backbuffer; ctx->registeredBytes = bufBytes;
-        }
-        else (void)cudaGetLastError();
-    }
-    // auto: the warp slab queue. Only where the sweep dwarfs everything else (>= 1024 spheres) AND the queue kernel cannot
-    // run a packed-pair sweep (pair array does not fit, or "fast_kform" < 2) is the block wavefront that sorts its paths
-    // by material before Scatter() faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312)
-    const bool waveFits = (long long)((numRows * (long long)width + 127) / 128) * 128 * ctx->spp * (numFrames < 256 ? numFrames : 256) <= 0x7fffffffLL;
-    SceneDev autoScene = ctx->scene;
-    autoScene.kformMode = ctx->fastKForm;
-    // (the wavefront keeps 1 + the light index in 16 bits: scenes with 65 535 or more lights stay on the slab queue)
-    int fastVariant = ctx->fastVariant < 0 ? (ctx->scene.count >= 1024 && waveFits && fast_queue_kform(autoScene) < 2 &&
-                                              ctx->scene.nLights < 0xffff ? 7 : 3) : ctx->fastVariant;
-    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && (ctx->fastVariant < 0 || fast_variant_writes_final_pixels(ctx->fastVariant)))
-    {
-        // Host-buffer draw whose `prev` has zero weight, into page-locked memory the GPU can address: the trace kernel's
-        // coalesced 128-bit pixel stores go straight into the caller's buffer over PCIe while the other pixels are still
-        // being traced — no staging image, no device-to-host copy after the kernel.
-        cudaPointerAttributes attr;
-        if (prev_weight(frameCount, numFrames, testFlags) == 0.0f && numFrames <= 256 && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
-            attr.type == cudaMemoryTypeHost && attr.devicePointer)
-        {
-            dImage = (float*)attr.devicePointer;
-            zeroCopy = true;
-            needPrev = false;
-            fastVariant = ctx->fastVariant < 0 ? 8 : ctx->fastVariant;
-        }
-        else (void)cudaGetLastError();
-    }
-    if (!bufferOnDevice && !zeroCopy)
-    {
-        auto& st = ctx->staging[kStageImage];
-        int r = ensure(ctx, &st.ptr, &st.cap, bufBytes, "cudaMalloc image");
-        if (r) return r;
-        dImage = (float*)st.ptr;
-        // `prev` is an input of the blend (Test.cpp:293). Exact mode always uploads it (NaN/Inf * 0 and the
-        // untouched alpha are part of bit parity). Fast mode uploads it only when prev has a non-zero weight;
-        // otherwise the kernel writes alpha = 0, which is what every reference shell's zero-initialised buffer
-        // holds (TestWin.cpp:73-74, Renderer.mm:148-149, Emscripten/main.cpp:50-51).
-        // (REFGPU writes alpha = 1 and lerp(col, prev, 0) does not read prev: same rule as the fast mode)
-        needPrev = mode == TPT_MODE_EXACT || prev_weight(frameCount, numFrames, testFlags) != 0.0f;
-        if (needPrev)
-        {
-            cudaError_t e = copy_rows(dImage, backbuffer, width, row0, numRows, rowStep, packed, cudaMemcpyHostToDevice, stream);
-            if (e != cudaSuccess) return fail(ctx, e, "H2D backbuffer");
-        }
-    }
-
-    // frames per launch: exact mode needs numFrames*numRows*width float4 of scratch when numFrames > 1
-    int framesPerLaunch = numFrames;
-    if (mode == TPT_MODE_EXACT && numFrames > 1)
-    {
-        const size_t perFrame = (size_t)numRows * width * 16;
-        size_t fit = ctx->maxScratchBytes / perFrame;
-        if (fit < 1) fit = 1;
-        if ((size_t)framesPerLaunch > fit) framesPerLaunch = (int)fit;
-    }
-    if (mode == TPT_MODE_FAST && framesPerLaunch > 256) framesPerLaunch = 256;
-
-    if (int r = start_kernels(ctx, stream, numFrames)) return r;
-    DrawParams p = image_params(ctx, width, height, row0, numRows, rowStep, packed, ctx->spp, testFlags);
-    p.image = dImage;
-    p.workCounter = next_work_counter(ctx);
-    // alpha is never written by the reference (Maths.h:38). When `prev` has zero weight the fast kernels keep the alpha
-    // that is in the buffer, unless the staging image was not uploaded (host buffer) or the caller waived it.
-    p.zeroAlpha = (ctx->fastAlphaZero || (!bufferOnDevice && !needPrev)) ? 1 : 0;     // (zero-copy: never reads host memory)
-
-    // Host-buffer fast draws: split the rows into bands, one stream per band (earlier band = higher priority). Each
-    // stream runs prepare + trace for its band and then copies the band to the caller's buffer, so the D2H of band b
-    // overlaps the tracing of band b+1 and the persistent CTAs of band b+1 fill the SMs as band b's tail drains.
-    bool pipelined = mode == TPT_MODE_FAST && !bufferOnDevice && (fastVariant == 9 || (fastVariant >= 3 && fastVariant <= 7)) && ctx->hostBands > 1 &&
-                     (rowStep == 1 || packed) && framesPerLaunch == numFrames && numRows >= 16 * ctx->hostBands;
-    // the per-band completion counters are 32-bit (cuStreamWaitValue32): a band never holds more paths than the image
-    const bool progress = pipelined && ctx->waitValue32 && ctx->hostProgress && (fastVariant == 3 || fastVariant == 4 || fastVariant == 9) &&
-                          (long long)numRows * width * ctx->spp * numFrames <= 0xFFFFFFFFLL;
-    if (progress)
-    {
-        // ONE kernel for the whole image; the copy stream waits on the kernel's per-band completion counters
-        const int NB = ctx->progressBands;
-        unsigned int expected[16];
-        CK(cudaMemsetAsync(ctx->dBandDone, 0, 64, stream), "zero band counters");
-        CK(cudaEventRecord(ctx->forkEvent, stream), "fork event");
-        CK(cudaStreamWaitEvent(ctx->copyStream, ctx->forkEvent, 0), "copy stream wait");
-        p.frame0 = frameCount; p.numFrames = numFrames; p.rayCounter = ctx->dRayCounters;
-        cudaError_t e = launch_fast(p, scene, fastVariant, ctx->numSMs, stream, ctx->dBandDone, NB, expected);
-        if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-        ctx->lastLaunches += fast_kernel_launches(p, fastVariant);
-        CK(cudaEventRecord(ctx->tlKernelEnd, stream), "timeline event");
-        ctx->tlBands = 0;
-        const long long regionPix = (long long)numRows * width, slab = fast_slab_pixels();
-        const long long mtiles = (regionPix + slab - 1) / slab, mpb = (mtiles + NB - 1) / NB;
-        const size_t firstPix = packed ? 0 : (size_t)row0 * width;
-        for (int b = NB - 1; b >= 0; --b)     // the kernel walks the image from its last macro-tile down: last band first
-        {
-            const long long p0 = (long long)b * mpb * slab, p1 = (long long)(b + 1) * mpb * slab < regionPix ? (long long)(b + 1) * mpb * slab : regionPix;
-            if (p1 <= p0) continue;
-            if (ctx->waitValue32((CUstream)ctx->copyStream, (CUdeviceptr)(ctx->dBandDone + b), expected[b], CU_STREAM_WAIT_VALUE_GEQ) != CUDA_SUCCESS)
-                return fail_msg(ctx, "cuStreamWaitValue32 failed");
-            const size_t off = (firstPix + (size_t)p0) * 4;
-            CK(cudaMemcpyAsync(backbuffer + off, dImage + off, (size_t)(p1 - p0) * 16, cudaMemcpyDeviceToHost, ctx->copyStream), "D2H band");
-            CK(cudaEventRecord(ctx->tlBand[ctx->tlBands++], ctx->copyStream), "timeline event");
-        }
-        CK(cudaEventRecord(ctx->bandEvent[0], ctx->copyStream), "copy event");
-        CK(cudaStreamWaitEvent(stream, ctx->bandEvent[0], 0), "join copies");
-    }
-    else if (pipelined)
-    {
-        const int NB = ctx->hostBands;
-        CK(cudaEventRecord(ctx->forkEvent, stream), "fork event");
-        p.frame0 = frameCount; p.numFrames = numFrames; p.rayCounter = ctx->dRayCounters;
-        for (int b = 0; b < NB; ++b)
-        {
-            const int rb0 = (int)((long long)numRows * b / NB), rb1 = (int)((long long)numRows * (b + 1) / NB);
-            cudaStream_t bs = ctx->bandStream[b];
-            CK(cudaStreamWaitEvent(bs, ctx->forkEvent, 0), "band wait");
-            DrawParams pb = p;
-            pb.row0 = row0 + rb0 * rowStep;
-            pb.numRows = rb1 - rb0;
-            pb.workCounter = p.workCounter + 4 * b;
-            const size_t firstRow = packed ? (size_t)rb0 : (size_t)(row0 + rb0);   // rowStep == 1 when not packed
-            if (packed) pb.image = dImage + firstRow * width * 4;
-            cudaError_t e = launch_fast(pb, scene, fastVariant, ctx->numSMs, bs);
-            if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-            ctx->lastLaunches += fast_kernel_launches(pb, fastVariant);
-            const size_t off = firstRow * width * 4, bytes = (size_t)(rb1 - rb0) * width * 16;
-            CK(cudaMemcpyAsync(backbuffer + off, dImage + off, bytes, cudaMemcpyDeviceToHost, bs), "D2H band");
-            CK(cudaEventRecord(ctx->bandEvent[b], bs), "band event");
-            CK(cudaStreamWaitEvent(stream, ctx->bandEvent[b], 0), "join band");
-        }
-    }
-    for (int f = 0; f < numFrames && !pipelined; f += framesPerLaunch)
-    {
-        const int nf = numFrames - f < framesPerLaunch ? numFrames - f : framesPerLaunch;
-        p.frame0 = frameCount + f;
-        p.numFrames = nf;
-        cudaError_t e;
-        if (mode == TPT_MODE_EXACT && numFrames == 1 && (ctx->exactLookahead > 1 || ctx->exactLookahead == -1) && !(testFlags & TPT_FLAG_ANIMATE))
-        {
-            // frame lookahead (see tpt_context::exactLookahead)
-            tpt_context::LookKey k{};
-            k.width = width; k.height = height; k.row0 = row0; k.numRows = numRows; k.rowStep = rowStep; k.spp = ctx->spp;
-            k.sceneGen = ctx->sceneGen; k.cam = ctx->cam;
-            const tpt_context::LookKey& c = ctx->look;
-            const size_t perFrame = (size_t)numRows * width * 4;           // floats
-            const bool sameSetup = c.width == k.width && c.height == k.height && c.row0 == k.row0 && c.numRows == k.numRows &&
-                                   c.rowStep == k.rowStep && c.spp == k.spp && c.sceneGen == k.sceneGen && !memcmp(&c.cam, &k.cam, sizeof(Camera88));
-            const bool hit = ctx->lookValid && frameCount >= c.frame0 && frameCount < c.frame0 + c.n && sameSetup;
-            if (!hit)
-            {
-                size_t L = ctx->exactLookahead > 1 ? (size_t)ctx->exactLookahead : 1;
-                if (ctx->exactLookahead == -1 && ctx->lookKeyValid && sameSetup && frameCount == c.frame0 + c.n &&
-                    ctx->lookLastServed == c.frame0 + c.n - 1)
-                    L = c.n >= 8 ? 16 : (size_t)c.n * 2;           // the caller consumed the whole window and continues: double it
-                const size_t fit = ctx->maxScratchBytes / (perFrame * 4);
-                if (L > fit) L = fit < 1 ? 1 : fit;
-                int r = ensure(ctx, (void**)&ctx->dLook, &ctx->lookCap, L * perFrame * 4, "cudaMalloc lookahead cache");
-                if (r) return r;
-                r = ensure(ctx, (void**)&ctx->dLookRays, &ctx->lookRaysCap, L * sizeof(unsigned long long), "cudaMalloc lookahead counters");
-                if (r) return r;
-                CK(cudaMemsetAsync(ctx->dLookRays, 0, L * sizeof(unsigned long long), stream), "zero lookahead counters");
-                DrawParams pl = p;
-                pl.frame0 = frameCount; pl.numFrames = (int)L; pl.scratch = ctx->dLook; pl.rayCounter = ctx->dLookRays;
-                e = launch_exact(pl, scene, ctx->exactLanes, ctx->numSMs, stream, /*resolve*/ L == 1);
-                if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-                ctx->lastLaunches += 1;
-                k.frame0 = frameCount; k.n = (int)L;
-                ctx->look = k; ctx->lookValid = L > 1; ctx->lookKeyValid = true; ctx->lookLastServed = frameCount;
-                if (L == 1) { CK(cudaMemcpyAsync(ctx->dRayCounters, ctx->dLookRays, 8, cudaMemcpyDeviceToDevice, stream), "counter copy"); continue; }
-            }
-            const int i = frameCount - ctx->look.frame0;
-            ctx->lookLastServed = frameCount;
-            DrawParams pr = p;
-            pr.frame0 = frameCount; pr.numFrames = 1; pr.scratch = ctx->dLook + (size_t)i * perFrame;
-            e = launch_resolve_exact(pr, stream);
-            ctx->lastLaunches += 1;
-            CK(cudaMemcpyAsync(ctx->dRayCounters, ctx->dLookRays + i, 8, cudaMemcpyDeviceToDevice, stream), "counter copy");
-        }
-        else if (mode == TPT_MODE_EXACT)
-        {
-            p.rayCounter = ctx->dRayCounters + f;
-            p.scratch = nullptr;
-            if (nf > 1)
-            {
-                int r = ensure(ctx, (void**)&ctx->dScratch, &ctx->scratchCap, (size_t)nf * numRows * width * 16, "cudaMalloc scratch");
-                if (r) return r;
-                p.scratch = ctx->dScratch;
-            }
-            e = launch_exact(p, scene, ctx->exactLanes, ctx->numSMs, stream);
-            ctx->lastLaunches += nf > 1 ? 2 : 1;
-        }
-        else if (refgpu)
-        {
-            p.rayCounter = ctx->dRayCounters;
-            e = mode == TPT_MODE_REFGPU ? launch_refgpu_exact(p, scene, ctx->numSMs, stream) : launch_refgpu_fast(p, scene, ctx->numSMs, stream);
-            ctx->lastLaunches += 1;
-        }
-        else
-        {
-            p.rayCounter = ctx->dRayCounters;
-            e = launch_fast(p, scene, fastVariant, ctx->numSMs, stream);
-            ctx->lastLaunches += fast_kernel_launches(p, fastVariant);
-        }
-        if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    }
-    if (int r = finish_kernels(ctx, stream, numFrames, outRayCount || outRaysPerFrame)) return r;
-
-    if (!bufferOnDevice && !pipelined && !zeroCopy)
-    {
-        // only the rows this draw rendered go back: the caller's other rows are not ours to touch (TraceRowJob writes
-        // rows [start,end) only, Test.cpp:278-297)
-        cudaError_t e = copy_rows(backbuffer, dImage, width, row0, numRows, rowStep, packed, cudaMemcpyDeviceToHost, stream);
-        if (e != cudaSuccess) return fail(ctx, e, "D2H backbuffer");
-    }
-    // host-buffer draws are synchronous like DrawTest
-    return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
-}
-
 } // extern "C" (the caller-buffer helpers below are templates, which cannot have C linkage)
 
-// A row region of a draw's image: rows y_i = row0 + i*rowStep (or the packed band) of `width` pixels, see copy_rows.
+// A row region of a draw's image: rows y_i = row0 + i*rowStep (or the packed band) of `width` pixels.
 struct RowRegion { int width, row0, numRows, rowStep, packed; };
 
 enum { kCopyUp = 1, kCopyDown = 2 };
 
-// One caller buffer of tpt_trace_rays, tpt_trace_aovs, tpt_draw_aovs or tpt_draw_samples. A null `ptr` is a buffer the
-// caller left out: it is neither checked nor staged.
+// One caller buffer of tpt_draw, tpt_trace_rays, tpt_trace_aovs, tpt_draw_aovs, tpt_draw_samples or tpt_tonemap_rgba8. A
+// null `ptr` is a buffer the caller left out: it is neither checked nor staged.
 struct CallerBuffer
 {
     const char* name;                   // as the error texts name it
@@ -824,11 +562,18 @@ static int check_buffers(tpt_context* ctx, const char* fn, const CallerBuffer (&
     return 0;
 }
 
-static cudaError_t copy_buffer(const CallerBuffer& b, void* dst, const void* src, cudaMemcpyKind kind, cudaStream_t stream)
+// Copies a buffer between host and device: all of it, or only its region's rows.
+static cudaError_t copy_buffer(const CallerBuffer& b, void* dstBase, const void* srcBase, cudaMemcpyKind kind, cudaStream_t stream)
 {
+    char* dst = (char*)dstBase;
+    const char* src = (const char*)srcBase;
     if (!b.rows) return cudaMemcpyAsync(dst, src, b.bytes, kind, stream);
     const RowRegion& r = *b.rows;
-    return copy_rows(dst, src, r.width, r.row0, r.numRows, r.rowStep, r.packed, kind, stream, b.pixBytes);
+    const size_t rowBytes = (size_t)r.width * b.pixBytes;
+    if (r.packed) return cudaMemcpyAsync(dst, src, rowBytes * r.numRows, kind, stream);
+    const size_t off = (size_t)r.row0 * rowBytes;
+    if (r.rowStep == 1) return cudaMemcpyAsync(dst + off, src + off, rowBytes * r.numRows, kind, stream);
+    return cudaMemcpy2DAsync(dst + off, rowBytes * r.rowStep, src + off, rowBytes * r.rowStep, rowBytes, r.numRows, kind, stream);
 }
 
 // Gives every buffer the pointer its kernels use: a host buffer's staging allocation, grown to the buffer's size and
@@ -857,7 +602,237 @@ static int stage_out(tpt_context* ctx, cudaStream_t stream, const CallerBuffer (
     return 0;
 }
 
+// Page-locks (and maps) the caller's host buffer once ("register_host"): copies run at full PCIe rate and the kernels can
+// store into it directly. Failure is not fatal.
+static void register_host(tpt_context* ctx, void* host, size_t bytes)
+{
+    if (ctx->registeredPtr == host && ctx->registeredBytes == bytes) return;
+    if (ctx->registeredPtr) { cudaHostUnregister(ctx->registeredPtr); ctx->registeredPtr = nullptr; }
+    if (cudaHostRegister(host, bytes, cudaHostRegisterMapped) == cudaSuccess)
+    {
+        ctx->registeredPtr = host; ctx->registeredBytes = bytes;
+    }
+    else (void)cudaGetLastError();
+}
+
+// Exact mode, one frame per call, with frame lookahead (see tpt_context::exactLookahead): a miss traces the window
+// [p.frame0, p.frame0 + L) into the lookahead cache; the frame is then blended from the cache into the image and its ray
+// count copied to the call's counter (a window of one frame is traced straight into the image).
+static int draw_exact_lookahead(tpt_context* ctx, const DrawParams& p, const SceneDev& sc, cudaStream_t stream)
+{
+    const int frame = p.frame0;
+    tpt_context::LookKey k{};
+    k.width = p.width; k.height = p.height; k.row0 = p.row0; k.numRows = p.numRows; k.rowStep = p.rowStep; k.spp = p.spp;
+    k.sceneGen = ctx->sceneGen; k.cam = p.cam;
+    const tpt_context::LookKey& c = ctx->look;
+    const size_t perFrame = (size_t)p.numRows * p.width * 4;           // floats
+    const bool sameSetup = c.width == k.width && c.height == k.height && c.row0 == k.row0 && c.numRows == k.numRows &&
+                           c.rowStep == k.rowStep && c.spp == k.spp && c.sceneGen == k.sceneGen && !memcmp(&c.cam, &k.cam, sizeof(Camera88));
+    const bool hit = ctx->lookValid && frame >= c.frame0 && frame < c.frame0 + c.n && sameSetup;
+    if (!hit)
+    {
+        size_t L = ctx->exactLookahead > 1 ? (size_t)ctx->exactLookahead : 1;
+        if (ctx->exactLookahead == -1 && ctx->lookKeyValid && sameSetup && frame == c.frame0 + c.n &&
+            ctx->lookLastServed == c.frame0 + c.n - 1)
+            L = c.n >= 8 ? 16 : (size_t)c.n * 2;           // the caller consumed the whole window and continues: double it
+        const size_t fit = ctx->maxScratchBytes / (perFrame * 4);
+        if (L > fit) L = fit < 1 ? 1 : fit;
+        int r = ensure(ctx, (void**)&ctx->dLook, &ctx->lookCap, L * perFrame * 4, "cudaMalloc lookahead cache");
+        if (r) return r;
+        r = ensure(ctx, (void**)&ctx->dLookRays, &ctx->lookRaysCap, L * sizeof(unsigned long long), "cudaMalloc lookahead counters");
+        if (r) return r;
+        CK(cudaMemsetAsync(ctx->dLookRays, 0, L * sizeof(unsigned long long), stream), "zero lookahead counters");
+        DrawParams pl = p;
+        pl.numFrames = (int)L; pl.scratch = ctx->dLook; pl.rayCounter = ctx->dLookRays;
+        cudaError_t e = launch_exact(pl, sc, ctx->exactLanes, ctx->numSMs, stream, /*resolve*/ L == 1);
+        if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+        k.frame0 = frame; k.n = (int)L;
+        ctx->look = k; ctx->lookValid = L > 1; ctx->lookKeyValid = true; ctx->lookLastServed = frame;
+        if (L == 1) { CK(cudaMemcpyAsync(ctx->dRayCounters, ctx->dLookRays, 8, cudaMemcpyDeviceToDevice, stream), "counter copy"); return 0; }
+    }
+    const int i = frame - ctx->look.frame0;
+    ctx->lookLastServed = frame;
+    DrawParams pr = p;
+    pr.scratch = ctx->dLook + (size_t)i * perFrame;
+    const cudaError_t e = launch_resolve_exact(pr, stream);
+    CK(cudaMemcpyAsync(ctx->dRayCounters, ctx->dLookRays + i, 8, cudaMemcpyDeviceToDevice, stream), "counter copy");
+    return e == cudaSuccess ? 0 : fail(ctx, e, "kernel launch");
+}
+
+// Host-buffer fast draws can hand the image to the caller's buffer `host` in bands, so that the D2H copies overlap the
+// tracing. Here ONE kernel for the whole image publishes per-band completion counters; the copy stream waits on them
+// (cuStreamWaitValue32) and copies a band while later bands are still being traced.
+static int draw_progress_bands(tpt_context* ctx, const DrawParams& p, const SceneDev& sc, int variant, float* host,
+                               cudaStream_t stream)
+{
+    const int NB = ctx->progressBands;
+    unsigned int expected[16];
+    CK(cudaMemsetAsync(ctx->dBandDone, 0, 64, stream), "zero band counters");
+    CK(cudaEventRecord(ctx->forkEvent, stream), "fork event");
+    CK(cudaStreamWaitEvent(ctx->copyStream, ctx->forkEvent, 0), "copy stream wait");
+    cudaError_t e = launch_fast(p, sc, variant, ctx->numSMs, stream, ctx->dBandDone, NB, expected);
+    if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+    CK(cudaEventRecord(ctx->tlKernelEnd, stream), "timeline event");
+    ctx->tlBands = 0;
+    const long long regionPix = (long long)p.numRows * p.width, slab = fast_slab_pixels();
+    const long long mtiles = (regionPix + slab - 1) / slab, mpb = (mtiles + NB - 1) / NB;
+    const size_t firstPix = p.packed ? 0 : (size_t)p.row0 * p.width;
+    for (int b = NB - 1; b >= 0; --b)     // the kernel walks the image from its last macro-tile down: last band first
+    {
+        const long long p0 = (long long)b * mpb * slab, p1 = (long long)(b + 1) * mpb * slab < regionPix ? (long long)(b + 1) * mpb * slab : regionPix;
+        if (p1 <= p0) continue;
+        if (ctx->waitValue32((CUstream)ctx->copyStream, (CUdeviceptr)(ctx->dBandDone + b), expected[b], CU_STREAM_WAIT_VALUE_GEQ) != CUDA_SUCCESS)
+            return fail_msg(ctx, "cuStreamWaitValue32 failed");
+        const size_t off = (firstPix + (size_t)p0) * 4;
+        CK(cudaMemcpyAsync(host + off, p.image + off, (size_t)(p1 - p0) * 16, cudaMemcpyDeviceToHost, ctx->copyStream), "D2H band");
+        CK(cudaEventRecord(ctx->tlBand[ctx->tlBands++], ctx->copyStream), "timeline event");
+    }
+    CK(cudaEventRecord(ctx->bandEvent[0], ctx->copyStream), "copy event");
+    CK(cudaStreamWaitEvent(stream, ctx->bandEvent[0], 0), "join copies");
+    return 0;
+}
+
+// The same with one launch sequence per band of contiguous or packed rows, each on its own stream (earlier band = higher
+// priority) followed by the band's copy: the D2H of band b overlaps the tracing of band b+1, and the persistent CTAs of
+// band b+1 fill the SMs as band b's tail drains.
+static int draw_row_bands(tpt_context* ctx, const DrawParams& p, const SceneDev& sc, int variant, float* host, cudaStream_t stream)
+{
+    const int NB = ctx->hostBands;
+    CK(cudaEventRecord(ctx->forkEvent, stream), "fork event");
+    for (int b = 0; b < NB; ++b)
+    {
+        const int rb0 = (int)((long long)p.numRows * b / NB), rb1 = (int)((long long)p.numRows * (b + 1) / NB);
+        cudaStream_t bs = ctx->bandStream[b];
+        CK(cudaStreamWaitEvent(bs, ctx->forkEvent, 0), "band wait");
+        DrawParams pb = p;
+        pb.row0 = p.row0 + rb0 * p.rowStep;
+        pb.numRows = rb1 - rb0;
+        pb.workCounter = p.workCounter + 4 * b;
+        const size_t firstRow = p.packed ? (size_t)rb0 : (size_t)(p.row0 + rb0);   // rowStep == 1 when not packed
+        if (p.packed) pb.image = p.image + firstRow * p.width * 4;
+        cudaError_t e = launch_fast(pb, sc, variant, ctx->numSMs, bs);
+        if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
+        const size_t off = firstRow * p.width * 4, bytes = (size_t)(rb1 - rb0) * p.width * 16;
+        CK(cudaMemcpyAsync(host + off, p.image + off, bytes, cudaMemcpyDeviceToHost, bs), "D2H band");
+        CK(cudaEventRecord(ctx->bandEvent[b], bs), "band event");
+        CK(cudaStreamWaitEvent(stream, ctx->bandEvent[b], 0), "join band");
+    }
+    return 0;
+}
+
+// One launch sequence of tpt_draw: frames [p.frame0, p.frame0 + p.numFrames) of the region in `mode`.
+static int draw_frames(tpt_context* ctx, DrawParams p, const SceneDev& sc, int mode, int variant, cudaStream_t stream)
+{
+    cudaError_t e;
+    if (mode == TPT_MODE_EXACT)
+    {
+        if (p.numFrames > 1)
+        {
+            int r = ensure(ctx, (void**)&ctx->dScratch, &ctx->scratchCap, (size_t)p.numFrames * p.numRows * p.width * 16, "cudaMalloc scratch");
+            if (r) return r;
+            p.scratch = ctx->dScratch;
+        }
+        e = launch_exact(p, sc, ctx->exactLanes, ctx->numSMs, stream);
+    }
+    else if (mode == TPT_MODE_REFGPU) e = launch_refgpu_exact(p, sc, ctx->numSMs, stream);
+    else if (mode == TPT_MODE_REFGPU_FAST) e = launch_refgpu_fast(p, sc, ctx->numSMs, stream);
+    else e = launch_fast(p, sc, variant, ctx->numSMs, stream);
+    return e == cudaSuccess ? 0 : fail(ctx, e, "kernel launch");
+}
+
 extern "C" {
+
+int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
+             int row0, int numRows, int rowStep, int packed,
+             float* backbuffer, int bufferOnDevice, unsigned testFlags, int mode,
+             long long* outRayCount, long long* outRaysPerFrame, void* cudaStreamArg)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!ctx->haveScene) return fail_msg(ctx, "tpt_draw: no scene (call tpt_set_scene after UpdateTest)");
+    if (!backbuffer || width <= 0 || height <= 0 || numFrames <= 0 || frameCount < 0 || numRows < 0 || rowStep <= 0 || row0 < 0)
+        return fail_msg(ctx, "tpt_draw: bad arguments");
+    if (mode != TPT_MODE_EXACT && mode != TPT_MODE_FAST && mode != TPT_MODE_REFGPU && mode != TPT_MODE_REFGPU_FAST)
+        return fail_msg(ctx, "tpt_draw: unknown mode");
+    // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
+    if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
+    if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
+    cudaStream_t stream;
+    SceneDev scene;
+    if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+
+    const RowRegion rows = {width, row0, numRows, rowStep, packed};
+    const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);
+    if (!bufferOnDevice && ctx->registerHost) register_host(ctx, backbuffer, bufBytes);
+    const float prevWeight = prev_weight(frameCount, numFrames, testFlags);
+    // Host-buffer draw whose `prev` has zero weight, into page-locked memory the GPU can address: the trace kernel's
+    // coalesced 128-bit pixel stores go straight into the caller's buffer over PCIe while the other pixels are still
+    // being traced — no staging image, no device-to-host copy after the kernel.
+    bool zeroCopy = false;
+    cudaPointerAttributes attr{};
+    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy &&
+        (ctx->fastVariant < 0 || fast_variant_info(ctx->fastVariant).writesFinalPixels))
+    {
+        zeroCopy = prevWeight == 0.0f && numFrames <= kMaxFramesPerDraw && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
+                   attr.type == cudaMemoryTypeHost && attr.devicePointer;
+        if (!zeroCopy) (void)cudaGetLastError();
+    }
+    const int variant = ctx->fastVariant >= 0 ? ctx->fastVariant
+                                              : fast_auto_variant(scene, (long long)numRows * width, ctx->spp, numFrames, zeroCopy);
+
+    // frames per launch: exact mode needs numFrames*numRows*width float4 of scratch when numFrames > 1
+    int framesPerLaunch = numFrames;
+    if (mode == TPT_MODE_EXACT && numFrames > 1)
+    {
+        const size_t perFrame = (size_t)numRows * width * 16;
+        size_t fit = ctx->maxScratchBytes / perFrame;
+        if (fit < 1) fit = 1;
+        if ((size_t)framesPerLaunch > fit) framesPerLaunch = (int)fit;
+    }
+    if (mode == TPT_MODE_FAST && framesPerLaunch > kMaxFramesPerDraw) framesPerLaunch = kMaxFramesPerDraw;
+    const bool lookahead = mode == TPT_MODE_EXACT && numFrames == 1 && (ctx->exactLookahead > 1 || ctx->exactLookahead == -1) &&
+                           !(testFlags & TPT_FLAG_ANIMATE);
+    const FastVariantInfo info = fast_variant_info(variant);
+    const bool banded = mode == TPT_MODE_FAST && !bufferOnDevice && info.rowBands && ctx->hostBands > 1 &&
+                        (rowStep == 1 || packed) && framesPerLaunch == numFrames && numRows >= 16 * ctx->hostBands;
+    // the per-band completion counters are 32-bit (cuStreamWaitValue32): a band never holds more paths than the image
+    const bool progress = banded && ctx->waitValue32 && ctx->hostProgress && info.progressCounters &&
+                          (long long)numRows * width * ctx->spp * numFrames <= 0xFFFFFFFFLL;
+
+    // `prev` is an input of the blend (Test.cpp:293). Exact mode always uploads it (NaN/Inf * 0 and the untouched alpha
+    // are part of bit parity). Fast mode uploads it only when prev has a non-zero weight; otherwise the kernel writes
+    // alpha = 0, which is what every reference shell's zero-initialised buffer holds (TestWin.cpp:73-74,
+    // Renderer.mm:148-149, Emscripten/main.cpp:50-51). (REFGPU writes alpha = 1 and lerp(col, prev, 0) does not read prev:
+    // same rule as the fast mode.) Only the rows this draw renders go back, unless bands deliver them: the caller's other
+    // rows are not ours to touch (TraceRowJob writes rows [start,end) only, Test.cpp:278-297). A zero-copy draw stores
+    // through the buffer's device alias.
+    const bool uploadPrev = mode == TPT_MODE_EXACT || prevWeight != 0.0f;
+    CallerBuffer image[] = {{"backbuffer", zeroCopy ? attr.devicePointer : backbuffer, bufferOnDevice || zeroCopy, 16, bufBytes,
+                             kStageImage, (uploadPrev ? kCopyUp : 0) | (banded ? 0 : kCopyDown), &rows}};
+    if (int r = stage_in(ctx, stream, image)) return r;
+
+    if (int r = start_kernels(ctx, stream, numFrames)) return r;
+    DrawParams p = image_params(ctx, width, height, row0, numRows, rowStep, packed, ctx->spp, testFlags);
+    p.image = (float*)image[0].dev;
+    p.workCounter = next_work_counter(ctx);
+    // alpha is never written by the reference (Maths.h:38). When `prev` has zero weight the fast kernels keep the alpha
+    // that is in the buffer, unless the staging image was not uploaded (host buffer) or the caller waived it.
+    p.zeroAlpha = (ctx->fastAlphaZero || (!bufferOnDevice && !uploadPrev)) ? 1 : 0;     // (zero-copy: never reads host memory)
+    for (int f = 0; f < numFrames; f += framesPerLaunch)     // banded: one pass
+    {
+        p.frame0 = frameCount + f;
+        p.numFrames = numFrames - f < framesPerLaunch ? numFrames - f : framesPerLaunch;
+        p.rayCounter = ctx->dRayCounters + (mode == TPT_MODE_EXACT ? f : 0);    // per-frame counts in exact mode
+        const int r = lookahead  ? draw_exact_lookahead(ctx, p, scene, stream)
+                      : progress ? draw_progress_bands(ctx, p, scene, variant, backbuffer, stream)
+                      : banded   ? draw_row_bands(ctx, p, scene, variant, backbuffer, stream)
+                                 : draw_frames(ctx, p, scene, mode, variant, stream);
+        if (r) return r;
+    }
+    if (int r = finish_kernels(ctx, stream, numFrames, outRayCount || outRaysPerFrame)) return r;
+    if (int r = stage_out(ctx, stream, image)) return r;
+    // host-buffer draws are synchronous like DrawTest
+    return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
+}
 
 int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
                    float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
@@ -889,7 +864,6 @@ int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     p.numRays = (uint32_t)n;
     cudaError_t e = launch_fast_rays(p, scene, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
@@ -904,7 +878,7 @@ int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, in
     if (!ctx->haveScene) return fail_msg(ctx, "tpt_draw_aovs: no scene (call tpt_set_scene first)");
     if (width <= 0 || height <= 0 || numFrames <= 0 || frameCount < 0 || numRows < 0 || rowStep <= 0 || row0 < 0)
         return fail_msg(ctx, "tpt_draw_aovs: bad arguments");
-    if (numFrames > 256) return fail_msg(ctx, "tpt_draw_aovs: numFrames > 256");
+    if (numFrames > kMaxFramesPerDraw) return fail_msg(ctx, "tpt_draw_aovs: numFrames > 256");
     if (!albedo4 && !normal4 && !ids) return fail_msg(ctx, "tpt_draw_aovs: albedo4, normal4 and ids are all null");
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufPix = (packed ? (size_t)numRows : (size_t)height) * width;
@@ -929,7 +903,6 @@ int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, in
     p.workCounter = next_work_counter(ctx);
     cudaError_t e = launch_fast_aovs(p, scene, false, (float*)bufs[0].dev, (float*)bufs[1].dev, (int*)bufs[2].dev, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !buffersOnDevice, outRayCount, nullptr);
@@ -967,7 +940,6 @@ int tpt_trace_aovs(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     p.numRays = (uint32_t)n;
     cudaError_t e = launch_fast_aovs(p, scene, true, (float*)bufs[1].dev, (float*)bufs[2].dev, (int*)bufs[3].dev, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    ctx->lastLaunches += 1;
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (int r = stage_out(ctx, stream, bufs)) return r;
     return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
@@ -1019,7 +991,6 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
     p.workCounter = next_work_counter(ctx);
     cudaError_t e = launch_fast_samples(p, scene, ctx->dBadPixel, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    ctx->lastLaunches += fast_samples_launches(p);
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (pixels) CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream), "D2H index check");
     if (int r = stage_out(ctx, stream, bufs)) return r;
@@ -1063,16 +1034,9 @@ int tpt_tonemap_rgba8(tpt_context* ctx, const float* image, int imageOnDevice, i
     if (transfer < 0 || transfer > 2) return fail_msg(ctx, "tpt_tonemap_rgba8: transfer 0..2");
     CK(cudaSetDevice(ctx->device), "cudaSetDevice");
     cudaStream_t stream = cudaStreamArg ? (cudaStream_t)cudaStreamArg : ctx->stream;
-    const size_t inBytes = (size_t)width * height * 16, outBytes = (size_t)width * height * 4;
-    const float* dIn = image;
-    if (!imageOnDevice)
-    {
-        auto& st = ctx->staging[kStageImage];
-        int r = ensure(ctx, &st.ptr, &st.cap, inBytes, "cudaMalloc image");
-        if (r) return r;
-        CK(cudaMemcpyAsync(st.ptr, image, inBytes, cudaMemcpyHostToDevice, stream), "H2D image");
-        dIn = (const float*)st.ptr;
-    }
+    const size_t outBytes = (size_t)width * height * 4;
+    CallerBuffer in[] = {{"image", (void*)image, imageOnDevice != 0, 16, (size_t)width * height * 16, kStageImage, kCopyUp}};
+    if (int r = stage_in(ctx, stream, in)) return r;
     unsigned char* dOut = dst;
     if (!dstOnDevice)
     {
@@ -1081,7 +1045,7 @@ int tpt_tonemap_rgba8(tpt_context* ctx, const float* image, int imageOnDevice, i
         dOut = (unsigned char*)ctx->dScratch;
     }
     const int n = width * height;
-    k_tonemap_rgba8<<<(n + 255) / 256, 256, 0, stream>>>((const float4*)dIn, width, height, (uchar4*)dOut, transfer, bgr ? 1 : 0, flipY ? 1 : 0);
+    k_tonemap_rgba8<<<(n + 255) / 256, 256, 0, stream>>>((const float4*)in[0].dev, width, height, (uchar4*)dOut, transfer, bgr ? 1 : 0, flipY ? 1 : 0);
     CK(cudaGetLastError(), "tonemap launch");
     if (!dstOnDevice)
     {

@@ -596,6 +596,7 @@ cudaError_t launch_refgpu_exact(const DrawParams& p, const SceneDev& sc, int num
 cudaError_t launch_resolve_exact(const DrawParams& p, cudaStream_t stream)
 {
     const long long n = (long long)p.numRows * p.width;
+    note_launch();
     k_resolve_exact<<<(int)((n + 255) / 256), 256, 0, stream>>>(p);
     return cudaGetLastError();
 }

@@ -31,7 +31,6 @@ namespace tpt {
 
 constexpr int kFastThreads = 256;
 constexpr int kTilePix = 1024;          // pixels per tile (12 KB of float3 accumulators)
-constexpr int kMaxFramesPerDraw = 256;  // per-frame blend weights live in shared memory
 
 __device__ __forceinline__ uint32_t fmix32(uint32_t h)
 {
@@ -1909,6 +1908,7 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
     if constexpr (SRC == kSrcRays) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
     else if constexpr (SRC == kSrcCamera)
     {
+        note_launch();
         k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
         e = cudaGetLastError();
     }
@@ -1991,8 +1991,6 @@ cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs
     return launch_queue<kSrcRays>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
 }
 
-int fast_samples_launches(const DrawParams& p) { return p.pixels ? 2 : 1; }
-
 cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
                                 cudaStream_t stream)
 {
@@ -2001,6 +1999,7 @@ cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigne
         cudaError_t e = cudaMemsetAsync(badPixel, 0xff, sizeof(unsigned long long), stream);
         if (e != cudaSuccess) return e;
         const long long blocks = ((long long)p.numRays + 255) / 256;
+        note_launch();
         k_check_pixels<<<(unsigned)(blocks < 4LL * numSMs ? blocks : 4LL * numSMs), 256, 0, stream>>>(
             p.pixels, p.numRays, (long long)p.width * p.height, badPixel);
         if ((e = cudaGetLastError()) != cudaSuccess) return e;
@@ -2149,8 +2148,30 @@ cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays,
 
 int fast_slab_pixels() { return kSlabPix; }
 
-int fast_kernel_launches(const DrawParams&, int variant) { return (variant == 3 || variant == 4 || variant == 9 || variant == 6 || variant == 7) ? 2 : 1; }
-bool fast_variant_writes_final_pixels(int variant) { return variant == 8; }
+FastVariantInfo fast_variant_info(int variant)
+{
+    const bool queue = variant == 3 || variant == 4 || variant == 9;
+    return {variant == 8, queue || (variant >= 5 && variant <= 7), queue};
+}
+
+// The block wavefront (variants 6/7) indexes its paths in 31 bits, over whole 128-pixel slabs (tail pixels are skipped),
+// and keeps 1 + the light index in 16 bits below kKindFree.
+static long long wave_paths(long long regionPix, long long S) { return ((regionPix + 127) / 128) * 128 * S; }
+static bool wave_fits(const SceneDev& sc, long long regionPix, long long S)
+{
+    return wave_paths(regionPix, S) <= 0x7fffffffLL && sc.nLights < kKindFree;
+}
+
+// The slab queue (3), except: a draw into mapped host memory runs the group queue (8), which stores its finished pixels
+// itself; and where the sweep dwarfs everything else (>= 1024 spheres) and the slab queue cannot run a packed-pair sweep
+// (pair array does not fit, or "fast_kform" < 2), the block wavefront that sorts its paths by material before Scatter()
+// is faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312).
+int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy)
+{
+    if (zeroCopy) return 8;
+    const long long S = (long long)spp * (numFrames < kMaxFramesPerDraw ? numFrames : kMaxFramesPerDraw);   // first launch
+    return sc.count >= 1024 && fast_queue_kform(sc) < 2 && wave_fits(sc, regionPix, S) ? 7 : 3;
+}
 
 cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, int numSMs, cudaStream_t stream,
                         unsigned int* bandDone, int numBands, unsigned int* bandExpected)
@@ -2205,13 +2226,13 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
     }
     if (variant == 6 || variant == 7)
     {
-        if (sc.nLights >= kKindFree) return cudaErrorInvalidValue;     // 1 + light index must stay below the free marker
+        if (!wave_fits(sc, regionPix, S)) return cudaErrorInvalidValue;
         auto kern = variant == 6 ? k_fast_wave<3> : k_fast_wave<4>;
         const FastSmem lay = fast_smem(sc.stagedBytes, 0, kWaveFields * kWaveSlots * 16);
-        const long long total = ((regionPix + 127) / 128) * 128 * S;      // whole 128-pixel slabs; tail pixels are skipped
-        if (total > 0x7fffffffLL) return cudaErrorInvalidValue;
+        const long long total = wave_paths(regionPix, S);
         e = persistent_grid(kern, kWaveThreads, lay.bytes, numSMs, (total + kWaveChunk - 1) / kWaveChunk, p, stream, grid);
         if (e != cudaSuccess) return e;
+        note_launch();
         k_prepare_image<<<(unsigned)((regionPix + 255) / 256), 256, 0, stream>>>(p, prev_weight(p.frame0, p.numFrames, p.flags));
         e = cudaGetLastError();
         if (e != cudaSuccess) return e;

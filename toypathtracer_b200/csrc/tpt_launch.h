@@ -29,10 +29,23 @@ cudaError_t launch_debug_libm(int fn, const float* dIn, float* dOut, long long n
 int fast_queue_kform(const SceneDev& sc);
 // nearest hit of n rays {o.xyz, d.xyz} with one sweep form of the fast kernels (0 reference, 1 expanded, 2 packed pairs, 3 conservative)
 cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, int* dId, float* dT, long long n, int numSMs, cudaStream_t stream);
+constexpr int kMaxFramesPerDraw = 256;  // frames per fast launch: per-frame blend weights live in shared memory
+
+// What a host-buffer draw needs to know about a fast variant.
+struct FastVariantInfo
+{
+    bool writesFinalPixels;   // the trace kernel stores finished pixels itself (no L2 reductions), also into mapped host memory
+    bool rowBands;            // a draw can be split into row bands, one launch per band
+    bool progressCounters;    // the trace kernel can publish per-band completion counters (launch_fast's bandDone)
+};
+FastVariantInfo fast_variant_info(int variant);
+// The variant a draw with "fast_variant" -1 runs over regionPix pixels of numFrames frames at spp; zeroCopy: the draw
+// stores straight into mapped host memory.
+int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy);
 // variant: see tpt_fast.cu
-// bandDone (optional, variant 3/4 only): device counters [numBands]; the kernel publishes finished paths per band of
-// macro-tiles, bandExpected[b] receives the final count of band b (host array) and kSlabPix*ceil(mtiles/numBands) pixels
-// form a band.
+// bandDone (optional, variants with progressCounters only): device counters [numBands]; the kernel publishes finished
+// paths per band of macro-tiles, bandExpected[b] receives the final count of band b (host array) and
+// kSlabPix*ceil(mtiles/numBands) pixels form a band.
 cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, int numSMs, cudaStream_t stream,
                         unsigned int* bandDone = nullptr, int numBands = 0, unsigned int* bandExpected = nullptr);
 // tpt_trace_rays: fast-mode radiance of p.numRays (>= 1) caller rays p.rays, p.spp samples each with streams
@@ -47,7 +60,6 @@ cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs
 // is traced. Runs the slab-queue instance variant 3 would run for the scene.
 cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
                                 cudaStream_t stream);
-int fast_samples_launches(const DrawParams& p);
 // tpt_draw_aovs (rays = false: the region of p, frames [p.frame0, p.frame0 + p.numFrames) at p.spp, blended over the outputs
 // with the weight of `prev`) and tpt_trace_aovs (rays = true: p.numRays >= 1 caller rays p.rays): first-hit albedo4,
 // normal4 and ids (each may be null) with the slab queue's sweep form, one ray counted per traced sample.
@@ -57,26 +69,28 @@ cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays,
 cudaError_t launch_refgpu_exact(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 cudaError_t launch_refgpu_fast(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 int fast_slab_pixels();
-int fast_kernel_launches(const DrawParams& p, int variant);
-bool fast_variant_writes_final_pixels(int variant);   // the trace kernel stores finished pixels itself (no L2 reductions)
 // weight of `prev` when frames [frame0, frame0 + numFrames) are blended into it: the product of their lerp_fac
 float prev_weight(int frame0, int numFrames, unsigned flags);
 
-// Diagnostic (tpt_debug_last_kernels): the trace kernels the calling thread's current library call launched, as the
-// function pointers its launch sites passed to note_kernel. start_kernels clears the record; a launch only stores a pointer.
-// n counts every launch; the first kCap are kept (tpt_debug_last_kernels reports the count, so a cut-off list shows).
+// The kernels the calling thread's current library call launched; start_kernels clears the record. `launches` counts every
+// launch (tpt_last_launch_count): trace kernels, and through note_launch the helpers that clear, blend or count.
+// Diagnostic (tpt_debug_last_kernels): the trace kernels, as the function pointers their launch sites passed to note_kernel
+// (a launch only stores a pointer); n counts them, the first kCap are kept (the count is reported, so a cut-off list shows).
 struct KernelRecord
 {
     static constexpr int kCap = 16;
     const void* fn[kCap];
     int n;
+    int launches;
 };
 extern thread_local KernelRecord t_lastKernels;
-inline void clear_kernels() { t_lastKernels.n = 0; }
+inline void clear_kernels() { t_lastKernels.n = 0; t_lastKernels.launches = 0; }
+inline void note_launch() { ++t_lastKernels.launches; }
 inline void note_kernel(const void* fn)
 {
     if (t_lastKernels.n < KernelRecord::kCap) t_lastKernels.fn[t_lastKernels.n] = fn;
     ++t_lastKernels.n;
+    note_launch();
 }
 
 // Launch set-up of a persistent kernel: allows `dyn` bytes of dynamic shared memory, sizes the grid to the CTAs that stay
