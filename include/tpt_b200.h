@@ -155,6 +155,32 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
 int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
                    float* out4, int outOnDevice, long long* outRayCount, void* cudaStream);
 
+/* Fast-mode irradiance E(p, n) at n caller-supplied surface points: the light arriving over the hemisphere around the normal
+ * n at p, what lightmaps and irradiance probes store, or the second pass of a renderer that takes its first hits from
+ * tpt_trace_aovs.
+ *   points6           n points of 6 floats {p.xyz, n.xyz}, the layout of rays6, loaded, validated and normalised exactly as
+ *                     tpt_trace_rays loads rays (same alignment). A point with a non-finite component, or a normal that does
+ *                     not normalise, is not traced: (0, 0, 0, 0), and it adds no rays.
+ *   ids               NULL, or n int32 sphere ids (host or device like points6, 4-byte aligned): point i lies on sphere
+ *                     ids[i], whose light is then not sampled from it (a light never samples itself). Any other value, -1
+ *                     included, has no effect; the id is only compared, never used as an index. A point on an emissive
+ *                     sphere must pass that sphere's id: otherwise it samples its own sphere as a light, which costs a
+ *                     shadow ray per sample and is not the estimator a draw's vertex on that sphere uses.
+ *   out4              n float4: out4[i] = (E.r, E.g, E.b, 0), pi x the mean over `spp` samples of the radiance a white
+ *                     Lambert surface at (p, n) reflects, with the estimator and scene options of tpt_trace_rays. Each
+ *                     sample is a Lambert vertex that a camera path has just reached at p, facing n: it draws its bounce
+ *                     direction, then samples the lights' cones with shadow rays, then continues along the bounce with the
+ *                     depth budget of a camera path after its first hit; the vertex adds no emission of its own. So for
+ *                     a camera ray whose first hit is a Lambert sphere `id` at (p, n), the expected tpt_trace_rays value
+ *                     is Le[id] + albedo[id] * E(p, n, id) / pi.
+ *   spp, frame        sample s of point i draws from the stream pixel_seed(i * spp + s, frame), as for tpt_trace_rays.
+ *   outRayCount       NULL or receives the number of rays traced: shadow rays, the bounce and the path's later rays. The
+ *                     point itself is not a ray.
+ * Buffers, streams, limits, refusals, ordering and accounting (tpt_read_ray_count, tpt_last_kernel_ms,
+ * tpt_last_launch_count, tpt_debug_last_kernels) are those of tpt_trace_rays; n == 0 launches nothing. */
+int tpt_trace_irradiance(tpt_context* ctx, const float* points6, const int* ids, int pointsOnDevice, long long n,
+                         int spp, int frame, float* out4, int outOnDevice, long long* outRayCount, void* cudaStream);
+
 /* First-hit AOVs (arbitrary output values) of the fast mode: the denoiser guides, depth, mask and id buffers that go next
  * to an image. One nearest-hit query per sample, no shading. Outputs, per pixel or per ray; each pointer may be NULL (not
  * written), but not all three:
@@ -264,8 +290,8 @@ int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long l
  * of at most 64 padded spheres only), tMin/tMax as Trace uses them. outId -1 = miss. */
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays6, int* outId, float* outT, long long n);
 /* Diagnostic: the mangled names of the trace kernels (path tracing and first-hit AOV kernels, not the helpers that clear,
- * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_draw_samples, tpt_draw_aovs or
- * tpt_trace_aovs launched, in launch order, separated by '\n' and NUL-terminated in buf[cap].
+ * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples,
+ * tpt_draw_aovs or tpt_trace_aovs launched, in launch order, separated by '\n' and NUL-terminated in buf[cap].
  *   - The record is per host thread, not per context: a call on another thread, or on another context from this
  *     thread, replaces it.
  *   - A call resets it when it starts launching (an empty call too). A call refused before that leaves the previous

@@ -1,10 +1,12 @@
-"""Throughput of Context.trace_rays against the fast draw of the same image, alternating in one process: the 46-sphere
-scene at 1280x720, camera_rays with one ray per pixel at spp 4 (the draw: one 4-spp frame, flags 0) into device buffers,
+"""Throughput of Context.trace_rays and Context.trace_irradiance against the fast draw of the same image, alternating in one
+process: the 46-sphere scene at 1280x720, camera_rays with one ray per pixel at spp 4 (the draw: one 4-spp frame, flags 0;
+the irradiance arm: E at the rays' primary hits, found once with trace_aovs, with their sphere ids) into device buffers,
 CUDA events around each call on the launching stream, L2 flushed (256 MiB fill) between steps outside the events, as
-tools/bench_light_sampling.py times. Rounds alternate the two so that clock and neighbour drift hit both alike. Prints one
+tools/bench_light_sampling.py times. Rounds alternate the calls so that clock and neighbour drift hit both alike. Prints one
 JSON line per round and a summary with the card name and power limit read in the same run.
     python tools/bench_trace_rays.py [--steps 200] [--rounds 5] [--warmup 10]
-Mray/s counts every traced ray (path and shadow rays), as bench.py does."""
+Mray/s counts every traced ray (path and shadow rays), as bench.py does; an irradiance point is not a ray, so that arm
+counts one ray fewer per sample than a camera ray that reaches the same point."""
 import argparse
 import json
 import os
@@ -43,9 +45,16 @@ def main():
     image = torch.zeros((H, W, 4), dtype=torch.float32, device=dev)
     rays = torch.from_numpy(tpt.camera_rays(cam, W, H, per_pixel=1, seed=0)).to(dev)
     out = torch.empty((W * H, 4), dtype=torch.float32, device=dev)
+    (_, nrm, ids), _ = ctx.trace_aovs(rays)
+    hit = ids >= 0
+    points = torch.cat([rays[hit, :3] + nrm[hit, 3:] * rays[hit, 3:], nrm[hit, :3]], 1).contiguous()
+    point_ids = ids[hit].contiguous()
+    eout = torch.empty((len(points), 4), dtype=torch.float32, device=dev)
     calls = {
         "draw": lambda f: ctx.draw(f, 1, W, H, image, flags=0, mode=tpt.MODE_FAST, stream=stream.cuda_stream, want_rays=False),
         "trace_rays": lambda f: ctx.trace_rays(rays, spp=SPP, frame=f, out=out, stream=stream.cuda_stream, want_rays=False),
+        "irradiance": lambda f: ctx.trace_irradiance(points, point_ids, spp=SPP, frame=f, out=eout, stream=stream.cuda_stream,
+                                                     want_rays=False),
     }
     for f in range(args.warmup):
         for call in calls.values():
@@ -68,7 +77,8 @@ def main():
             print(json.dumps({"round": r, "call": name, "Mray_per_s": rates[name][-1], "ms_per_step": ms / args.steps,
                               "rays_per_step": n / args.steps, "steps": args.steps}), flush=True)
     print(json.dumps({"card": card(), "median_Mray_per_s": {k: statistics.median(v) for k, v in rates.items()},
-                      "trace_rays_over_draw": statistics.median(rates["trace_rays"]) / statistics.median(rates["draw"])}),
+                      "trace_rays_over_draw": statistics.median(rates["trace_rays"]) / statistics.median(rates["draw"]),
+                      "irradiance_points": len(points)}),
           flush=True)
     ctx.close()
 

@@ -77,6 +77,8 @@ def _load_lib():
     L.tpt_debug_hit.argtypes = [vp, ci, vp, vp, vp, cll]; L.tpt_debug_hit.restype = ci
     L.tpt_debug_last_kernels.argtypes = [vp, ctypes.c_char_p, ci]; L.tpt_debug_last_kernels.restype = ci
     L.tpt_trace_rays.argtypes = [vp, vp, ci, cll, ci, ci, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_rays.restype = ci
+    L.tpt_trace_irradiance.argtypes = [vp, vp, vp, ci, cll, ci, ci, vp, ci, ctypes.POINTER(cll), vp]
+    L.tpt_trace_irradiance.restype = ci
     L.tpt_draw_aovs.argtypes = [vp, ci, ci, ci, ci, ci, ci, ci, ci, vp, vp, vp, ci, cu, ctypes.POINTER(cll), vp]
     L.tpt_draw_aovs.restype = ci
     L.tpt_trace_aovs.argtypes = [vp, vp, ci, cll, vp, vp, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_aovs.restype = ci
@@ -383,6 +385,25 @@ class Context:
         (po,), oon, _keep_out = _buffer_ptrs("trace_rays", [("out", out, "float32", 4)], n)
         total = self._call("tpt_trace_rays", want_rays, stream, ctypes.c_void_p(raddr), 1 if ron else 0, n, int(spp),
                            int(frame), po, 1 if oon else 0)
+        return (out, total) if want_rays else out
+
+    def trace_irradiance(self, points, ids=None, spp: int = 4, frame: int = 0, out=None, stream: int = 0,
+                         want_rays: bool = True, n=None):
+        """tpt_trace_irradiance: fast-mode irradiance E(p, n) (pi x the mean of `spp` samples, streams keyed by `frame`)
+        at caller surface points {p.xyz, n.xyz}, in an (N, 6) float32 buffer of the kinds trace_rays takes for its rays.
+        `ids` (N,) int32 of the same kind, or None: the sphere each point lies on, whose light is then not sampled from
+        it; a point on an emissive sphere must pass that sphere's id. For a camera ray whose first hit is a Lambert sphere
+        at (p, n), trace_rays estimates Le + albedo * E / pi. `out`, the allocation of a missing `out`, `stream` and the
+        return value are as for trace_rays."""
+        n = _entries("trace_irradiance", "points", points, n, (6,))
+        if ids is not None:
+            _entries("trace_irradiance", "ids", ids, n, ())
+        (pp, pi), pon, _keep = _buffer_ptrs("trace_irradiance", [("points", points, "float32", 6), ("ids", ids, "int32", 1)], n)
+        if out is None:
+            (out,) = _alloc_like(points, self.device, [((n, 4), "float32")])
+        (po,), oon, _keep_out = _buffer_ptrs("trace_irradiance", [("out", out, "float32", 4)], n)
+        total = self._call("tpt_trace_irradiance", want_rays, stream, pp, pi, 1 if pon else 0, n, int(spp), int(frame), po,
+                           1 if oon else 0)
         return (out, total) if want_rays else out
 
     def draw_aovs(self, frame: int, num_frames: int, width: int, height: int, albedo=None, normal=None, ids=None,

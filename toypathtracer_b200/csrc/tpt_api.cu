@@ -519,8 +519,8 @@ struct RowRegion { int width, row0, numRows, rowStep, packed; };
 
 enum { kCopyUp = 1, kCopyDown = 2 };
 
-// One caller buffer of tpt_draw, tpt_trace_rays, tpt_trace_aovs, tpt_draw_aovs, tpt_draw_samples or tpt_tonemap_rgba8. A
-// null `ptr` is a buffer the caller left out: it is neither checked nor staged.
+// One caller buffer of tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_trace_aovs, tpt_draw_aovs, tpt_draw_samples or
+// tpt_tonemap_rgba8. A null `ptr` is a buffer the caller left out: it is neither checked nor staged.
 struct CallerBuffer
 {
     const char* name;                   // as the error texts name it
@@ -834,19 +834,24 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
 }
 
-int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
-                   float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
+// tpt_trace_rays (points = false: in6 holds rays {o, d}) and tpt_trace_irradiance (points = true: in6 holds surface points
+// {p, n}, ids their sphere ids or null): the same checks, staging and launch of the slab queue on caller entries.
+static int trace_caller_entries(tpt_context* ctx, const char* fn, bool points, const float* in6, const int* ids, int inOnDevice,
+                                long long n, int spp, int frame, float* out4, int outOnDevice, long long* outRayCount,
+                                void* cudaStreamArg)
 {
+    const char* inName = points ? "points6" : "rays6";
     if (!ctx) return (int)cudaErrorInvalidValue;
-    if (!ctx->haveScene) return fail_msg(ctx, "tpt_trace_rays: no scene (call tpt_set_scene first)");
-    if (!rays6 || !out4) return fail_msg(ctx, "tpt_trace_rays: null rays6 or out4");
-    if (n < 0) return fail_msg(ctx, "tpt_trace_rays: n < 0");
-    if (spp < 1) return fail_msg(ctx, "tpt_trace_rays: spp < 1");
-    // the sample stream of (ray i, sample s) is i * spp + s in 32 bits, and so is the ray index
-    if (n > (1LL << 32) / spp || n > 0xffffffffLL) return fail_msg(ctx, "tpt_trace_rays: n * spp > 2^32 (32-bit sample streams)");
-    CallerBuffer bufs[] = {{"rays6", (void*)rays6, raysOnDevice != 0, 4, (size_t)n * 24, kStageRays, kCopyUp},
+    if (!ctx->haveScene) return fail_msgf(ctx, "%s: no scene (call tpt_set_scene first)", fn);
+    if (!in6 || !out4) return fail_msgf(ctx, "%s: null %s or out4", fn, inName);
+    if (n < 0) return fail_msgf(ctx, "%s: n < 0", fn);
+    if (spp < 1) return fail_msgf(ctx, "%s: spp < 1", fn);
+    // the sample stream of (entry i, sample s) is i * spp + s in 32 bits, and so is the entry index
+    if (n > (1LL << 32) / spp || n > 0xffffffffLL) return fail_msgf(ctx, "%s: n * spp > 2^32 (32-bit sample streams)", fn);
+    CallerBuffer bufs[] = {{inName, (void*)in6, inOnDevice != 0, 4, (size_t)n * 24, kStageRays, kCopyUp},
+                           {"ids", (void*)ids, inOnDevice != 0, 4, (size_t)n * 4, kStageIds, kCopyUp},
                            {"out4", out4, outOnDevice != 0, 16, (size_t)n * 16, kStageImage, kCopyDown}};
-    if (int r = check_buffers(ctx, "tpt_trace_rays", bufs)) return r;
+    if (int r = check_buffers(ctx, fn, bufs)) return r;
     if (n == 0) return empty_call(ctx, outRayCount);
     cudaStream_t stream;
     SceneDev scene;
@@ -857,16 +862,32 @@ int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long 
     memset(&p, 0, sizeof(p));
     p.spp = spp;
     p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
-    p.image = (float*)bufs[1].dev;
+    p.image = (float*)bufs[2].dev;
     p.rayCounter = ctx->dRayCounters;
     p.workCounter = next_work_counter(ctx);
     p.rays = (const float*)bufs[0].dev;
     p.numRays = (uint32_t)n;
+    p.pointStart = points ? 1 : 0;
+    p.pointIds = (const int*)bufs[1].dev;
     cudaError_t e = launch_fast_rays(p, scene, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
     if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
     if (int r = stage_out(ctx, stream, bufs)) return r;
-    return finish_call(ctx, stream, 1, !raysOnDevice || !outOnDevice, outRayCount, nullptr);
+    return finish_call(ctx, stream, 1, !inOnDevice || !outOnDevice, outRayCount, nullptr);
+}
+
+int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
+                   float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
+{
+    return trace_caller_entries(ctx, "tpt_trace_rays", false, rays6, nullptr, raysOnDevice, n, spp, frame, out4, outOnDevice,
+                                outRayCount, cudaStreamArg);
+}
+
+int tpt_trace_irradiance(tpt_context* ctx, const float* points6, const int* ids, int pointsOnDevice, long long n,
+                         int spp, int frame, float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
+{
+    return trace_caller_entries(ctx, "tpt_trace_irradiance", true, points6, ids, pointsOnDevice, n, spp, frame, out4,
+                                outOnDevice, outRayCount, cudaStreamArg);
 }
 
 int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, int height,

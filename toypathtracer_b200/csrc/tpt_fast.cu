@@ -771,6 +771,28 @@ __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 n
     return m * omega * (1.0f / TPT_PI);
 }
 
+// The rest of a Lambert vertex after its shadow ray towards light lightFrom - 1 (or, lightFrom = 0, after the vertex's
+// own shading): the next light the vertex samples, its cone and shadow ray, or, when none is left, the bounce along
+// st.nextDir with throughput st.thrAlb. Without light sampling (kLsOff) there are no lights to sample: the bounce.
+template <int LS>
+__device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom)
+{
+    const int j = LS == kLsOff ? sc.nLights : next_light(sc, lightFrom, st.mid);
+    if (j < sc.nLights)
+    {
+        st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
+        st.kind = 1 + j;
+    }
+    else
+    {
+        st.d = st.nextDir;
+        st.thr = st.thrAlb;
+        st.kind = 0;
+        st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
+        ++st.depth;
+    }
+}
+
 // Metal bounce direction (Test.cpp:137-150); the path goes on when dot(result, normal) > 0. With roughness == 0 the
 // unit-sphere sample has zero weight, so the fast mode skips drawing it (the exact mode must draw it: it advances the
 // shared RNG stream).
@@ -865,24 +887,22 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             wantLight = true; lightFrom = j + 1;
         }
     }
-    if (LS != kLsOff && wantLight)
-    {
-        const int j = next_light(sc, lightFrom, st.mid);
-        if (j < sc.nLights)
-        {
-            st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
-            st.kind = 1 + j;
-        }
-        else
-        {
-            st.d = st.nextDir;
-            st.thr = st.thrAlb;
-            st.kind = 0;
-            st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
-            ++st.depth;
-        }
-    }
+    if (LS != kLsOff && wantLight) lambert_next<LS>(sc, st, lightFrom);
     return finished;
+}
+
+// tpt_trace_irradiance: the lane's fresh path (begin_path from a point entry {p, n}: st.o = p, st.d = n) becomes a white
+// Lambert vertex at p whose facing normal is n, as if a camera ray had just hit it: the bounce direction drawn first, then
+// lambert_next picks the first light (or the bounce). No emission of its own (doMaterialE is not looked at before the
+// next hit); depth 0, so the path keeps a camera path's budget. `mid`: the sphere the point lies on, or -1.
+template <int LS>
+__device__ __forceinline__ void begin_vertex(const SceneView& sc, QPath& st, int mid)
+{
+    st.nl = st.d;
+    st.nextDir = M<false>::normalize(st.d + RandomUnitVector<false>(st.rng));
+    st.thrAlb = v3(1, 1, 1);
+    st.mid = mid;
+    lambert_next<LS>(sc, st, 0);
 }
 
 // ---- variant 0 ------------------------------------------------------------------------------------------------
@@ -1032,7 +1052,8 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // Dynamic shared memory (FastSmem): [staged blob][pair array (KFORM 2/3)][per-warp camera-ray buffers, 2 KB per warp at raysOffset].
 // The body is shared by k_fast_queue (light sampling) and k_fast_queue_nolight (DO_LIGHT_SAMPLING 0) below.
 // SRC: the ray source. kSrcCamera: camera rays of the image region. kSrcRays (k_fast_rays): the caller's p.numRays rays
-// (load_slab_rays), a slab being 64 consecutive rays x one sample index, finished paths adding col / spp to p.image[ray].
+// (load_slab_rays), a slab being 64 consecutive rays x one sample index, finished paths adding col / spp to p.image[ray];
+// with p.pointStart (tpt_trace_irradiance) the entries are surface points, each sample starting as a Lambert vertex.
 // kSrcPixels (k_fast_samples): the draw's camera rays for the p.numRays entries of a pixel list (generate_list_rays), a
 // slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
 // MOMENTS, (col^2, 0) to p.sq4[entry].
@@ -1083,6 +1104,15 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     uint32_t slabBand = 0;
     int curBand = -1;
     uint32_t doneCnt = 0, myBand = 0;
+    // tpt_trace_irradiance (p.pointStart, launch-uniform): a lane that takes a point entry starts it as a Lambert vertex
+    // (begin_vertex) inside the deal in the 128-thread instances, and right after the deal in the 768-thread ones. Both
+    // places were measured (H100 SXM, 700 W; trace_rays, whose paths never take the branch): inside the deal the
+    // 768-thread form-3 instance sweeps the 4096-sphere stress scene 4.5 % slower than without the feature, after the deal
+    // it runs as before (+0.5 %), while for the 128-thread instances the deal is the place that costs nothing.
+    constexpr bool kStartInDeal = THREADS != TPT_BIG_THREADS;
+    const bool pointStart = SRC == kSrcRays && p.pointStart;
+    const int* pointIds = p.pointIds;
+    bool fresh = false;       // the lane has just been dealt an entry (the 768-thread instances' start after the deal)
 
     QPath st;
     st.active = false;
@@ -1116,8 +1146,24 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             __syncwarp();
             return kDealRefilled;
         };
-        deal_paths(p, st, sRays[threadIdx.x >> 5], slabCur, slabEnd, exhausted, lane, refill,
-                   [&](uint32_t tag) { st.pixOff = tag; st.weight = slabW; myBand = slabBand; });
+        deal_paths(p, st, sRays[threadIdx.x >> 5], slabCur, slabEnd, exhausted, lane, refill, [&](uint32_t tag) {
+            st.pixOff = tag; st.weight = slabW; myBand = slabBand;
+            // tpt_trace_irradiance: the entry is a point {p, n}; E = pi x the white Lambert vertex's radiance
+            if constexpr (SRC == kSrcRays && kStartInDeal)
+                if (pointStart)
+                {
+                    begin_vertex<LS>(sc, st, pointIds ? __ldg(pointIds + tag) : -1);
+                    st.weight *= TPT_PI;
+                }
+            if constexpr (SRC == kSrcRays && !kStartInDeal) fresh = true;
+        });
+        if constexpr (SRC == kSrcRays && !kStartInDeal)
+            if (pointStart && fresh)
+            {
+                begin_vertex<LS>(sc, st, pointIds ? __ldg(pointIds + st.pixOff) : -1);
+                st.weight *= TPT_PI;
+                fresh = false;
+            }
         if (!__any_sync(0xffffffffu, st.active)) break;
 #if TPT_TRACE_WARPS
         if (!trReady) trReady = gtimer();

@@ -50,7 +50,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
                         unsigned int* bandDone = nullptr, int numBands = 0, unsigned int* bandExpected = nullptr);
 // tpt_trace_rays: fast-mode radiance of p.numRays (>= 1) caller rays p.rays, p.spp samples each with streams
 // pixel_seed(ray * spp + sample, p.frame0), mean written to the float4 p.image[ray] (zeroed first); p.numFrames = 1, p.flags = 0.
-// Runs the slab-queue instance variant 3 would run for the scene.
+// Runs the slab-queue instance variant 3 would run for the scene. tpt_trace_irradiance: the same launch with p.pointStart
+// set, p.rays holding surface points {p, n} and p.pointIds their sphere ids (or null); the mean is then scaled by pi.
 cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
 // tpt_draw_samples: p.spp samples of each of the p.numRays (>= 1) entries of the pixel list p.pixels (null: pixels 0 ..
 // numRays - 1 of the width x height image), sample s of pixel i being the fast draw's camera ray with stream

@@ -102,6 +102,11 @@ struct DrawParams
     const int* pixels;
     float* sq4;
     const unsigned long long* badPixel;
+    // tpt_trace_irradiance: the numRays `rays` are surface points {p.xyz, n.xyz}, and each sample starts as a white Lambert
+    // vertex at (p, n) instead of a ray from p (launch-uniform). pointIds: null, or numRays sphere ids, entry i the sphere
+    // point i lies on (that sphere's light is not sampled from it).
+    int pointStart;
+    const int* pointIds;
 };
 
 } // namespace tpt
