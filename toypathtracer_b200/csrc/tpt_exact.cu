@@ -531,9 +531,7 @@ static cudaError_t launch_chains(Kernel kern, long long grid, int block, size_t 
 {
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
     if (e != cudaSuccess) return e;
-    note_kernel((const void*)kern);
-    kern<<<(unsigned)grid, block, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
-    return cudaGetLastError();
+    return launch_trace(kern, (unsigned)grid, block, dyn, stream, p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
 }
 
 static cudaError_t launch_exact_cluster(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)

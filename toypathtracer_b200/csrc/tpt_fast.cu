@@ -1981,10 +1981,8 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
         cudaMemsetAsync(dTrace, 0, traceWords * 8, stream);
     }
 #endif
-    note_kernel((const void*)kern);
-    kern<<<(unsigned)grid, threads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                          (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers,
-                                                          sc.pairs);
+    e = launch_trace(kern, (unsigned)grid, threads, lay.bytes, stream, p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                     (uint32_t)slabs, S, mpb ? bandDone : nullptr, mpb ? mpb : 1u, lay.buffers, sc.pairs);
 #if TPT_TRACE_WARPS
     if (const char* tf = getenv("TPT_TRACE_FILE"))
     {
@@ -1994,7 +1992,7 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
         if (FILE* f = fopen(tf, "wb")) { fwrite(h.data(), 8, traceWords, f); fclose(f); }     // the last traced launch wins
     }
 #endif
-    return cudaGetLastError();
+    return e;
 }
 
 // Diagnostic (tpt_debug_hit): the nearest-hit query of one sweep form on caller-supplied rays, staged exactly like
@@ -2186,10 +2184,8 @@ cudaError_t launch_fast_aovs(const DrawParams& p, const SceneDev& sc, bool rays,
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, kAovThreads, dyn, numSMs, (chunks + kAovThreads / 32 - 1) / (kAovThreads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
-    note_kernel((const void*)kern);
-    kern<<<(unsigned)grid, kAovThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, (uint32_t)chunks,
-                                                       rays ? 0.0f : prev_weight(p.frame0, p.numFrames, p.flags), albedo4, normal4, ids);
-    return cudaGetLastError();
+    return launch_trace(kern, (unsigned)grid, kAovThreads, dyn, stream, p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                        (uint32_t)chunks, rays ? 0.0f : prev_weight(p.frame0, p.numFrames, p.flags), albedo4, normal4, ids);
 }
 
 int fast_slab_pixels() { return kSlabPix; }
@@ -2232,9 +2228,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         e = cudaFuncSetAttribute(k_fast_mega, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sc.stagedBytes);
         if (e != cudaSuccess) return e;
         const int tilesX = (p.width + 15) / 16, tilesY = (p.numRows + 15) / 16;
-        note_kernel((const void*)k_fast_mega);
-        k_fast_mega<<<tilesX * tilesY, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes);
-        return cudaGetLastError();
+        return launch_trace(k_fast_mega, tilesX * tilesY, kFastThreads, sc.stagedBytes, stream, p, sc.blob, sc.layout, sc.count,
+                            sc.nLights, sc.stagedBytes);
     }
     if (variant == 1 || variant == 2)
     {
@@ -2242,9 +2237,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         const int numTiles = (int)((regionPix + kTilePix - 1) / kTilePix);
         e = persistent_grid(kern, kFastThreads, sc.stagedBytes, numSMs, numTiles, p, stream, grid);
         if (e != cudaSuccess) return e;
-        note_kernel((const void*)kern);
-        kern<<<(unsigned)grid, kFastThreads, sc.stagedBytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, numTiles);
-        return cudaGetLastError();
+        return launch_trace(kern, (unsigned)grid, kFastThreads, sc.stagedBytes, stream, p, sc.blob, sc.layout, sc.count, sc.nLights,
+                            sc.stagedBytes, numTiles);
     }
     if (variant == 3 || variant == 4 || variant == 9)
     {
@@ -2260,15 +2254,13 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
             return alls ? light_twin(sc, k_fast_group<TPT_QUEUE_MINB, k, true>, k_fast_group_nolight<TPT_QUEUE_MINB, k, true>)
                         : light_twin(sc, k_fast_group<TPT_QUEUE_MINB, k, false>, k_fast_group_nolight<TPT_QUEUE_MINB, k, false>);
         });
-        const size_t dyn = fast_smem(sc.stagedBytes, kform == 2 ? simd_count(sc) * 16 : 0).bytes;
+        const size_t dyn = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, kform)).bytes;
         const long long groups = (regionPix + kGroupPix - 1) / kGroupPix;
         if (groups > 0x7fffffffLL) return cudaErrorInvalidValue;
         e = persistent_grid(kern, kQueueThreads, dyn, numSMs, (groups + kQueueThreads / 32 - 1) / (kQueueThreads / 32), p, stream, grid);
         if (e != cudaSuccess) return e;
-        note_kernel((const void*)kern);
-        kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                               (uint32_t)groups, S, prev_weight(p.frame0, p.numFrames, p.flags));
-        return cudaGetLastError();
+        return launch_trace(kern, (unsigned)grid, kQueueThreads, dyn, stream, p, sc.blob, sc.layout, sc.count, sc.nLights,
+                            sc.stagedBytes, (uint32_t)groups, S, prev_weight(p.frame0, p.numFrames, p.flags));
     }
     if (variant == 6 || variant == 7)
     {
@@ -2286,15 +2278,14 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         wa.S = S;
         wa.totalPaths = (uint32_t)total;
         wa.divS = make_fastdiv(wa.S); wa.divW = make_fastdiv((uint32_t)p.width); wa.divSpp = make_fastdiv((uint32_t)p.spp);
-        note_kernel((const void*)kern);
-        kern<<<(unsigned)grid, kWaveThreads, lay.bytes, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, lay.buffers, wa);
-        return cudaGetLastError();
+        return launch_trace(kern, (unsigned)grid, kWaveThreads, lay.bytes, stream, p, sc.blob, sc.layout, sc.count, sc.nLights,
+                            sc.stagedBytes, lay.buffers, wa);
     }
     if (variant == 5)
     {
         const int kform = fast_group_kform(sc);
         auto kern = for_kform<2>(kform, [](auto K) { return k_fast_tileq<6, decltype(K)::value>; });
-        const size_t dyn = fast_smem(sc.stagedBytes, kform == 2 ? simd_count(sc) * 16 : 0).bytes;
+        const size_t dyn = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, kform)).bytes;
         // the tile size follows from the resident grid, which is clamped to the tiles afterwards
         e = persistent_grid(kern, kQueueThreads, dyn, numSMs, LLONG_MAX, p, stream, grid);
         if (e != cudaSuccess) return e;
@@ -2306,10 +2297,8 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
         while (tileQPix > (uint32_t)kSlabPix && (regionPix + tileQPix - 1) / tileQPix < 8 * grid && tileQPix * S > 2048) tileQPix -= kSlabPix;
         const long long tiles = (regionPix + tileQPix - 1) / tileQPix;
         if (grid > tiles) grid = tiles;
-        note_kernel((const void*)kern);
-        kern<<<(unsigned)grid, kQueueThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
-                                                               (uint32_t)tiles, S, prev_weight(p.frame0, p.numFrames, p.flags), tileQPix);
-        return cudaGetLastError();
+        return launch_trace(kern, (unsigned)grid, kQueueThreads, dyn, stream, p, sc.blob, sc.layout, sc.count, sc.nLights,
+                            sc.stagedBytes, (uint32_t)tiles, S, prev_weight(p.frame0, p.numFrames, p.flags), tileQPix);
     }
     return cudaErrorInvalidValue;
 }

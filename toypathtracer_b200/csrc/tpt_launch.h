@@ -75,7 +75,7 @@ float prev_weight(int frame0, int numFrames, unsigned flags);
 
 // The kernels the calling thread's current library call launched; start_kernels clears the record. `launches` counts every
 // launch (tpt_last_launch_count): trace kernels, and through note_launch the helpers that clear, blend or count.
-// Diagnostic (tpt_debug_last_kernels): the trace kernels, as the function pointers their launch sites passed to note_kernel
+// Diagnostic (tpt_debug_last_kernels): the trace kernels, as the function pointers launch_trace passed to note_kernel
 // (a launch only stores a pointer); n counts them, the first kCap are kept (the count is reported, so a cut-off list shows).
 struct KernelRecord
 {
@@ -92,6 +92,15 @@ inline void note_kernel(const void* fn)
     if (t_lastKernels.n < KernelRecord::kCap) t_lastKernels.fn[t_lastKernels.n] = fn;
     ++t_lastKernels.n;
     note_launch();
+}
+// Records a trace kernel (note_kernel) and launches it, so that the record and the launch cannot drift apart. The
+// diagnostic kernels (k_debug_hit, k_debug_libm) are launched directly and stay out of the record.
+template <class Kernel, class... Args>
+cudaError_t launch_trace(Kernel kern, dim3 grid, dim3 block, size_t dyn, cudaStream_t stream, const Args&... args)
+{
+    note_kernel((const void*)kern);
+    kern<<<grid, block, dyn, stream>>>(args...);
+    return cudaGetLastError();
 }
 
 // Launch set-up of a persistent kernel: allows `dyn` bytes of dynamic shared memory, sizes the grid to the CTAs that stay

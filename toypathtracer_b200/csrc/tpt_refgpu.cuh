@@ -352,9 +352,8 @@ static cudaError_t launch_refgpu_t(const DrawParams& p, const SceneDev& sc, int 
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, kRgThreads, dyn, numSMs, (slabs + kRgThreads / 32 - 1) / (kRgThreads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
-    note_kernel((const void*)kern);
-    kern<<<(unsigned)grid, kRgThreads, dyn, stream>>>(p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, (uint32_t)slabs);
-    return cudaGetLastError();
+    return launch_trace(kern, (unsigned)grid, kRgThreads, dyn, stream, p, sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes,
+                        (uint32_t)slabs);
 }
 
 } // namespace tpt
