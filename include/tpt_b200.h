@@ -81,9 +81,11 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * copy stream waits on them with cuStreamWaitValue32, "progress_bands" bands, default 4; 0 falls back to host_bands),
  * "fast_kform" (fast kernels' sphere sweep: 0 reference form, 1 expanded form, 2 (default) expanded form on a pair-interleaved
  * sphere array, one 128-bit shared load per coordinate of two spheres — the slab queue of a scene of at most 64 padded
- * spheres takes that array in its kernel parameters instead, so its first pass reads the spheres as constant operands;
- * 3 as 2 but with the array always in shared memory, for A/B comparisons; 1, 2 and 3 only when the scene passes the gate in
- * tpt_set_scene — a scene that fails it gets, with 2 or 3, the packed sweep made conservative by a folded-in error bound
+ * spheres takes that array in its kernel parameters instead, so its first pass reads the spheres as constant operands,
+ * and where the scene passes the half-precision gate its first pass tests two spheres per packed half instruction with a
+ * folded-in error bound (same hits and distances); 4 as 2 but without that half-precision first pass, for A/B comparisons;
+ * 3 as 2 but with the array always in shared memory, for A/B comparisons; 1 to 4 only when the scene passes the gate in
+ * tpt_set_scene — a scene that fails it gets, with 2 to 4, the packed sweep made conservative by a folded-in error bound
  * plus reference-form hit decisions, and the reference form otherwise; per context), "fast_alpha_zero" (default 0; 1: fast-mode draws whose `prev` has zero weight write
  * alpha = 0 instead of keeping the buffer's alpha — saves the read over NVLink when the buffer is a peer GPU's),
  * "exact_lookahead" (default 0; L > 1: an exact-mode draw of ONE frame that misses the cache traces frames [f, f+L) in a
@@ -287,7 +289,7 @@ int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long l
 /* Diagnostic used by the parity tests: nearest hit (HitWorld, Test.cpp:85-106) of n host rays {o.xyz, d.xyz} in the
  * current scene with one sweep form of the fast kernels (kform 0 reference form, 1 expanded, 2 expanded on packed pairs,
  * 3 conservative packed pass + reference-form decisions, 4 expanded on packed pairs read from the kernel parameters: scenes
- * of at most 64 padded spheres only), tMin/tMax as Trace uses them. outId -1 = miss. */
+ * of at most 64 padded spheres only, 5 as 4 with the half-precision first pass: scenes that pass its gate only), tMin/tMax as Trace uses them. outId -1 = miss. */
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays6, int* outId, float* outT, long long n);
 /* Diagnostic: the mangled names of the trace kernels (path tracing and first-hit AOV kernels, not the helpers that clear,
  * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples,

@@ -54,7 +54,8 @@ struct tpt_context
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
     int fastKForm = 2;        // 0: reference-form sweep, 1: expanded form, 2: expanded form on the pair array (slab queue: in the
                               // kernel parameter for scenes of <= 64 padded spheres), 3: as 2 with the pair array always in
-                              // shared memory (A/B); gated per scene by kformOk
+                              // shared memory (A/B), 4: as 2 without the half-precision pass 1 of form 5 (A/B); gated
+                              // per scene by kformOk
     int fastAlphaZero = 0;
     int sceneUploadAlways = 0;   // 1: tpt_set_scene copies the blob even when its bytes are the resident scene's (benchmarks: a real H2D per step)
     long long lastSceneUploadBytes = 0;
@@ -297,6 +298,7 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
                     ctx->sceneFlags);
     ParamPairs pairs;
     build_param_pairs(blob, L, count, pairs);
+    const bool halfOk = build_half_pairs(blob, L, count, pairs);
     // geometry + light table must fit in shared memory next to the kernels' static shared arrays
     const uint32_t kMaxStage = 200 * 1024;
     if (L.geomBytes > kMaxStage) return fail_msg(ctx, "tpt_set_scene: too many spheres for shared-memory staging");
@@ -337,6 +339,7 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
     ctx->scene.layout = L;
     ctx->scene.count = count;
     ctx->scene.pairs = pairs;
+    ctx->scene.halfOk = halfOk;
     ctx->scene.nLights = sampled_lights(L.flags, nLights);   // 0 with light sampling off: every light loop is empty
     // small scenes: stage everything (spheres + materials); large ones: geometry only, materials from L2
     ctx->scene.stagedBytes = L.totalBytes <= 64 * 1024 ? L.totalBytes : L.geomBytes;
@@ -381,7 +384,7 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     if (!strcmp(key, "exact_lanes")) { if (value != 0 && value != 1 && value != 2 && value != 8 && value != 9 && value != 32 && (value < 64 || value > 71)) return fail_msg(ctx, "exact_lanes: 0,1,2,8,9,32,64..71"); ctx->exactLanes = value; return 0; }
     if (!strcmp(key, "exact_lookahead")) { if (value < -1 || value > 256) return fail_msg(ctx, "exact_lookahead: -1 (adaptive), 0..256"); ctx->exactLookahead = value; ctx->lookValid = false; ctx->lookKeyValid = false; return 0; }
     if (!strcmp(key, "register_host")) { ctx->registerHost = value ? 1 : 0; return 0; }
-    if (!strcmp(key, "fast_kform")) { if (value < 0 || value > 3) return fail_msg(ctx, "fast_kform: 0..3"); ctx->fastKForm = value; return 0; }
+    if (!strcmp(key, "fast_kform")) { if (value < 0 || value > 4) return fail_msg(ctx, "fast_kform: 0..4"); ctx->fastKForm = value; return 0; }
     if (!strcmp(key, "fast_alpha_zero")) { ctx->fastAlphaZero = value ? 1 : 0; return 0; }
     if (!strcmp(key, "scene_upload_always")) { ctx->sceneUploadAlways = value ? 1 : 0; return 0; }
     if (!strcmp(key, "mitsuba_compare")) { ctx->sceneFlags = value ? (ctx->sceneFlags | kSceneMitsuba) : (ctx->sceneFlags & ~(uint32_t)kSceneMitsuba); return 0; }
@@ -416,6 +419,7 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
     *scene = ctx->scene;
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
+    scene->pairs.half = scene->halfOk && scene->kformOk && ctx->fastKForm == 2;
     return 0;
 }
 
@@ -1167,9 +1171,10 @@ int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long l
 
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays, int* outId, float* outT, long long n)
 {
-    if (!ctx || !rays || !outId || !outT || n <= 0 || kform < 0 || kform > 4) return (int)cudaErrorInvalidValue;
+    if (!ctx || !rays || !outId || !outT || n <= 0 || kform < 0 || kform > 5) return (int)cudaErrorInvalidValue;
     if (!ctx->scene.blob) return fail_msg(ctx, "tpt_debug_hit: no scene");
     if (kform == 4 && (ctx->scene.count + 3) / 4 * 4 > kParamPairSpheres) return fail_msg(ctx, "tpt_debug_hit: kform 4 takes at most 64 padded spheres");
+    if (kform == 5 && !ctx->scene.halfOk) return fail_msg(ctx, "tpt_debug_hit: the scene has no half-precision pass 1 (kform 5)");
     CK(cudaSetDevice(ctx->device), "cudaSetDevice");
     float *dRays = nullptr, *dT = nullptr;
     int* dId = nullptr;

@@ -22,6 +22,7 @@
 #include <cstdlib>
 #include <type_traits>
 #include <vector>
+#include <cuda_fp16.h>
 #include "tpt_integrator.cuh"
 #include "tpt_device_utils.cuh"
 #include "tpt_launch.h"
@@ -518,8 +519,89 @@ __device__ __forceinline__ unsigned long long sweep_chunk64(const P& pairs, int 
     const uint32_t c1 = n1 > 0 ? ~neg1 << (32 - n1) : 0u;
     return ((unsigned long long)c0 << 32) | c1;
 }
+// Sweep form 5's pass 1: packed half precision on ParamPairs::h (build_half_pairs states the test; DESIGN §3.1c derives its
+// error bound). Per pair of spheres: 6 HFMA2 for xu, xv, 2 HFMA2 for q = xu^2 + xv^2 - R'^2, and LOP3 + LEA.HI that shift
+// the two sign bits (15: low sphere, 31: high sphere) into the block's mask. There is no "wholly behind the origin" test:
+// pass 2 rejects those spheres (t <= tMin), and the study in DESIGN §3.1c found its 5 more slots per pair dearer than the
+// pass-2 trips it saves. The candidates contain form 4's, so pass 2 (unchanged, on {s, K}, ascending sphere order) makes
+// the same decisions. The form-4 kernels run it (FastHitterKH) when the parameter's `half` is set. The bound assumes
+// |o| <= kHalfOriginBound and a unit direction: if any active lane of the warp has a ray outside that, the warp runs
+// form 4's FP32 pass 1 on this trip.
+struct HalfPairsRef
+{
+    static constexpr bool kOneChunk = true;
+    const ParamPairs* pp;       // the kernel's __grid_constant__ parameter
+};
+struct HalfRay { __half2 ux, uy, uz, vx, vy, vz, nou, nov; };
+__device__ __forceinline__ __half2 u32_h2(uint32_t w) { __half2 h; memcpy(&h, &w, 4); return h; }
+__device__ __forceinline__ uint32_t h2_u32(__half2 h) { uint32_t w; memcpy(&w, &h, 4); return w; }
+template <int G>
+__device__ __forceinline__ void half_sweep_full(const ParamPairs* pp, int p0, uint32_t& acc, const HalfRay& r)
+{
+#pragma unroll
+    for (int j = 0; j < G; ++j)
+    {
+        const uint32_t* w = pp->h + (p0 + j) * kHalfPairWords;
+        const __half2 X = u32_h2(w[0]), Y = u32_h2(w[1]), Z = u32_h2(w[2]);
+        const __half2 xu = __hfma2(X, r.ux, __hfma2(Y, r.uy, __hfma2(Z, r.uz, r.nou)));
+        const __half2 xv = __hfma2(X, r.vx, __hfma2(Y, r.vy, __hfma2(Z, r.vz, r.nov)));
+        const __half2 q = __hfma2(xu, xu, __hfma2(xv, xv, u32_h2(w[3])));
+        acc = (acc >> 1) | (h2_u32(q) & 0x80008000u);
+    }
+}
+template <int G>
+__device__ __forceinline__ void half_sweep_upto(const ParamPairs* pp, int p0, int left, uint32_t& acc, const HalfRay& r)
+{
+    if (left >= G) half_sweep_full<G>(pp, p0, acc, r);
+    else if constexpr (G > 2)
+    {
+        if (left > 0)
+        {
+            half_sweep_upto<G / 2>(pp, p0, left, acc, r);
+            half_sweep_upto<G / 2>(pp, p0 + G / 2, left - G / 2, acc, r);
+        }
+    }
+}
+// The candidate mask of the block of 2h spheres whose h pairs start at pair p0: sphere j of the block at bit 31 - j.
+__device__ __forceinline__ uint32_t half_block_mask(const ParamPairs* pp, int p0, int h, const HalfRay& r)
+{
+    uint32_t acc = 0;
+    half_sweep_upto<TPT_P1_GROUP / 2>(pp, p0, h, acc, r);
+    half_sweep_upto<TPT_P1_GROUP / 2>(pp, p0 + TPT_P1_GROUP / 2, h - TPT_P1_GROUP / 2, acc, r);
+    // after h pairs, pair p's signs sit at bits 16 - h + p (sphere p) and 32 - h + p (sphere h + p)
+    const uint32_t low = (1u << h) - 1u;
+    return __brev(((acc >> (16 - h)) & low) | ((acc >> (32 - 2 * h)) & ~low));
+}
+
+// Pass 1 of one chunk of n spheres at base: sphere base + J <-> bit 63 - J of the candidate mask.
+template <class P>
+__device__ __forceinline__ unsigned long long pass1(const P& pairs, int base, int n, const SweepConsts& C, V3, V3)
+{
+    return sweep_chunk64(pairs, base, n, C);
+}
+__device__ __forceinline__ unsigned long long pass1(const HalfPairsRef& pairs, int, int n, const SweepConsts& C, V3 o, V3 d)
+{
+    const bool inBound = dot(o, o) <= kHalfOriginBound * kHalfOriginBound && fabsf(dot(d, d) - 1.0f) <= 0x1p-18f;
+    if (!__all_sync(__activemask(), inBound)) return sweep_chunk64(ParamPairsRef{pairs.pp}, 0, n, C);
+    // the branch-free orthonormal basis (u, v) around d of sample_light_cone
+    const float sgn = copysignf(1.0f, d.z);
+    const float a = __fdividef(-1.0f, sgn + d.z);
+    const float b = d.x * d.y * a;
+    const V3 u = v3(1.0f + sgn * d.x * d.x * a, sgn * b, -sgn * d.x);
+    const V3 v = v3(b, sgn + d.y * d.y * a, -d.y);
+    HalfRay r;
+    r.ux = __float2half2_rn(u.x); r.uy = __float2half2_rn(u.y); r.uz = __float2half2_rn(u.z);
+    r.vx = __float2half2_rn(v.x); r.vy = __float2half2_rn(v.y); r.vz = __float2half2_rn(v.z);
+    r.nou = __float2half2_rn(-dot(o, u)); r.nov = __float2half2_rn(-dot(o, v));
+    const int n0 = n < 32 ? n : 32, n1 = n - n0;
+    const uint32_t m0 = half_block_mask(pairs.pp, 0, n0 / 2, r);
+    const uint32_t m1 = n1 > 0 ? half_block_mask(pairs.pp, 16, n1 / 2, r) : 0u;
+    return ((unsigned long long)m0 << 32) | m1;
+}
+
 // FastHitterK2: pass 1 on the pair array in shared memory; FastHitterKC: on the pair array in the kernel parameter (scenes
-// of at most 64 padded spheres). Same values in the same operations: ids and distances are bit-identical.
+// of at most 64 padded spheres); FastHitterKH: form 5's half-precision pass 1 on the same parameter (form 4's on a fallback
+// trip). Same pass 2 on the same candidates or a superset of them: ids and distances are bit-identical.
 template <class P>
 struct FastHitterK2T
 {
@@ -545,7 +627,7 @@ struct FastHitterK2T
         // chunks of 64 spheres: pass 1 fills a 64-bit candidate mask (sphere base + J <-> bit 63 - J), pass 2 walks it
         for (int base = 0; base < (P::kOneChunk ? 1 : simdCount); base += 64)
         {
-            unsigned long long cand = sweep_chunk64(pairs, base, simdCount - base < 64 ? simdCount - base : 64, C);
+            unsigned long long cand = pass1(pairs, base, simdCount - base < 64 ? simdCount - base : 64, C, o, d);
             // pass 2, two candidates per trip (independent LDS.128 / 9 FMA / MUFU chains); ascending sphere order as before
             while (cand)
             {
@@ -574,6 +656,20 @@ struct FastHitterK2T
 };
 using FastHitterK2 = FastHitterK2T<SmemPairs>;
 using FastHitterKC = FastHitterK2T<ParamPairsRef>;
+using FastHitterKH = FastHitterK2T<HalfPairsRef>;
+// The sweep of the form-4 kernels: form 5's (FastHitterKH) when the launch's parameter sets `half`, else form 4's. Each
+// is a whole sweep, pass 1 and pass 2, so the FP32 one compiles as it does without form 5. (A choice inside pass 1 only
+// left the FP32 pass 1 9-14 % slower than without form 5 on H100; two whole queue bodies doubled the kernel's LDS.128.)
+struct FastHitterK45
+{
+    FastHitterKC fp32;
+    const ParamPairs* pp;
+    __device__ __forceinline__ int hit(const SceneView& sc, V3 o, V3 d, float tMin, float tMax, float& tOut) const
+    {
+        if (pp->half) return FastHitterKH{fp32.sphK, HalfPairsRef{pp}, fp32.simdCount}.hit(sc, o, d, tMin, tMax, tOut);
+        return fp32.hit(sc, o, d, tMin, tMax, tOut);
+    }
+};
 
 // Conservative form for scenes the expanded form is NOT accurate enough for (centres far from the origin: the gate in
 // tpt_set_scene fails, e.g. the 4096-sphere stress scene): pass 1 is the packed expanded-form sweep with an error bound
@@ -685,6 +781,8 @@ __host__ __device__ inline FastSmem fast_smem(uint32_t stagedBytes, uint32_t pai
 //   3  conservative pair array built from {s, r^2}, which stays for the reference-form pass 2 (FastHitterK2C)
 //   4  form 2 with the pair array in the kernel parameter pp (FastHitterKC; at most kParamPairSpheres padded spheres),
 //      no pair array in shared memory; pass 2 on {s, K} as in form 2
+//   5  form 4 with the half-precision pass 1 on pp->h (FastHitterKH). Not an instance of its own: the form-4 kernels
+//      sweep with FastHitterK45, which takes form 4's or form 5's complete sweep per call from pp->half
 // The sweep's loads are plain (schedulable) asm: their addresses are made opaque AFTER the barrier so that none of them
 // can be hoisted above the rewrite of the sphere array or the construction of the pair array.
 template <int KFORM>
@@ -712,8 +810,8 @@ __device__ __forceinline__ auto prepare_sweep(const SceneView& sc, unsigned char
     }
     else if constexpr (KFORM == 4)
     {
-        FastHitterKC h; h.sphK = sc.sphShared; h.pairs.pp = pp; h.simdCount = sc.simdCount;
-        asm volatile("" : "+r"(h.sphK));
+        FastHitterK45 h; h.fp32.sphK = sc.sphShared; h.fp32.pairs.pp = pp; h.fp32.simdCount = sc.simdCount; h.pp = pp;
+        asm volatile("" : "+r"(h.fp32.sphK));
         return h;
     }
     else
@@ -1817,7 +1915,8 @@ namespace tpt {
 // The families differ on purpose:
 //   slab queue (variants 3/4/9, and tpt_draw's automatic variant): the pair array where the blob, the pairs and 24
 //     camera-ray buffers fit in 200 KB, else form 1; pick_queue turns form 2 into form 4 (pair array in the kernel
-//     parameter) for scenes of at most 64 padded spheres when fast_kform is 2. A scene that fails the gate runs the
+//     parameter) for scenes of at most 64 padded spheres when fast_kform is 2 or 4; the form-4 instances run form 5 (the
+//     half-precision pass 1) when fast_kform is 2 and build_half_pairs accepted the scene. A scene that fails the gate runs the
 //     conservative form 3 when fast_kform is 2 or 3 and the pairs fit, else form 0.
 //   group and tile queue (variants 8 and 5): the pair array up to 1024 spheres, else form 1. No form 3: a scene that
 //     fails the gate runs form 0.
@@ -1914,9 +2013,10 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     QueuePick q;
     q.kform = fast_queue_kform(sc);
     // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
-    // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2)
-    if (q.kform == 2 && sc.kformMode == 2 && simd_count(sc) <= (uint32_t)kParamPairSpheres && SRC != kSrcPixels &&
-        !(SRC == kSrcCamera && variant == 4))
+    // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2). The same
+    // instances run form 5 (the half-precision pass 1) when the parameter says so (sc.pairs.half, begin_call).
+    if (q.kform == 2 && (sc.kformMode == 2 || sc.kformMode == 4) && simd_count(sc) <= (uint32_t)kParamPairSpheres &&
+        SRC != kSrcPixels && !(SRC == kSrcCamera && variant == 4))
         q.kform = 4;
     const bool big = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, q.kform), 4 * 2048).bytes > 36 * 1024 ||
                      sc.stagedBytes != sc.layout.totalBytes;
@@ -2019,13 +2119,15 @@ k_debug_hit(const unsigned char* __restrict__ blob, SceneBlobLayout L, int count
 
 cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, int* dId, float* dT, long long n, int numSMs, cudaStream_t stream)
 {
-    auto kern = for_kform<4>(kform, [](auto K) { return k_debug_hit<decltype(K)::value>; });
+    auto kern = for_kform<4>(kform == 5 ? 4 : kform, [](auto K) { return k_debug_hit<decltype(K)::value>; });
     // the blob padded to 128 B even without a pair array: the end of the (possibly empty) pair array
     const size_t dyn = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, kform)).buffers;
     if (dyn > 200 * 1024) return cudaErrorInvalidValue;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)dyn);
     if (e != cudaSuccess) return e;
-    kern<<<numSMs, 256, dyn, stream>>>(sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, dRays, dId, dT, n, sc.pairs);
+    ParamPairs pp = sc.pairs;
+    pp.half = kform == 5;
+    kern<<<numSMs, 256, dyn, stream>>>(sc.blob, sc.layout, sc.count, sc.nLights, sc.stagedBytes, dRays, dId, dT, n, pp);
     return cudaGetLastError();
 }
 

@@ -12,11 +12,12 @@ struct SceneDev
     int count, nLights;
     uint32_t stagedBytes;        // prefix of the blob every CTA stages into shared memory via TMA
     int kformMode;               // fast kernels: 2 = expanded form on the pair array where it fits (kernel parameter up to
-                                 // kParamPairSpheres, else shared memory), 3 = the same always in shared memory (A/B),
-                                 // 1 = expanded form, scalar
+                                 // kParamPairSpheres, else shared memory; form 5 where halfOk), 3 = the same always in
+                                 // shared memory (A/B), 4 = as 2 but form 4 never runs form 5's pass 1 (A/B), 1 = expanded form, scalar
     bool kformOk;                // every sphere satisfies |c|^2 <= 128 + 2 r^2: the expanded-form sweep of the fast kernels
                                  // then rounds no worse than the reference form (see FastHitterK)
-    ParamPairs pairs;            // pass-1 operands of sweep form 4 (all zero for scenes of more than kParamPairSpheres)
+    ParamPairs pairs;            // pass-1 operands of sweep forms 4 and 5 (all zero for scenes of more than kParamPairSpheres)
+    bool halfOk;                 // pairs.h holds form 5's half-precision pass 1 (build_half_pairs)
 };
 
 // lanes: 0 = choose from the number of (frame,row) chains; 1, 2, 8, 9, 32 or 64..71 to force (see tpt_exact.cu).
@@ -27,7 +28,8 @@ cudaError_t launch_resolve_exact(const DrawParams& p, cudaStream_t stream);
 cudaError_t launch_debug_libm(int fn, const float* dIn, float* dOut, long long n, cudaStream_t stream);
 // sweep form variants 3/4 run for this scene (0 reference, 1 expanded, 2 packed pairs, 3 conservative packed)
 int fast_queue_kform(const SceneDev& sc);
-// nearest hit of n rays {o.xyz, d.xyz} with one sweep form of the fast kernels (0 reference, 1 expanded, 2 packed pairs, 3 conservative)
+// nearest hit of n rays {o.xyz, d.xyz} with one sweep form of the fast kernels (0 reference, 1 expanded, 2 packed pairs, 3 conservative,
+// 4 packed pairs in the kernel parameter, 5 form 4 with the half-precision pass 1)
 cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, int* dId, float* dT, long long n, int numSMs, cudaStream_t stream);
 constexpr int kMaxFramesPerDraw = 256;  // frames per fast launch: per-frame blend weights live in shared memory
 

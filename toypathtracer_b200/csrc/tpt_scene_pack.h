@@ -6,6 +6,7 @@
 #include "tpt_types.h"
 #include <vector>
 #include <string.h>
+#include <math.h>
 
 namespace tpt {
 
@@ -101,6 +102,61 @@ inline void build_param_pairs(const std::vector<unsigned char>& blob, const Scen
         f[0] = s.x; f[2] = s.y; f[4] = s.z;
         f[6] = -(i < count ? (float)K : 1.0e30f);
     }
+}
+
+// IEEE binary16 bits of x rounded to nearest-even (mode 0), up (+1) or down (-1); |x| must stay below 65504.
+inline uint16_t half_bits(double x, int mode)
+{
+    const double ax = fabs(x);
+    int e = 0;
+    if (ax > 0) { frexp(ax, &e); --e; }                 // ax in [2^e, 2^(e+1))
+    const double q = ldexp(1.0, (e > -14 ? e : -14) - 10);
+    double k = x / q;                                    // exact: q is a power of two
+    k = mode > 0 ? ceil(k) : mode < 0 ? floor(k) : nearbyint(k);
+    const double v = fabs(k * q);
+    const uint16_t sign = (k < 0 || (k == 0 && signbit(x))) ? 0x8000u : 0u;
+    if (v < ldexp(1.0, -14)) return (uint16_t)(sign | (uint16_t)(v / ldexp(1.0, -24)));
+    int ev = 0;
+    const double m = frexp(v, &ev);                      // v = m 2^ev, m in [0.5, 1)
+    return (uint16_t)(sign | (uint16_t)((ev - 1 + 15) << 10) | (uint16_t)(m * 2048.0 - 1024.0));
+}
+
+// Sweep form 5's pass-1 operands (FastHitterKH, tpt_fast.cu; the bound is derived in DESIGN §3.1c). A sphere is a pass-1
+// candidate when, in half precision with u = 2^-11, xu = s.u - o.u and xv = s.v - o.v (u, v an orthonormal basis
+// around d) give xu^2 + xv^2 - R'^2 < 0: its line passes within R' of the centre. R' is the radius widened by the error
+// bound (E per coordinate, Rw for the FP32 rounding of form 2, the basis and |d|) for origins with |o| <= kHalfOriginBound and |d|^2 within 2^-18 of 1, so the candidate set contains every sphere
+// form 2's FP32 pass 2 accepts. Returns false (form 4 keeps the scene) when a scene has more than kParamPairSpheres
+// padded spheres or a sphere whose intermediates could leave the half range.
+inline bool build_half_pairs(const std::vector<unsigned char>& blob, const SceneBlobLayout& L, int count, ParamPairs& pp)
+{
+    const int simdCount = (count + 3) / 4 * 4;
+    if (simdCount > kParamPairSpheres) return false;
+    const Q4* sph = (const Q4*)(blob.data() + L.offSph);
+    const double u = ldexp(1.0, -11), Om = kHalfOriginBound, kLimit = 30000.0;
+    for (int base = 0; base < simdCount; base += 32)
+    {
+        const int n = simdCount - base < 32 ? simdCount - base : 32, h = n / 2;
+        for (int j = 0; j < n; ++j)
+        {
+            uint16_t x = 0, y = 0, z = 0, nr2 = half_bits(60000.0, 0);   // padding: q >= 60000, never a candidate
+            if (base + j < count)
+            {
+                const Q4 s = sph[base + j];
+                const double S = sqrt((double)s.x * s.x + (double)s.y * s.y + (double)s.z * s.z), R2 = s.w;
+                const double E = u * (5.01 * S + 4.01 * Om) + ldexp(1.0, -20);
+                const double Rw = sqrt(R2 + ldexp(S * S + Om * Om + R2, -15));
+                const double Rp2 = (Rw + 1.4143 * E) * (Rw + 1.4143 * E) / (1.0 - u) * (1.0 + ldexp(1.0, -20));
+                if ((S + Om + 1.0) * (S + Om + 1.0) > kLimit || Rp2 > kLimit) return false;
+                x = half_bits(s.x, 0); y = half_bits(s.y, 0); z = half_bits(s.z, 0);
+                nr2 = half_bits(-Rp2, -1);
+            }
+            uint32_t* w = pp.h + (base / 2 + j % h) * kHalfPairWords;
+            const int sh = j < h ? 0 : 16;
+            w[0] |= (uint32_t)x << sh; w[1] |= (uint32_t)y << sh; w[2] |= (uint32_t)z << sh;
+            w[3] |= (uint32_t)nr2 << sh;
+        }
+    }
+    return true;
 }
 
 inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlobLayout& L, int count, int nLights)

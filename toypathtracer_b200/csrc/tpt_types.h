@@ -76,8 +76,17 @@ inline int sampled_lights(uint32_t sceneFlags, int nLights) { return (sceneFlags
 // array of the expanded form, pair p = spheres 2p, 2p+1 as f[8p ..] = {x0, x1, y0, y1, z0, z1, -K0, -K1}, built on the
 // host (build_param_pairs) and passed by value in a __grid_constant__ kernel parameter, so that pass 1 reads the sphere
 // values from the constant bank into uniform registers instead of from shared memory into vector registers.
+// h: sweep form 5's half-precision pass 1 (build_half_pairs), four packed half2 words per pair {X, Y, Z, -R'^2};
+// pair p of the block of n spheres at 32B holds sphere 32B + p in its low half and sphere 32B + n/2 + p in its high half.
 constexpr int kParamPairSpheres = 64;
-struct ParamPairs { float f[kParamPairSpheres * 4]; };
+constexpr int kHalfPairWords = 4;
+constexpr float kHalfOriginBound = 16.0f;   // form 5's bound holds for ray origins with |o| <= kHalfOriginBound
+struct ParamPairs
+{
+    float f[kParamPairSpheres * 4];
+    uint32_t h[kParamPairSpheres / 2 * kHalfPairWords];
+    int half;           // 1: the form-4 kernels sweep with form 5's half-precision pass 1 on h (0: FP32 pass 1 on f)
+};
 
 struct DrawParams
 {
