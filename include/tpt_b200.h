@@ -249,6 +249,41 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
                      float* sum4, float* sq4, int buffersOnDevice,
                      long long* outRayCount, void* cudaStream);
 
+/* Per-entry sample sums and second moments of tpt_trace_rays (points = 0) or tpt_trace_irradiance (points = 1), for all
+ * inputs or a caller-listed subset: what adaptive sampling of caller rays and surface points needs (panoramas, lightmaps,
+ * irradiance probes), as tpt_draw_samples gives it for image pixels.
+ *   in6, numIn        numIn rays {o, d} (points = 0) or surface points {p, n} (points = 1), 6 floats each, loaded, validated
+ *                     and normalised exactly as tpt_trace_rays / tpt_trace_irradiance load them (same alignment).
+ *   ids               NULL, or numIn int32 sphere ids with tpt_trace_irradiance's meaning (id i belongs to input i). Only
+ *                     taken with points = 1.
+ *   entries           n int32 indices into in6, any order, duplicates allowed. NULL = every input, and then n must be numIn.
+ *   spp, frame        samples per listed entry. Sample s of input i at `frame` is exactly the sample tpt_trace_rays /
+ *                     tpt_trace_irradiance traces for input i: stream pixel_seed(i * spp + s, frame), keyed by the INPUT,
+ *                     not by the list position. So an all-input call traces the samples of the mean call with the same spp
+ *                     and frame, a list call traces for each listed input the samples the all-input call traces for it,
+ *                     and frame + 1, frame + 2, ... give independent further samples. numIn * spp must not exceed 2^32.
+ *   sum4              n float4, ACCUMULATED: entry k (list position) receives += (sum v.r, sum v.g, sum v.b, count), v being
+ *                     the path radiance for rays and pi x the white-Lambert radiance for points; sum.rgb / sum.w estimates
+ *                     what tpt_trace_rays / tpt_trace_irradiance return.
+ *   sq4               NULL, or n float4 accumulated as += (sum v.r^2, sum v.g^2, sum v.b^2, 0).
+ *   buffersOnDevice   0: host pointers, staged through the context (sum4 and sq4 are uploaded, since the call adds to them)
+ *                     and the call is synchronous; 1: device pointers of the context's device (or mapped host memory),
+ *                     in6, ids and entries 4-byte, sum4 / sq4 16-byte aligned.
+ *   outRayCount       NULL or receives the number of rays traced (as tpt_trace_rays / tpt_trace_irradiance count them).
+ * An input that tpt_trace_rays would not trace (a non-finite component, or a direction or normal that does not normalise)
+ * adds NOTHING: its entries' counts stay as they were and it adds no rays. (tpt_draw_samples always adds spp.)
+ * An index outside [0, numIn) is found on the device before anything is traced: the call then traces nothing, adds nothing
+ * and fails, tpt_last_error naming the first such entry and its value. A call with a list is therefore synchronous; one
+ * without it and with device buffers synchronises only when a ray count is requested. n == 0 launches nothing and reads
+ * no buffer. n must not exceed 2^32 - 1, nor the slabs (64 entries x one sample) 2^31 - 1.
+ * Ordering and accounting (tpt_read_ray_count, tpt_last_kernel_ms, tpt_last_launch_count, tpt_debug_last_kernels) are
+ * those of tpt_trace_rays. NULL in6 or sum4, ids with points = 0, n != numIn without a list, n or numIn < 0, spp < 1, a
+ * misaligned device buffer or one on another device are refused (tpt_last_error gives the reason). */
+int tpt_trace_samples(tpt_context* ctx, const float* in6, const int* ids, int points, long long numIn,
+                      const int* entries, long long n, int spp, int frame,
+                      float* sum4, float* sq4, int buffersOnDevice,
+                      long long* outRayCount, void* cudaStream);
+
 /* Rays traced by all draws since the last call of this function (synchronises the stream). */
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStream, long long* outRays);
 /* Device time (CUDA events on the launching stream) of the kernels of the most recent tpt_draw, in ms. */
@@ -292,8 +327,8 @@ int tpt_debug_libm(tpt_context* ctx, int fn, const float* in, float* out, long l
  * of at most 64 padded spheres only, 5 as 4 with the half-precision first pass: scenes that pass its gate only), tMin/tMax as Trace uses them. outId -1 = miss. */
 int tpt_debug_hit(tpt_context* ctx, int kform, const float* rays6, int* outId, float* outT, long long n);
 /* Diagnostic: the mangled names of the trace kernels (path tracing and first-hit AOV kernels, not the helpers that clear,
- * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples,
- * tpt_draw_aovs or tpt_trace_aovs launched, in launch order, separated by '\n' and NUL-terminated in buf[cap].
+ * blend or count) that the CALLING THREAD's most recent tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_trace_samples,
+ * tpt_draw_samples, tpt_draw_aovs or tpt_trace_aovs launched, in launch order, separated by '\n' and NUL-terminated in buf[cap].
  *   - The record is per host thread, not per context: a call on another thread, or on another context from this
  *     thread, replaces it.
  *   - A call resets it when it starts launching (an empty call too). A call refused before that leaves the previous

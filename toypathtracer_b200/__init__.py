@@ -84,6 +84,8 @@ def _load_lib():
     L.tpt_trace_aovs.argtypes = [vp, vp, ci, cll, vp, vp, vp, ci, ctypes.POINTER(cll), vp]; L.tpt_trace_aovs.restype = ci
     L.tpt_draw_samples.argtypes = [vp, ci, ci, ci, vp, cll, ci, vp, vp, ci, ctypes.POINTER(cll), vp]
     L.tpt_draw_samples.restype = ci
+    L.tpt_trace_samples.argtypes = [vp, vp, vp, ci, cll, vp, cll, ci, ci, vp, vp, ci, ctypes.POINTER(cll), vp]
+    L.tpt_trace_samples.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -457,19 +459,30 @@ class Context:
             n = _entries("draw_samples", "pixels", pixels, n, ())
         if n < 0:
             raise TptError("draw_samples: n < 0")
+        sum4, sq4, stream = self._sums_outputs("draw_samples", pixels, n, sum4, sq4, stream, pixels)
+        (pp, ps, pq), on_dev, _keep = _buffer_ptrs(
+            "draw_samples", [("pixels", pixels, "int32", 1), ("sum4", sum4, "float32", 4), ("sq4", sq4, "float32", 4)], n)
+        total = self._call("tpt_draw_samples", want_rays, stream, int(frame), int(width), int(height), pp, n, spp, ps, pq,
+                           1 if on_dev else 0)
+        return ((sum4, sq4), total) if want_rays else (sum4, sq4)
+
+    def _sums_outputs(self, what: str, like, n: int, sum4, sq4, stream: int, *inputs):
+        """(sum4, sq4, stream) of a sums call (draw_samples, trace_samples) with the caller's `inputs` buffers: missing
+        outputs allocated zeroed, of the kind of `like` (a CUDA tensor on the context's device for None or a DevicePtr),
+        and the stream the call runs on."""
         if sum4 is None and sq4 is not None:
-            raise TptError("draw_samples: sq4 needs sum4")
+            raise TptError(f"{what}: sq4 needs sum4")
         alloc_dev = None
         if sum4 is None:
-            if isinstance(pixels, np.ndarray):
+            if isinstance(like, np.ndarray):
                 sum4, sq4 = np.zeros((n, 4), np.float32), np.zeros((n, 4), np.float32)
             else:
                 import torch
-                alloc_dev = pixels.device if hasattr(pixels, "device") else torch.device("cuda", self.device)
+                alloc_dev = like.device if hasattr(like, "device") else torch.device("cuda", self.device)
         # Torch CUDA tensors are written and read on torch's streams, which the library does not know: without an
         # explicit stream the call runs on torch's current stream of their device, after the torch work that filled
         # them (and the zeroing of outputs allocated here) and before the torch work that reads the sums.
-        tdev = _cuda_device(pixels, sum4, sq4) or (alloc_dev if alloc_dev is not None and alloc_dev.type == "cuda" else None)
+        tdev = _cuda_device(*inputs, sum4, sq4) or (alloc_dev if alloc_dev is not None and alloc_dev.type == "cuda" else None)
         explicit = bool(stream)
         if tdev is not None and not explicit:
             stream = _torch_stream(tdev)
@@ -482,11 +495,90 @@ class Context:
             with on:
                 sum4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
                 sq4 = torch.zeros((n, 4), dtype=torch.float32, device=alloc_dev)
-        (pp, ps, pq), on_dev, _keep = _buffer_ptrs(
-            "draw_samples", [("pixels", pixels, "int32", 1), ("sum4", sum4, "float32", 4), ("sq4", sq4, "float32", 4)], n)
-        total = self._call("tpt_draw_samples", want_rays, stream, int(frame), int(width), int(height), pp, n, spp, ps, pq,
-                           1 if on_dev else 0)
+        return sum4, sq4, stream
+
+    def trace_samples(self, inputs, ids=None, points: bool = False, entries=None, spp: int = 4, frame: int = 0, sum4=None,
+                      sq4=None, stream: int = 0, want_rays: bool = True, n=None, num_in=None):
+        """tpt_trace_samples: `spp` more samples of trace_rays (points False: `inputs` are rays {o.xyz, d.xyz}) or
+        trace_irradiance (points True: surface points {p.xyz, n.xyz}, `ids` their sphere ids or None) for each entry of
+        `entries` — int32 indices into inputs, duplicates and any order allowed; None = every input — ADDED to sum4
+        (sum v.r, v.g, v.b, sample count) and, when given, sq4 (sum v.r^2, v.g^2, v.b^2, 0), both (N, 4) float32, v being
+        the radiance (rays) or pi x the white-Lambert radiance (points). Sample s of input i at `frame` is the mean call's
+        own (stream pixel_seed(i * spp + s, frame)), so an all-input call traces trace_rays' / trace_irradiance's samples
+        at the same spp and frame. An input those calls do not trace adds no sample and no rays. Buffers are numpy
+        arrays, torch tensors (CPU or CUDA) or DevicePtr (DevicePtr inputs need `num_in`, a DevicePtr list `n`), all host
+        or all device. Allocation of missing sums (of the kind of `inputs`), streams and the return value are those of
+        draw_samples. A call with a list is synchronous."""
+        what = "trace_samples"
+        if isinstance(inputs, DevicePtr) and num_in is None:
+            raise TptError("trace_samples: DevicePtr inputs need num_in")
+        num_in = _entries(what, "inputs", inputs, num_in, (6,))
+        if ids is not None:
+            if not points:
+                raise TptError("trace_samples: ids are only taken with points")
+            _entries(what, "ids", ids, num_in, ())
+        if entries is None:
+            if n is not None and int(n) != num_in:
+                raise TptError("trace_samples: without entries n must be num_in")
+            n = num_in
+        else:
+            n = _entries(what, "entries", entries, n, ())
+        sum4, sq4, stream = self._sums_outputs(what, inputs, n, sum4, sq4, stream, inputs, ids, entries)
+        (pi, pd), in_dev, _keep = _buffer_ptrs(what, [("inputs", inputs, "float32", 6), ("ids", ids, "int32", 1)], num_in)
+        (pe, ps, pq), out_dev, _keep_out = _buffer_ptrs(
+            what, [("entries", entries, "int32", 1), ("sum4", sum4, "float32", 4), ("sq4", sq4, "float32", 4)], n)
+        if in_dev != out_dev:
+            raise TptError("trace_samples: inputs, ids, entries, sum4 and sq4 must be all host or all device buffers")
+        total = self._call("tpt_trace_samples", want_rays, stream, pi, pd, 1 if points else 0, num_in, pe, n, int(spp),
+                           int(frame), ps, pq, 1 if in_dev else 0)
         return ((sum4, sq4), total) if want_rays else (sum4, sq4)
+
+    @staticmethod
+    def _adaptive_rounds(call, base_spp: int, max_spp: int, rel_err: float, frame: int, shape):
+        """The round loop of render_adaptive and trace_adaptive: call(frame, entries or None) -> ((sum4, sq4), rays) adds
+        base_spp samples per entry. One all-entry pass at `frame`, then rounds at frame + 1, ... over the entries
+        adaptive_pixels picks (`shape`: its dilation grid), until it picks none or every entry has max_spp. Entries the
+        first pass gave no sample (untraceable inputs) are shown to the rule as finished, with max_spp samples and no
+        variance, so they are neither picked nor grow the picked set. Returns (sum4, rays)."""
+        import torch
+        (s, q), rays = call(frame, None)
+        dead = (s[:, 3] == 0).unsqueeze(1)
+        finished = torch.tensor([0.0, 0.0, 0.0, float(max_spp)], dtype=s.dtype, device=s.device)
+        for f in range(frame + 1, frame + 1 + (max_spp - base_spp) // base_spp):
+            idx = adaptive_pixels(torch.where(dead, finished, s), q, rel_err, max_spp, shape)
+            if idx.numel() == 0:
+                break
+            (ds, dq), r = call(f, idx)
+            s.index_add_(0, idx.long(), ds)
+            q.index_add_(0, idx.long(), dq)
+            rays += r
+        return s, rays
+
+    def trace_adaptive(self, inputs, ids=None, points: bool = False, base_spp: int = 4, max_spp: int = 64,
+                       rel_err: float = 0.05, frame: int = 0, shape: Optional[Tuple[int, int]] = None):
+        """Adaptive trace_rays (points False) or trace_irradiance (points True) on the device: one trace_samples pass over
+        every input at base_spp (frame `frame`), then rounds at frames frame + 1, frame + 2, ... that give base_spp more
+        samples to the inputs adaptive_pixels picks, until it picks none or every input has max_spp. shape = (h, w)
+        declares that the N inputs form a row-major h x w grid (an equirect panorama, a lightmap's texels): the rule then
+        grows the picked set by each picked entry's 3 x 3 neighbourhood, as render_adaptive does; without it there is no
+        dilation. `inputs` and `ids` are (N, 6) float32 and (N,) int32 arrays or tensors (copied to the context's device
+        if they are elsewhere). Untraceable inputs get no sample: they report 0 samples and a zero mean. Returns (mean
+        float32 (N, 4) with alpha 0, samples per input int32 (N,), rays traced), all but the ray count CUDA tensors."""
+        import torch
+        if base_spp < 1 or max_spp < base_spp:
+            raise TptError("trace_adaptive: need 1 <= base_spp <= max_spp")
+        dev = torch.device("cuda", self.device)
+        inputs = torch.as_tensor(inputs, device=dev)
+        ids = None if ids is None else torch.as_tensor(ids, device=dev)
+        n = _entries("trace_adaptive", "inputs", inputs, None, (6,))
+        if shape is not None and int(shape[0]) * int(shape[1]) != n:
+            raise TptError("trace_adaptive: shape does not hold N inputs")
+        # every buffer is a CUDA tensor, so each trace_samples call runs on torch's current stream
+        s, rays = self._adaptive_rounds(lambda f, idx: self.trace_samples(inputs, ids, points, idx, base_spp, f),
+                                        base_spp, max_spp, rel_err, frame, shape)
+        mean = torch.zeros((n, 4), dtype=torch.float32, device=dev)
+        mean[:, :3] = s[:, :3] / s[:, 3:].clamp(min=1.0)
+        return mean, s[:, 3].round().to(torch.int32), rays
 
     def render_adaptive(self, width: int, height: int, base_spp: int = 4, max_spp: int = 64, rel_err: float = 0.05,
                         frame: int = 0):
@@ -500,15 +592,8 @@ class Context:
             raise TptError("render_adaptive: need 1 <= base_spp <= max_spp")
         dev = torch.device("cuda", self.device)
         # every buffer is a CUDA tensor, so each draw_samples call runs on torch's current stream
-        (s, q), rays = self.draw_samples(frame, width, height, None, base_spp)
-        for f in range(frame + 1, frame + 1 + (max_spp - base_spp) // base_spp):
-            idx = adaptive_pixels(s, q, rel_err, max_spp, (height, width))
-            if idx.numel() == 0:
-                break
-            (ds, dq), r = self.draw_samples(f, width, height, idx, base_spp)
-            s.index_add_(0, idx.long(), ds)
-            q.index_add_(0, idx.long(), dq)
-            rays += r
+        s, rays = self._adaptive_rounds(lambda f, idx: self.draw_samples(f, width, height, idx, base_spp),
+                                        base_spp, max_spp, rel_err, frame, (height, width))
         image = torch.zeros((height, width, 4), dtype=torch.float32, device=dev)
         image.view(-1, 4)[:, :3] = s[:, :3] / s[:, 3:]
         return image, s[:, 3].round().to(torch.int32).view(height, width), rays
@@ -577,7 +662,8 @@ class Context:
         return ids, t
 
     def last_kernels(self):
-        """Trace kernels the calling thread's most recent draw / trace_rays / draw_samples / AOV call launched, as
+        """Trace kernels the calling thread's most recent draw / trace_rays / trace_irradiance / trace_samples /
+        draw_samples / AOV call launched, as
         readable template instances (kernel_signature), in launch order. The library names the first 16 launches; past
         that the list ends with "... N more launches" (see tpt_debug_last_kernels)."""
         buf = ctypes.create_string_buffer(4096)

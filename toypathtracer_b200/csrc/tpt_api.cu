@@ -606,6 +606,29 @@ static int stage_out(tpt_context* ctx, cudaStream_t stream, const CallerBuffer (
     return 0;
 }
 
+// The device index check of a caller list (tpt_draw_samples, tpt_trace_samples): its word and the pinned host word
+// its result comes back in, allocated on first use.
+static int ensure_index_check(tpt_context* ctx)
+{
+    if (ctx->dBadPixel) return 0;
+    CK(cudaMalloc(&ctx->dBadPixel, sizeof(unsigned long long)), "cudaMalloc index check");
+    CK(cudaMallocHost(&ctx->hBadPixel, sizeof(unsigned long long)), "cudaMallocHost index check");
+    return 0;
+}
+
+// The end of a caller-buffer call of one frame: the ray count, the index check's result (list = the call had a list),
+// the host outputs, and the synchronisation (sync: a host buffer; a list makes the call synchronous too, its index check
+// being the call's result, which the caller then reads from *ctx->hBadPixel).
+template <int N>
+static int end_caller_call(tpt_context* ctx, cudaStream_t stream, const CallerBuffer (&bufs)[N], bool list, bool sync,
+                           long long* outRayCount)
+{
+    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
+    if (list) CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream), "D2H index check");
+    if (int r = stage_out(ctx, stream, bufs)) return r;
+    return finish_call(ctx, stream, 1, sync || list, outRayCount, nullptr);
+}
+
 // Page-locks (and maps) the caller's host buffer once ("register_host"): copies run at full PCIe rate and the kernels can
 // store into it directly. Failure is not fatal.
 static void register_host(tpt_context* ctx, void* host, size_t bytes)
@@ -838,60 +861,91 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     return finish_call(ctx, stream, numFrames, !bufferOnDevice, outRayCount, outRaysPerFrame);
 }
 
-// tpt_trace_rays (points = false: in6 holds rays {o, d}) and tpt_trace_irradiance (points = true: in6 holds surface points
-// {p, n}, ids their sphere ids or null): the same checks, staging and launch of the slab queue on caller entries.
-static int trace_caller_entries(tpt_context* ctx, const char* fn, bool points, const float* in6, const int* ids, int inOnDevice,
-                                long long n, int spp, int frame, float* out4, int outOnDevice, long long* outRayCount,
+// tpt_trace_rays (points = false: in6 holds rays {o, d}), tpt_trace_irradiance (points = true: in6 holds surface points
+// {p, n}, ids their sphere ids or null) and tpt_trace_samples (sums = true: entries null or a list of n indices into the
+// numIn inputs, out4 = sum4 and sq4 accumulated): the same checks, staging and launch of the slab queue on caller entries.
+// Without sums, n == numIn and there is no list.
+static int trace_caller_entries(tpt_context* ctx, const char* fn, const char* inName, bool points, bool sums, const float* in6,
+                                const int* ids, int inOnDevice, long long numIn, const int* entries, long long n, int spp,
+                                int frame, float* out4, float* sq4, int outOnDevice, long long* outRayCount,
                                 void* cudaStreamArg)
 {
-    const char* inName = points ? "points6" : "rays6";
+    const char* outName = sums ? "sum4" : "out4";
     if (!ctx) return (int)cudaErrorInvalidValue;
     if (!ctx->haveScene) return fail_msgf(ctx, "%s: no scene (call tpt_set_scene first)", fn);
-    if (!in6 || !out4) return fail_msgf(ctx, "%s: null %s or out4", fn, inName);
-    if (n < 0) return fail_msgf(ctx, "%s: n < 0", fn);
+    if (!in6 || !out4) return fail_msgf(ctx, "%s: null %s or %s", fn, inName, outName);
+    if (numIn < 0 || n < 0) return fail_msgf(ctx, "%s: n < 0", fn);
     if (spp < 1) return fail_msgf(ctx, "%s: spp < 1", fn);
-    // the sample stream of (entry i, sample s) is i * spp + s in 32 bits, and so is the entry index
-    if (n > (1LL << 32) / spp || n > 0xffffffffLL) return fail_msgf(ctx, "%s: n * spp > 2^32 (32-bit sample streams)", fn);
-    CallerBuffer bufs[] = {{inName, (void*)in6, inOnDevice != 0, 4, (size_t)n * 24, kStageRays, kCopyUp},
-                           {"ids", (void*)ids, inOnDevice != 0, 4, (size_t)n * 4, kStageIds, kCopyUp},
-                           {"out4", out4, outOnDevice != 0, 16, (size_t)n * 16, kStageImage, kCopyDown}};
+    // the sample stream of (input i, sample s) is i * spp + s in 32 bits, and so is the input index
+    if (numIn > (1LL << 32) / spp || numIn > 0xffffffffLL)
+        return fail_msgf(ctx, "%s: %s * spp > 2^32 (32-bit sample streams)", fn, sums ? "numIn" : "n");
+    if (ids && !points) return fail_msgf(ctx, "%s: ids are only taken with points", fn);
+    if (!entries && n != numIn) return fail_msgf(ctx, "%s: without entries n must be numIn", fn);
+    if (sums && (n > 0xffffffffLL || (n + fast_slab_pixels() - 1) / fast_slab_pixels() * spp > 0x7fffffffLL))
+        return fail_msgf(ctx, "%s: n * spp too large (2^31 slabs of 64 entries x one sample)", fn);
+    // an empty sums call: nothing to trace, no buffer is read (as tpt_draw_samples)
+    if (sums && n == 0) return empty_call(ctx, outRayCount);
+    // the sums accumulate: host sums go up and come back
+    const int outCopy = sums ? kCopyUp | kCopyDown : kCopyDown;
+    CallerBuffer bufs[] = {{inName, (void*)in6, inOnDevice != 0, 4, (size_t)numIn * 24, kStageRays, kCopyUp},
+                           {"ids", (void*)ids, inOnDevice != 0, 4, (size_t)numIn * 4, kStageIds, kCopyUp},
+                           {"entries", (void*)entries, inOnDevice != 0, 4, (size_t)n * 4, kStagePixels, kCopyUp},
+                           {outName, out4, outOnDevice != 0, 16, (size_t)n * 16, kStageImage, outCopy},
+                           {"sq4", sq4, outOnDevice != 0, 16, (size_t)n * 16, kStageSq4, kCopyUp | kCopyDown}};
     if (int r = check_buffers(ctx, fn, bufs)) return r;
     if (n == 0) return empty_call(ctx, outRayCount);
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+    if (entries)
+        if (int r = ensure_index_check(ctx)) return r;
     if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
     DrawParams p;
     memset(&p, 0, sizeof(p));
     p.spp = spp;
     p.frame0 = frame; p.numFrames = 1;     // flags 0: the one frame has weight 1, `prev` none
-    p.image = (float*)bufs[2].dev;
+    p.image = (float*)bufs[3].dev;
+    p.sq4 = (float*)bufs[4].dev;
     p.rayCounter = ctx->dRayCounters;
     p.workCounter = next_work_counter(ctx);
     p.rays = (const float*)bufs[0].dev;
     p.numRays = (uint32_t)n;
     p.pointStart = points ? 1 : 0;
     p.pointIds = (const int*)bufs[1].dev;
-    cudaError_t e = launch_fast_rays(p, scene, ctx->numSMs, stream);
+    p.sums = sums ? 1 : 0;
+    p.entries = (const int*)bufs[2].dev;
+    cudaError_t e = launch_fast_rays(p, scene, numIn, ctx->dBadPixel, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
-    if (int r = stage_out(ctx, stream, bufs)) return r;
-    return finish_call(ctx, stream, 1, !inOnDevice || !outOnDevice, outRayCount, nullptr);
+    if (int r = end_caller_call(ctx, stream, bufs, entries != nullptr, !inOnDevice || !outOnDevice, outRayCount)) return r;
+    if (entries && *ctx->hBadPixel != ~0ull)
+        return fail_msgf(ctx, "%s: entries[%llu] = %d is outside the %lld inputs (nothing was traced)", fn,
+                         *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, numIn);
+    return 0;
 }
 
 int tpt_trace_rays(tpt_context* ctx, const float* rays6, int raysOnDevice, long long n, int spp, int frame,
                    float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
 {
-    return trace_caller_entries(ctx, "tpt_trace_rays", false, rays6, nullptr, raysOnDevice, n, spp, frame, out4, outOnDevice,
-                                outRayCount, cudaStreamArg);
+    return trace_caller_entries(ctx, "tpt_trace_rays", "rays6", false, false, rays6, nullptr, raysOnDevice, n, nullptr, n, spp,
+                                frame, out4, nullptr, outOnDevice, outRayCount, cudaStreamArg);
 }
 
 int tpt_trace_irradiance(tpt_context* ctx, const float* points6, const int* ids, int pointsOnDevice, long long n,
                          int spp, int frame, float* out4, int outOnDevice, long long* outRayCount, void* cudaStreamArg)
 {
-    return trace_caller_entries(ctx, "tpt_trace_irradiance", true, points6, ids, pointsOnDevice, n, spp, frame, out4,
-                                outOnDevice, outRayCount, cudaStreamArg);
+    return trace_caller_entries(ctx, "tpt_trace_irradiance", "points6", true, false, points6, ids, pointsOnDevice, n, nullptr, n,
+                                spp, frame, out4, nullptr, outOnDevice, outRayCount, cudaStreamArg);
+}
+
+int tpt_trace_samples(tpt_context* ctx, const float* in6, const int* ids, int points, long long numIn,
+                      const int* entries, long long n, int spp, int frame,
+                      float* sum4, float* sq4, int buffersOnDevice,
+                      long long* outRayCount, void* cudaStreamArg)
+{
+    if (ctx && points != 0 && points != 1) return fail_msg(ctx, "tpt_trace_samples: points must be 0 or 1");
+    return trace_caller_entries(ctx, "tpt_trace_samples", "in6", points != 0, true, in6, ids, buffersOnDevice, numIn, entries, n,
+                                spp, frame, sum4, sq4, buffersOnDevice, outRayCount, cudaStreamArg);
 }
 
 int tpt_draw_aovs(tpt_context* ctx, int frameCount, int numFrames, int width, int height,
@@ -999,11 +1053,8 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    if (pixels && !ctx->dBadPixel)
-    {
-        CK(cudaMalloc(&ctx->dBadPixel, sizeof(unsigned long long)), "cudaMalloc index check");
-        CK(cudaMallocHost(&ctx->hBadPixel, sizeof(unsigned long long)), "cudaMallocHost index check");
-    }
+    if (pixels)
+        if (int r = ensure_index_check(ctx)) return r;
     if (int r = stage_in(ctx, stream, bufs)) return r;
     if (int r = start_kernels(ctx, stream, 1)) return r;
     DrawParams p = image_params(ctx, width, height, 0, height, 1, 0, spp, 0);
@@ -1016,11 +1067,7 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
     p.workCounter = next_work_counter(ctx);
     cudaError_t e = launch_fast_samples(p, scene, ctx->dBadPixel, ctx->numSMs, stream);
     if (e != cudaSuccess) return fail(ctx, e, "kernel launch");
-    if (int r = finish_kernels(ctx, stream, 1, outRayCount != nullptr)) return r;
-    if (pixels) CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, stream), "D2H index check");
-    if (int r = stage_out(ctx, stream, bufs)) return r;
-    // a pixel list makes the call synchronous: its index check is the call's result
-    if (int r = finish_call(ctx, stream, 1, !buffersOnDevice || pixels, outRayCount, nullptr)) return r;
+    if (int r = end_caller_call(ctx, stream, bufs, pixels != nullptr, !buffersOnDevice, outRayCount)) return r;
     if (pixels && *ctx->hBadPixel != ~0ull)
         return fail_msgf(ctx, "tpt_draw_samples: pixels[%llu] = %d is outside the %d x %d image (nothing was traced)",
                          *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, width, height);

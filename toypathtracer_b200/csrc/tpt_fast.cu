@@ -217,21 +217,42 @@ __device__ __forceinline__ void generate_slab_rays(const DrawParams& p, float4 (
 // pixel_seed(ray * spp + sample, frame). A ray with a non-finite component, or whose direction does not normalise to a finite
 // non-zero vector (zero length, or a squared length that underflows or overflows), is dropped: the survivors are written
 // compacted, in ray order, as {origin.xyz, rng state} {direction.xyz, ray index}. Returns their number.
+// With a list (p.entries, tpt_trace_samples) [r0, r0 + count) are list entries: each lane reads its two indices (32
+// consecutive ints per row) and gathers those inputs' 6 floats; the stream is the input's, pixel_seed(input * spp + sample,
+// frame), and the tag the entry. The indices were checked against the inputs before the launch (k_check_pixels).
 __device__ __forceinline__ uint32_t load_slab_rays(const DrawParams& p, float4 (*rays)[2], int lane, uint32_t count,
                                                    uint32_t r0, uint32_t sample, uint32_t frame)
 {
-    float* raw = reinterpret_cast<float*>(rays);
-    const float* src = p.rays + (size_t)r0 * 6;
-#pragma unroll
-    for (uint32_t k = 0; k < 6 * kSlabPix; k += 32)
-        if (k + lane < 6 * count) raw[k + lane] = __ldg(src + k + lane);
-    __syncwarp();
     float v[2][6];
+    uint32_t in[2];
+    if (p.entries)
+    {
 #pragma unroll
-    for (int h = 0; h < 2; ++h)
+        for (int h = 0; h < 2; ++h)
+        {
+            const uint32_t q = (uint32_t)lane + 32u * h;
+            in[h] = q < count ? (uint32_t)__ldg(p.entries + r0 + q) : 0u;
 #pragma unroll
-        for (int j = 0; j < 6; ++j) v[h][j] = (uint32_t)(lane + 32 * h) < count ? raw[(lane + 32 * h) * 6 + j] : 0.0f;
-    __syncwarp();
+            for (int j = 0; j < 6; ++j) v[h][j] = q < count ? __ldg(p.rays + (size_t)in[h] * 6 + j) : 0.0f;
+        }
+    }
+    else
+    {
+        float* raw = reinterpret_cast<float*>(rays);
+        const float* src = p.rays + (size_t)r0 * 6;
+#pragma unroll
+        for (uint32_t k = 0; k < 6 * kSlabPix; k += 32)
+            if (k + lane < 6 * count) raw[k + lane] = __ldg(src + k + lane);
+        __syncwarp();
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+        {
+            in[h] = r0 + (uint32_t)lane + 32u * h;
+#pragma unroll
+            for (int j = 0; j < 6; ++j) v[h][j] = (uint32_t)(lane + 32 * h) < count ? raw[(lane + 32 * h) * 6 + j] : 0.0f;
+        }
+        __syncwarp();
+    }
     uint32_t base = 0;
     const unsigned ltMask = (1u << lane) - 1u;
 #pragma unroll
@@ -246,7 +267,7 @@ __device__ __forceinline__ uint32_t load_slab_rays(const DrawParams& p, float4 (
         if (ok)
         {
             const uint32_t slot = base + (uint32_t)__popc(m & ltMask);
-            const uint32_t rng = pixel_seed((r0 + q) * (uint32_t)p.spp + sample, frame);
+            const uint32_t rng = pixel_seed(in[h] * (uint32_t)p.spp + sample, frame);
             rays[slot][0] = make_float4(o.x, o.y, o.z, __uint_as_float(rng));
             rays[slot][1] = make_float4(d.x, d.y, d.z, __uint_as_float(r0 + q));
         }
@@ -1003,6 +1024,13 @@ __device__ __forceinline__ void begin_vertex(const SceneView& sc, QPath& st, int
     lambert_next<LS>(sc, st, 0);
 }
 
+// The sphere id of point entry `tag` (tpt_trace_irradiance, tpt_trace_samples): ids are per input, so an entry of a list
+// reads its input's. -1 without ids.
+__device__ __forceinline__ int point_id(const int* ids, const int* entries, uint32_t tag)
+{
+    return ids ? __ldg(ids + (entries ? (uint32_t)__ldg(entries + tag) : tag)) : -1;
+}
+
 // ---- variant 0 ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(kFastThreads)
 k_fast_mega(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights, uint32_t stagedBytes)
@@ -1152,6 +1180,8 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // SRC: the ray source. kSrcCamera: camera rays of the image region. kSrcRays (k_fast_rays): the caller's p.numRays rays
 // (load_slab_rays), a slab being 64 consecutive rays x one sample index, finished paths adding col / spp to p.image[ray];
 // with p.pointStart (tpt_trace_irradiance) the entries are surface points, each sample starting as a Lambert vertex.
+// With p.sums (tpt_trace_samples) they add (v, 1) and, with p.sq4, (v^2, 0) per sample instead, and with p.entries the
+// slab's entries are list positions whose inputs load_slab_rays gathers.
 // kSrcPixels (k_fast_samples): the draw's camera rays for the p.numRays entries of a pixel list (generate_list_rays), a
 // slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
 // MOMENTS, (col^2, 0) to p.sq4[entry].
@@ -1162,9 +1192,12 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                 uint32_t raysOffset, const ParamPairs& pp)
 {
-    // a pixel list with an index outside the image traces nothing (the call reports the index)
+    // a pixel list with an index outside the image, or an entry list with an index outside the inputs, traces nothing
+    // (the call reports the index)
     if constexpr (SRC == kSrcPixels)
         if (p.pixels && *p.badPixel != ~0ull) return;
+    if constexpr (SRC == kSrcRays)
+        if (p.entries && *p.badPixel != ~0ull) return;
     extern __shared__ __align__(128) unsigned char smem[];
     __shared__ uint64_t bar;
     __shared__ float sW[kMaxFramesPerDraw];
@@ -1210,6 +1243,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
     constexpr bool kStartInDeal = THREADS != TPT_BIG_THREADS;
     const bool pointStart = SRC == kSrcRays && p.pointStart;
     const int* pointIds = p.pointIds;
+    const int* entries = p.entries;
     bool fresh = false;       // the lane has just been dealt an entry (the 768-thread instances' start after the deal)
 
     QPath st;
@@ -1235,7 +1269,8 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             const int ri0 = (int)(pix0 / (uint32_t)p.width), x0 = (int)(pix0 - (uint32_t)ri0 * (uint32_t)p.width);
             const uint32_t fi = s / (uint32_t)p.spp;
             const uint32_t sample = s - fi * (uint32_t)p.spp, frame = (uint32_t)p.frame0 + fi;
-            slabW = invSpp * sW[fi];
+            // tpt_trace_samples: a sample's value is col x weight, weight 1 (rays) or pi (points, set at the start)
+            slabW = SRC == kSrcRays && p.sums ? 1.0f : invSpp * sW[fi];
             slabBand = bandDone ? mtile / mtilesPerBand : 0u;
             __syncwarp();       // every lane has popped what it needed from the previous slab
             if constexpr (SRC == kSrcRays) slabEnd = load_slab_rays(p, sRays[threadIdx.x >> 5], lane, slabEnd, pix0, sample, frame);
@@ -1250,7 +1285,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             if constexpr (SRC == kSrcRays && kStartInDeal)
                 if (pointStart)
                 {
-                    begin_vertex<LS>(sc, st, pointIds ? __ldg(pointIds + tag) : -1);
+                    begin_vertex<LS>(sc, st, point_id(pointIds, entries, tag));
                     st.weight *= TPT_PI;
                 }
             if constexpr (SRC == kSrcRays && !kStartInDeal) fresh = true;
@@ -1258,7 +1293,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if constexpr (SRC == kSrcRays && !kStartInDeal)
             if (pointStart && fresh)
             {
-                begin_vertex<LS>(sc, st, pointIds ? __ldg(pointIds + st.pixOff) : -1);
+                begin_vertex<LS>(sc, st, point_id(pointIds, entries, st.pixOff));
                 st.weight *= TPT_PI;
                 fresh = false;
             }
@@ -1277,7 +1312,14 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
                 if constexpr (MOMENTS)
                     red_add_f4(p.sq4 + (size_t)st.pixOff * 4, st.col.x * st.col.x, st.col.y * st.col.y, st.col.z * st.col.z);
             }
-            else red_add_f4(p.image + (size_t)st.pixOff * 4, st.col.x * st.weight, st.col.y * st.weight, st.col.z * st.weight);
+            else
+            {
+                // the mean's share col / spp, or with p.sums (tpt_trace_samples) the sample v and its count
+                const V3 v = st.col * st.weight;
+                red_add_f4(p.image + (size_t)st.pixOff * 4, v.x, v.y, v.z, SRC == kSrcRays && p.sums ? 1.0f : 0.0f);
+                if constexpr (SRC == kSrcRays)
+                    if (p.sq4) red_add_f4(p.sq4 + (size_t)st.pixOff * 4, v.x * v.x, v.y * v.y, v.z * v.z);
+            }
             st.active = false;
             if (bandDone)
             {
@@ -1364,7 +1406,7 @@ k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, Sce
                                                                   mtilesPerBand, raysOffset, pp);
 }
 
-// tpt_draw_samples' index check: the smallest (entry << 32 | index) of the entries whose index lies outside [0, numPix)
+// The index check of tpt_draw_samples' pixel list and tpt_trace_samples' entry list: the smallest (entry << 32 | index) of the entries whose index lies outside [0, numPix)
 // into *bad, which stays ~0 when there is none.
 __global__ void k_check_pixels(const int* __restrict__ pixels, long long n, long long numPix, unsigned long long* bad)
 {
@@ -2035,9 +2077,10 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     return q;
 }
 
-// regionPix: pixels of the draw's region, tpt_trace_rays' ray count or the length of tpt_draw_samples' list. The
-// accumulation buffer is prepared first: a draw's region blended by the weight of `prev` (k_prepare_image), caller rays'
-// float4 outputs zeroed; tpt_draw_samples adds to the caller's sums as they are.
+// regionPix: pixels of the draw's region, tpt_trace_rays' ray count or the length of tpt_draw_samples' or
+// tpt_trace_samples' list. The accumulation buffer is prepared first: a draw's region blended by the weight of `prev`
+// (k_prepare_image), caller rays' float4 outputs zeroed; tpt_draw_samples and tpt_trace_samples (p.sums) add to the
+// caller's sums as they are.
 template <int SRC>
 static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const DrawParams& p, const SceneDev& sc, int numSMs,
                                 cudaStream_t stream, unsigned int* bandDone, int numBands, unsigned int* bandExpected)
@@ -2051,7 +2094,10 @@ static cudaError_t launch_queue(const QueuePick& q, long long regionPix, const D
     long long grid = 0;
     cudaError_t e = persistent_grid(kern, threads, lay.bytes, numSMs, (slabs + threads / 32 - 1) / (threads / 32), p, stream, grid);
     if (e != cudaSuccess) return e;
-    if constexpr (SRC == kSrcRays) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
+    if constexpr (SRC == kSrcRays)
+    {
+        if (!p.sums) e = cudaMemsetAsync(p.image, 0, (size_t)regionPix * 16, stream);
+    }
     else if constexpr (SRC == kSrcCamera)
     {
         note_launch();
@@ -2131,25 +2177,38 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
     return cudaGetLastError();
 }
 
-cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream)
+// The index check of a caller list of n entries before the trace kernel that reads *badPixel: k_check_pixels against
+// [0, limit).
+static cudaError_t launch_list_check(const int* list, long long n, long long limit, unsigned long long* badPixel, int numSMs,
+                                     cudaStream_t stream)
 {
-    const QueuePick q = pick_queue<kSrcRays>(sc, 3, p.numRays, p.spp, numSMs);
-    return launch_queue<kSrcRays>(q, p.numRays, p, sc, numSMs, stream, nullptr, 0, nullptr);
+    cudaError_t e = cudaMemsetAsync(badPixel, 0xff, sizeof(unsigned long long), stream);
+    if (e != cudaSuccess) return e;
+    const long long blocks = (n + 255) / 256;
+    note_launch();
+    k_check_pixels<<<(unsigned)(blocks < 4LL * numSMs ? blocks : 4LL * numSMs), 256, 0, stream>>>(list, n, limit, badPixel);
+    return cudaGetLastError();
+}
+
+cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, long long numIn, unsigned long long* badPixel, int numSMs,
+                             cudaStream_t stream)
+{
+    DrawParams q = p;
+    if (p.entries)
+    {
+        if (cudaError_t e = launch_list_check(p.entries, p.numRays, numIn, badPixel, numSMs, stream)) return e;
+        q.badPixel = badPixel;
+    }
+    const QueuePick k = pick_queue<kSrcRays>(sc, 3, p.numRays, p.spp, numSMs);
+    return launch_queue<kSrcRays>(k, p.numRays, q, sc, numSMs, stream, nullptr, 0, nullptr);
 }
 
 cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
                                 cudaStream_t stream)
 {
     if (p.pixels)
-    {
-        cudaError_t e = cudaMemsetAsync(badPixel, 0xff, sizeof(unsigned long long), stream);
-        if (e != cudaSuccess) return e;
-        const long long blocks = ((long long)p.numRays + 255) / 256;
-        note_launch();
-        k_check_pixels<<<(unsigned)(blocks < 4LL * numSMs ? blocks : 4LL * numSMs), 256, 0, stream>>>(
-            p.pixels, p.numRays, (long long)p.width * p.height, badPixel);
-        if ((e = cudaGetLastError()) != cudaSuccess) return e;
-    }
+        if (cudaError_t e = launch_list_check(p.pixels, p.numRays, (long long)p.width * p.height, badPixel, numSMs, stream))
+            return e;
     DrawParams q = p;
     q.badPixel = badPixel;
     const QueuePick k = p.sq4 ? pick_queue<kSrcPixels, true>(sc, 3, p.numRays, p.spp, numSMs)

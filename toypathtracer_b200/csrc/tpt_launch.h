@@ -54,7 +54,11 @@ cudaError_t launch_fast(const DrawParams& p, const SceneDev& sc, int variant, in
 // pixel_seed(ray * spp + sample, p.frame0), mean written to the float4 p.image[ray] (zeroed first); p.numFrames = 1, p.flags = 0.
 // Runs the slab-queue instance variant 3 would run for the scene. tpt_trace_irradiance: the same launch with p.pointStart
 // set, p.rays holding surface points {p, n} and p.pointIds their sphere ids (or null); the mean is then scaled by pi.
-cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, int numSMs, cudaStream_t stream);
+// tpt_trace_samples: the same launch with p.sums set, adding (v, 1) and, with p.sq4, (v^2, 0) per sample to the
+// caller's sums (not zeroed), v being the path's radiance (x pi for points); with the list p.entries of p.numRays indices
+// into the numIn inputs, whose check lands in *badPixel (device) as for launch_fast_samples before anything is traced.
+cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, long long numIn, unsigned long long* badPixel, int numSMs,
+                             cudaStream_t stream);
 // tpt_draw_samples: p.spp samples of each of the p.numRays (>= 1) entries of the pixel list p.pixels (null: pixels 0 ..
 // numRays - 1 of the width x height image), sample s of pixel i being the fast draw's camera ray with stream
 // pixel_seed(i * spp + s, p.frame0). Adds (sum of col, spp) to the float4 p.image[entry] and, when p.sq4 is not null,

@@ -116,6 +116,11 @@ struct DrawParams
     // point i lies on (that sphere's light is not sampled from it).
     int pointStart;
     const int* pointIds;
+    // tpt_trace_samples (launch-uniform): with `sums`, image (sum4) and, when set, sq4 get (v, 1) and (v^2, 0) per sample
+    // instead of the mean. entries: null (entry i is input i), or numRays indices into the inputs `rays`, entry k tracing
+    // input entries[k] with that input's streams and ids; checked against the inputs before the launch (badPixel).
+    int sums;
+    const int* entries;
 };
 
 } // namespace tpt
