@@ -58,6 +58,36 @@ const char* tpt_last_error(tpt_context* ctx);
  * wait for it on the device. Bytes identical to the scene already resident are not uploaded again. */
 int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials36, int count,
                   const void* camera88, const int* emissives, int emissiveCount);
+/* Environment lighting for the fast mode: a lat-long (equirectangular) radiance map that replaces the sky. While it is
+ * set, every path of a TPT_MODE_FAST tpt_draw (all fast variants), tpt_trace_rays, tpt_trace_irradiance,
+ * tpt_draw_samples and tpt_trace_samples that leaves the scene adds the map's radiance in its direction instead of the
+ * reference's gradient sky or "mitsuba_compare"'s constant sky ("mitsuba_compare"'s zero Metal roughness still applies).
+ * The map is reached by bounce rays only, like the sky: it is not light-sampled, so "light_sampling" on and off both
+ * stay unbiased. tpt_draw_aovs and tpt_trace_aovs are unaffected (a miss stays zeros and id -1). tpt_draw in
+ * TPT_MODE_EXACT, TPT_MODE_REFGPU and TPT_MODE_REFGPU_FAST is refused while a map is set: those modes reproduce the
+ * reference, which has no environment.
+ *   rgba      width * height float4 texels, row-major, row 0 at the zenith (+y): an image stored top row first is
+ *             upright. Alpha is ignored; R, G and B must be finite and not negative (sign
+ *             bit clear, so -0 is refused too). NULL removes the environment (the calls that
+ *             follow see the reference sky again).
+ *   onDevice  0: host memory; 1: device memory of the context's device, 16-byte aligned, whose contents are complete
+ *             when the call is made (a small kernel checks the texels there).
+ * Refused, with tpt_last_error text: width or height below 1, width * height >= 2^31, a misaligned device buffer or one
+ * on another device, a texel with a negative or non-finite R, G or B (the error names it). A refused map leaves the environment as it was.
+ * The call copies the texels and returns once they have been read, so the caller may free or reuse its buffer; it is a
+ * set-up call that may block. Calls issued before it keep the environment they were issued with, even while in flight,
+ * and calls issued after it see the new one, without any synchronisation by the caller (two device copies, as for the
+ * scene). The environment belongs to the context: tpt_set_scene keeps it, tpt_destroy frees it.
+ * Mapping of a unit direction d (fast module, env_radiance):
+ *   phi = atan2f(d.x, -d.z), theta = acosf(clamp(d.y, -1, 1)),
+ *   u = (phi + pi) / (2 pi) * width, v = theta / pi * height (continuous texel coordinates),
+ *   texel (i, j) has its centre at (i + 1/2, j + 1/2); bilinear filtering, columns wrap, rows clamp; every blend is
+ *   a + f * (b - a), so a constant map returns its constant exactly.
+ * The map's centre column lies along -z (where the reference camera looks), +x to its right: the reference view shows the
+ * map unmirrored
+ * While a map is set, the slab queue runs its 6-CTA instances where it would pick the 8-CTA ones (long draws and caller
+ * calls, "fast_variant" 9): those have no lookup, which would make them spill at 64 registers. */
+int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int height, int onDevice);
 /* Camera only (UpdateTest rebuilds it every frame from the aspect ratio, Test.cpp:341). */
 int tpt_set_camera(tpt_context* ctx, const void* camera88);
 

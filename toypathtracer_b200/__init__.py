@@ -86,6 +86,7 @@ def _load_lib():
     L.tpt_draw_samples.restype = ci
     L.tpt_trace_samples.argtypes = [vp, vp, vp, ci, cll, vp, cll, ci, ci, vp, vp, ci, ctypes.POINTER(cll), vp]
     L.tpt_trace_samples.restype = ci
+    L.tpt_set_environment.argtypes = [vp, vp, ci, ci, ci]; L.tpt_set_environment.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -344,6 +345,46 @@ class Context:
         self._check(self._L.tpt_set_scene(self._h, spheres.ctypes.data, materials.ctypes.data, n,
                                           camera.ctypes.data, ep, ec), "tpt_set_scene")
         self.count = n
+
+    def set_environment(self, image):
+        """tpt_set_environment: light the fast mode with a lat-long radiance map instead of the sky. `image` is an
+        (H, W, 3) or (H, W, 4) float32 numpy array or torch tensor (CPU, or CUDA on the context's device), row 0 at the
+        zenith (an HDR image loaded top row first is upright), the centre column along -z; RGB is padded to RGBA and
+        alpha is ignored. None removes the environment. Refused here: other shapes and dtypes, and negative (-0
+        included) or non-finite RGB values. The texels are copied, and a CUDA tensor is read after torch's current stream has
+        finished writing it. See include/tpt_b200.h for the mapping and which calls use the map."""
+        if image is None:
+            self._check(self._L.tpt_set_environment(self._h, None, 0, 0, 0), "tpt_set_environment")
+            return
+        if not isinstance(image, np.ndarray) and not hasattr(image, "data_ptr"):
+            raise TptError("set_environment: image must be a numpy array or a torch tensor")
+        shape = tuple(image.shape)
+        if len(shape) != 3 or shape[2] not in (3, 4):
+            raise TptError(f"set_environment: image must have shape (H, W, 3) or (H, W, 4), not {shape}")
+        if isinstance(image, np.ndarray):
+            if image.dtype != np.float32:
+                raise TptError(f"set_environment: image must be float32, not {image.dtype}")
+            rgb = image[..., :3]
+            if not np.isfinite(rgb).all() or np.signbit(rgb).any():
+                raise TptError("set_environment: RGB values must be finite and not negative (-0 included)")
+            rgba = np.zeros(shape[:2] + (4,), np.float32)
+            rgba[..., :shape[2]] = image
+            addr, on_dev = rgba.ctypes.data, False
+        else:
+            import torch
+            if image.dtype != torch.float32:
+                raise TptError(f"set_environment: image must be float32, not {image.dtype}")
+            rgb = image[..., :3]
+            if not bool(torch.isfinite(rgb).all()) or bool(torch.signbit(rgb).any()):
+                raise TptError("set_environment: RGB values must be finite and not negative (-0 included)")
+            rgba = torch.zeros(shape[:2] + (4,), dtype=torch.float32, device=image.device)
+            rgba[..., :shape[2]] = image
+            on_dev = bool(rgba.is_cuda)
+            if on_dev:
+                torch.cuda.current_stream(rgba.device).synchronize()   # the library reads it on its own stream
+            addr = int(rgba.data_ptr())
+        self._check(self._L.tpt_set_environment(self._h, ctypes.c_void_p(addr), shape[1], shape[0], 1 if on_dev else 0),
+                    "tpt_set_environment")
 
     def set_camera(self, camera: np.ndarray):
         camera = np.ascontiguousarray(camera)

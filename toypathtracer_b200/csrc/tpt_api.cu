@@ -50,6 +50,17 @@ struct tpt_context
     bool haveScene = false;
     int spp = 4;
 
+    // environment (tpt_set_environment): two device slots with the scene blob's discipline. A new map goes into the slot
+    // that is not current, on the upload stream after that slot's last use; calls wait on the current slot's upload and
+    // mark its last use. It belongs to the context, not to the scene: tpt_set_scene leaves it alone.
+    Q4* dEnv[2] = {nullptr, nullptr};
+    size_t envCap[2] = {0, 0};
+    int curEnv = 1;                               // the first map goes into slot 0
+    bool haveEnv = false;
+    int envW = 0, envH = 0;                       // of the current slot
+    cudaEvent_t envUploadDone[2] = {nullptr, nullptr};
+    cudaEvent_t envLastUse[2] = {nullptr, nullptr};
+
     // options
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
     int fastKForm = 2;        // 0: reference-form sweep, 1: expanded form, 2: expanded form on the pair array (slab queue: in the
@@ -179,6 +190,16 @@ __global__ void k_tonemap_rgba8(const float4* __restrict__ img, int width, int h
 }
 } // namespace tpt
 
+// tpt_set_environment's channel rule: finite with the sign bit clear. As an int32, such a float lies in [0, +Inf's bits):
+// negative values (-0 included) are below, +Inf and NaN at or above. The device check runs the list check on these ints.
+static const long long kEnvBitsLimit = 0x7f800000LL;
+static bool env_channel_ok(float v)
+{
+    int32_t b;
+    memcpy(&b, &v, 4);
+    return b >= 0 && b < kEnvBitsLimit;
+}
+
 extern "C" {
 
 int tpt_device_count(void)
@@ -212,6 +233,8 @@ int tpt_create(int device, tpt_context** out)
     {
         e = cudaEventCreateWithFlags(&ctx->uploadDone[i], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->blobLastUse[i], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->envUploadDone[i], cudaEventDisableTiming);
+        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->envLastUse[i], cudaEventDisableTiming);
     }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->lastDraw, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->forkEvent, cudaEventDisableTiming);
@@ -255,6 +278,9 @@ void tpt_destroy(tpt_context* ctx)
         if (ctx->hBlob[i]) cudaFreeHost(ctx->hBlob[i]);
         if (ctx->uploadDone[i]) cudaEventDestroy(ctx->uploadDone[i]);
         if (ctx->blobLastUse[i]) cudaEventDestroy(ctx->blobLastUse[i]);
+        cudaFree(ctx->dEnv[i]);
+        if (ctx->envUploadDone[i]) cudaEventDestroy(ctx->envUploadDone[i]);
+        if (ctx->envLastUse[i]) cudaEventDestroy(ctx->envLastUse[i]);
     }
     if (ctx->uploadStream) cudaStreamDestroy(ctx->uploadStream);
     if (ctx->lastDraw) cudaEventDestroy(ctx->lastDraw);
@@ -417,6 +443,17 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
     if (ctx->haveLastDraw && ctx->lastDrawStream != *stream) CK(cudaStreamWaitEvent(*stream, ctx->lastDraw, 0), "order after previous draw");
     CK(cudaStreamWaitEvent(*stream, ctx->uploadDone[ctx->curBlob], 0), "wait for scene upload");
     *scene = ctx->scene;
+    if (ctx->haveEnv)
+    {
+        // the call reads the environment that is current now, in its slot, once that slot's upload has landed
+        CK(cudaStreamWaitEvent(*stream, ctx->envUploadDone[ctx->curEnv], 0), "wait for environment upload");
+        const uint64_t env = (uint64_t)(uintptr_t)ctx->dEnv[ctx->curEnv];
+        scene->layout.flags |= kSceneEnvironment;
+        scene->layout.envLo = (uint32_t)env;
+        scene->layout.envHi = (uint32_t)(env >> 32);
+        scene->layout.envW = ctx->envW;
+        scene->layout.envH = ctx->envH;
+    }
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
     scene->pairs.half = scene->halfOk && scene->kformOk && ctx->fastKForm == 2;
@@ -466,6 +503,7 @@ static int finish_call(tpt_context* ctx, cudaStream_t stream, int n, bool hostBu
 {
     CK(cudaEventRecord(ctx->lastDraw, stream), "draw end event");
     CK(cudaEventRecord(ctx->blobLastUse[ctx->curBlob], stream), "scene last-use event");
+    if (ctx->haveEnv) CK(cudaEventRecord(ctx->envLastUse[ctx->curEnv], stream), "environment last-use event");
     ctx->lastDrawStream = stream; ctx->haveLastDraw = true;
     if (outRayCount || outPerFrame)
     {
@@ -780,6 +818,10 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
         return fail_msg(ctx, "tpt_draw: bad arguments");
     if (mode != TPT_MODE_EXACT && mode != TPT_MODE_FAST && mode != TPT_MODE_REFGPU && mode != TPT_MODE_REFGPU_FAST)
         return fail_msg(ctx, "tpt_draw: unknown mode");
+    // the parity modes reproduce the reference, which has no environment to be bit-identical to
+    if (mode != TPT_MODE_FAST && ctx->haveEnv)
+        return fail_msg(ctx, "tpt_draw: an environment is set, and only TPT_MODE_FAST draws use one (clear it with "
+                             "tpt_set_environment(ctx, NULL, 0, 0, 0) for exact and reference-GPU draws)");
     // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
     if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
@@ -1071,6 +1113,71 @@ int tpt_draw_samples(tpt_context* ctx, int frame, int width, int height,
     if (pixels && *ctx->hBadPixel != ~0ull)
         return fail_msgf(ctx, "tpt_draw_samples: pixels[%llu] = %d is outside the %d x %d image (nothing was traced)",
                          *ctx->hBadPixel >> 32, (int)(uint32_t)*ctx->hBadPixel, width, height);
+    return 0;
+}
+
+int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int height, int onDevice)
+{
+    static const char* fn = "tpt_set_environment";
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    // NULL: the calls issued from now on see the reference sky; those in flight keep reading their slot
+    if (!rgba) { ctx->haveEnv = false; return 0; }
+    if (width < 1 || height < 1) return fail_msgf(ctx, "%s: width and height must be >= 1 (got %d x %d)", fn, width, height);
+    const long long n = (long long)width * height;
+    if (n >= (1LL << 31)) return fail_msgf(ctx, "%s: width * height must be below 2^31 (got %lld)", fn, n);
+    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+    if (onDevice)
+    {
+        if ((uintptr_t)rgba & 15) return fail_msgf(ctx, "%s: device rgba is not 16-byte aligned", fn);
+        if (int r = check_device_buffer(ctx, fn, rgba, "rgba")) return r;
+        if (int r = ensure_index_check(ctx)) return r;
+    }
+    else
+        for (long long i = 0; i < n; ++i)
+            for (int c = 0; c < 3; ++c)
+                if (!env_channel_ok(rgba[4 * i + c]))
+                    return fail_msgf(ctx, "%s: texel %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative",
+                                     fn, i, i % width, i / width, c == 0 ? "R" : c == 1 ? "G" : "B", rgba[4 * i + c]);
+    // The slot that is not current: the calls issued since the last tpt_set_environment read the other one. The upload
+    // waits on the device for the slot's last reader (issued before the previous tpt_set_environment).
+    const int slot = ctx->curEnv ^ 1;
+    const size_t bytes = (size_t)n * 16;
+    if (bytes > ctx->envCap[slot])
+    {
+        CK(cudaEventSynchronize(ctx->envLastUse[slot]), "sync before environment realloc");
+        cudaFree(ctx->dEnv[slot]); ctx->dEnv[slot] = nullptr; ctx->envCap[slot] = 0;
+        CK(cudaMalloc(&ctx->dEnv[slot], bytes), "cudaMalloc environment");
+        ctx->envCap[slot] = bytes;
+    }
+    cudaStream_t s = ctx->uploadStream;
+    CK(cudaStreamWaitEvent(s, ctx->envLastUse[slot], 0), "environment upload waits for the slot's readers");
+    if (onDevice)
+    {
+        // R, G and B of every texel packed into the slot's first 12 n bytes, then checked as 3 n int32 in [0, +Inf's bits)
+        // by the caller-list check (entry = channel index); the texels themselves are copied over them afterwards
+        CK(cudaMemcpy2DAsync(ctx->dEnv[slot], 12, rgba, 16, 12, (size_t)n, cudaMemcpyDefault, s), "pack environment RGB");
+        CK(launch_list_check((const int*)ctx->dEnv[slot], 3 * n, kEnvBitsLimit, ctx->dBadPixel, ctx->numSMs, s),
+           "environment check launch");
+        CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s), "D2H environment check");
+    }
+    CK(cudaMemcpyAsync(ctx->dEnv[slot], rgba, bytes, onDevice ? cudaMemcpyDefault : cudaMemcpyHostToDevice, s), "environment upload");
+    CK(cudaEventRecord(ctx->envUploadDone[slot], s), "environment upload event");
+    // A set-up call: it returns once the caller's texels have been read (the caller may then free or reuse its buffer) and,
+    // for a device map, checked. A refused map leaves the current environment as it was.
+    CK(cudaStreamSynchronize(s), "environment upload sync");
+    if (onDevice && *ctx->hBadPixel != ~0ull)
+    {
+        const long long k = (long long)(*ctx->hBadPixel >> 32), i = k / 3;
+        uint32_t bits = (uint32_t)*ctx->hBadPixel;
+        float v;
+        memcpy(&v, &bits, 4);
+        return fail_msgf(ctx, "%s: texel %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative", fn, i,
+                         i % width, i / width, k % 3 == 0 ? "R" : k % 3 == 1 ? "G" : "B", v);
+    }
+    ctx->curEnv = slot;
+    ctx->haveEnv = true;
+    ctx->envW = width;
+    ctx->envH = height;
     return 0;
 }
 

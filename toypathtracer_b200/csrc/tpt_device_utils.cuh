@@ -106,6 +106,10 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     v.nLights = nLights;
     v.flags = L.flags;
     v.sphShared = smem_u32(smemBase + L.offSph);   // geometry is always inside the staged prefix
+    v.envLo = L.envLo;
+    v.envHi = L.envHi;
+    v.envW = L.envW;
+    v.envH = L.envH;
     return v;
 }
 

@@ -922,9 +922,48 @@ __device__ __forceinline__ V3 metal_dir(V3 d, V3 normal, float roughness, uint32
     return M<false>::normalize(refl);
 }
 
+// Radiance of tpt_set_environment's lat-long map in the unit direction d (include/tpt_b200.h pins the mapping):
+// phi = atan2(d.x, -d.z), theta = acos(d.y); continuous texel coordinates u = (phi + pi) / 2pi * W, v = theta / pi * H,
+// texel (i, j) centred at (i + 1/2, j + 1/2), row 0 at the zenith; bilinear, columns wrapping, rows clamped. Every blend is
+// a + f * (b - a), so a constant map returns its constant bit for bit. Four 128-bit read-only loads.
+__device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d)
+{
+    constexpr float kPi = 3.14159265358979f;
+    const int W = sc.envW, H = sc.envH;
+    const float phi = atan2f(d.x, -d.z);
+    const float theta = acosf(fminf(fmaxf(d.y, -1.0f), 1.0f));
+    const float u = (phi + kPi) * (0.5f / kPi) * (float)W - 0.5f;
+    const float v = theta * (1.0f / kPi) * (float)H - 0.5f;
+    const float fu = floorf(u), fv = floorf(v);
+    const float tu = u - fu, tv = v - fv;
+    int x0 = (int)fu, y0 = (int)fv;                  // x0 in [-1, W - 1] up to rounding, y0 in [-1, H - 1]
+    x0 = x0 < 0 ? x0 + W : (x0 >= W ? x0 - W : x0);
+    x0 = min(max(x0, 0), W - 1);                     // a non-finite d converts to 0: any texel, never out of bounds
+    const int x1 = x0 + 1 == W ? 0 : x0 + 1;
+    const int y1 = min(max(y0 + 1, 0), H - 1);
+    y0 = min(max(y0, 0), H - 1);
+    const float4* env = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
+    const float4* row0 = env + (size_t)y0 * W;
+    const float4* row1 = env + (size_t)y1 * W;
+    const float4 a = __ldg(row0 + x0), b = __ldg(row0 + x1), c = __ldg(row1 + x0), e = __ldg(row1 + x1);
+    auto lerp = [](float p, float q, float f) { return p + f * (q - p); };
+    const V3 top = v3(lerp(a.x, b.x, tu), lerp(a.y, b.y, tu), lerp(a.z, b.z, tu));
+    const V3 bot = v3(lerp(c.x, e.x, tu), lerp(c.y, e.y, tu), lerp(c.z, e.z, tu));
+    return v3(lerp(top.x, bot.x, tv), lerp(top.y, bot.y, tv), lerp(top.z, bot.z, tv));
+}
+
+// What a fast path sees when it leaves the scene: the caller's environment while one is set, else the reference sky
+// (sky() stays the exact and reference-GPU kernels' own, untouched).
+__device__ __forceinline__ V3 fast_sky(V3 d, const SceneView& sc)
+{
+    return (sc.flags & kSceneEnvironment) ? env_radiance(sc, d) : sky(d, sc);
+}
+
 // One iteration of the per-lane path state machine every fast kernel shades with: intersect the lane's current ray
 // (path or shadow) against all spheres, then shade. Returns true when the lane's path has ended (st.col is final).
-template <int LS, class Hitter>
+// ENV = false: the miss sees the reference sky only (the slab queue's 64-register 8-CTA instances, which a lookup made
+// spill; pick_queue does not choose them while an environment is set).
+template <int LS, bool ENV = true, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
@@ -940,7 +979,12 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
     {
         if (LS == kLsOff || st.kind == 0)
         {
-            if (id < 0) { st.col = st.col + st.thr * sky(st.d, sc); finished = true; }
+            if (id < 0)
+            {
+                if constexpr (ENV) st.col = st.col + st.thr * fast_sky(st.d, sc);
+                else st.col = st.col + st.thr * sky(st.d, sc);
+                finished = true;
+            }
             else
             {
                 Q4 s = ld_sph(sc, id);
@@ -1186,7 +1230,7 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
 // MOMENTS, (col^2, 0) to p.sq4[entry].
 enum QueueSource { kSrcCamera = 0, kSrcRays = 1, kSrcPixels = 2 };
-template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false>
+template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false, bool ENV = true>
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
@@ -1304,7 +1348,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if (exhausted) { if (!trDry) trDry = gtimer(); ++trDryTrips; trDryLanes += (unsigned)__popc(__ballot_sync(0xffffffffu, st.active)); }
 #endif
 
-        if (path_step<LS>(sc, st, rc, hitter))
+        if (path_step<LS, ENV>(sc, st, rc, hitter))
         {
             if constexpr (SRC == kSrcPixels)
             {
@@ -1350,7 +1394,7 @@ k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
              uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
              uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcCamera, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // DO_LIGHT_SAMPLING 0 (scene flag kSceneNoLightSampling): the same kernel without the light-sampling half of the state
@@ -1361,7 +1405,7 @@ k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, Scene
                      uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                      uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcCamera, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_trace_rays: the slab queue on caller rays (RAYS = true), with the same launch shapes as k_fast_queue and the
@@ -1372,7 +1416,7 @@ k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
             uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 template <int THREADS, int MINB, int KFORM>
@@ -1381,7 +1425,7 @@ k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneB
                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                     uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_draw_samples: the slab queue on a pixel list (SRC = kSrcPixels), per-entry sums and, with MOMENTS, sums of squares.
@@ -1392,7 +1436,7 @@ k_fast_samples(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLa
                uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                  mtilesPerBand, raysOffset, pp);
 }
 
@@ -1402,7 +1446,7 @@ k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, Sce
                        uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone,
                        uint32_t mtilesPerBand, uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                   mtilesPerBand, raysOffset, pp);
 }
 
@@ -1823,7 +1867,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                     uint32_t rng = __float_as_uint(fthr.w);
                     const V3 d = v3(fdd.x, fdd.y, fdd.z);
                     const bool doMatE = (m2 >> 24) & 1;
-                    if (T == WT_MISS) { col = col + thr * sky(d, sc); finished = true; }
+                    if (T == WT_MISS) { col = col + thr * fast_sky(d, sc); finished = true; }
                     else if (T == WT_SHADOW)
                     {
                         const int j = (m2 & 0xffff) - 1;
@@ -2048,7 +2092,8 @@ struct QueuePick
 // x 4 warps with a copy each). Long launches (many slabs per warp) run 8 CTAs of 64 registers per SM instead of 6 of 80
 // (the same rule for form 4: at 720p x 4 spp its 8-CTA instance is 3 % slower than the 6-CTA one);
 // short ones keep 6, where a warp only gets ~12 slabs and the drain of the last ones weighs more with more warps. Variant
-// 9 forces the 8-CTA instance (A/B runs).
+// 9 forces the 8-CTA instance (A/B runs). While an environment is set the 6-CTA instances run instead (the 8-CTA ones
+// have no lookup).
 template <int SRC, bool MOMENTS = false>
 static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix, long long samples, int numSMs)
 {
@@ -2063,15 +2108,16 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     const bool big = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, q.kform), 4 * 2048).bytes > 36 * 1024 ||
                      sc.stagedBytes != sc.layout.totalBytes;
     const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
+    // the 8-CTA instances have no environment lookup (at 64 registers it made them spill): with one set, the 6-CTA ones run
+    const bool eight = !(sc.layout.flags & kSceneEnvironment) && (variant == 9 || (variant == 3 && slabsPerWarp >= 48));
     q.threads = big ? TPT_BIG_THREADS : 128;
     if (big) q.kern = queue_kernel<SRC, MOMENTS, TPT_BIG_THREADS, 1>(sc, q.kform);
     else if (q.kform == 4)
     {
         if constexpr (SRC != kSrcPixels)
-            q.kern = variant == 9 || (variant == 3 && slabsPerWarp >= 48) ? queue_instance<SRC, MOMENTS, 128, 8, 4>(sc)
-                                                                          : queue_instance<SRC, MOMENTS, 128, 6, 4>(sc);
+            q.kern = eight ? queue_instance<SRC, MOMENTS, 128, 8, 4>(sc) : queue_instance<SRC, MOMENTS, 128, 6, 4>(sc);
     }
-    else if (q.kform == 2 && (variant == 9 || (variant == 3 && slabsPerWarp >= 48))) q.kern = queue_instance<SRC, MOMENTS, 128, 8, 2>(sc);
+    else if (q.kform == 2 && eight) q.kern = queue_instance<SRC, MOMENTS, 128, 8, 2>(sc);
     else if (SRC == kSrcCamera && variant == 4) q.kern = queue_kernel<kSrcCamera, false, 128, 7>(sc, q.kform);
     else q.kern = queue_kernel<SRC, MOMENTS, 128, TPT_QUEUE_MINB>(sc, q.kform);
     return q;
@@ -2179,8 +2225,8 @@ cudaError_t launch_debug_hit(const SceneDev& sc, int kform, const float* dRays, 
 
 // The index check of a caller list of n entries before the trace kernel that reads *badPixel: k_check_pixels against
 // [0, limit).
-static cudaError_t launch_list_check(const int* list, long long n, long long limit, unsigned long long* badPixel, int numSMs,
-                                     cudaStream_t stream)
+cudaError_t launch_list_check(const int* list, long long n, long long limit, unsigned long long* badPixel, int numSMs,
+                              cudaStream_t stream)
 {
     cudaError_t e = cudaMemsetAsync(badPixel, 0xff, sizeof(unsigned long long), stream);
     if (e != cudaSuccess) return e;

@@ -67,6 +67,11 @@ cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, long long 
 // is traced. Runs the slab-queue instance variant 3 would run for the scene.
 cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
                                 cudaStream_t stream);
+// The check of n int32 `list` against [0, limit) that the caller lists get before their trace kernel: the smallest
+// (entry << 32 | value) of an entry outside lands in *bad (device; ~0 when there is none). tpt_set_environment checks a
+// device map's channels with it, as their bits.
+cudaError_t launch_list_check(const int* list, long long n, long long limit, unsigned long long* bad, int numSMs,
+                              cudaStream_t stream);
 // tpt_draw_aovs (rays = false: the region of p, frames [p.frame0, p.frame0 + p.numFrames) at p.spp, blended over the outputs
 // with the weight of `prev`) and tpt_trace_aovs (rays = true: p.numRays >= 1 caller rays p.rays): first-hit albedo4,
 // normal4 and ids (each may be null) with the slab queue's sweep form, one ray counted per traced sample.

@@ -26,6 +26,8 @@ inline SceneBlobLayout scene_blob_layout(int count, int nLights)
     L.offMatRi = off;      off += align16((uint32_t)(count + 1) * 4u);
     L.totalBytes = off;
     L.flags = 0;
+    L.envLo = L.envHi = 0;
+    L.envW = L.envH = 0;
     return L;
 }
 
@@ -173,6 +175,8 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.nLights = sampled_lights(L.flags, nLights);
     v.flags = L.flags;
     v.sphShared = 0;
+    v.envLo = v.envHi = 0;     // host views never look up an environment
+    v.envW = v.envH = 0;
     return v;
 }
 

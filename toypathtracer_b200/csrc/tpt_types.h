@@ -47,6 +47,8 @@ struct SceneView
     int count, simdCount, nLights;
     uint32_t flags;       // kScene* bits
     uint32_t sphShared;   // device: 32-bit shared-memory address of sph[] (always staged), for ld.shared.v4
+    uint32_t envLo, envHi; // kSceneEnvironment: address of the envW x envH RGBA texels of the lat-long environment (row 0 =
+    int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it
 };
 
 // Blob layout in global memory (one contiguous, 16 B-aligned allocation so a single bulk copy stages it
@@ -57,6 +59,11 @@ struct SceneBlobLayout
     uint32_t offSph, offMatA, offMatB, offLights, offInvRadius, offMatRi, totalBytes;
     uint32_t geomBytes; // bytes of [sph .. end] needed by intersection + lights only (== totalBytes here)
     uint32_t flags;     // kScene* bits (travels to the kernels with the layout)
+    // tpt_set_environment's map (kSceneEnvironment): its device address as two 32-bit halves, which keeps the struct 4-byte
+    // aligned (an 8-byte aligned kernel parameter changes how the compiler loads the fields around it), and its size.
+    // Not part of the blob: each call's copy of the layout gets them (begin_call).
+    uint32_t envLo, envHi;
+    int envW, envH;
 };
 
 // DO_MITSUBA_COMPARE (Config.h:25) as a runtime switch: constant sky (Test.cpp:226-227) and zero Metal roughness
@@ -66,7 +73,9 @@ struct SceneBlobLayout
 // draws, no shadow rays, Test.cpp:95-133) and the emission of every hit is added (the doMaterialE suppression of
 // Test.cpp:209-215 is compiled out there). The kernels see it as a light count of 0 (sampled_lights()) plus the
 // emission rule (emission_after_lambert()).
-enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u };
+// An environment set with tpt_set_environment: a lat-long radiance map replaces the sky at the fast kernels' miss sites
+// (fast_sky) for the calls issued while it is set; the mitsuba constant sky included, its zero Metal roughness not.
+enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u };
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.

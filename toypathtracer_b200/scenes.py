@@ -54,6 +54,17 @@ def camera_rays(camera, width: int, height: int, per_pixel: int = 1, seed: int =
     return np.concatenate([cam["origin"] + offset, d], axis=1).astype(np.float32)
 
 
+def sky_environment(width: int, height: int) -> np.ndarray:
+    """The reference's gradient sky (Test.cpp:228-231: 0.3 * lerp(white, (0.5, 0.7, 1.0), (d.y + 1) / 2)) as a lat-long
+    map for Context.set_environment: an (height, width, 3) float32 array, texel (i, j) holding the sky at its centre,
+    theta = (j + 1/2) / height * pi from the zenith (d.y = cos theta; the sky does not depend on phi). Computed in
+    float64. With it the fast mode reproduces the default look up to the map's bilinear error."""
+    theta = (np.arange(height, dtype=np.float64) + 0.5) / height * np.pi
+    t = 0.5 * (np.cos(theta) + 1.0)
+    col = ((1.0 - t)[:, None] * np.ones(3) + t[:, None] * np.array([0.5, 0.7, 1.0])) * 0.3
+    return np.ascontiguousarray(np.broadcast_to(col[:, None, :], (height, width, 3)), dtype=np.float32)
+
+
 def reference_scene(width: int, height: int, time: float = 0.0, flags: int = 0, big_scene: bool = True,
                     mitsuba_compare: bool = False):
     """(spheres, materials, camera, emissives) of the reference scene at this aspect ratio, produced by the
