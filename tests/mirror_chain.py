@@ -361,7 +361,8 @@ def oracle_scene(count, layout):
 
 
 # ---- coverage table: every __global__ kernel of libtpt_b200.so (as toypathtracer_b200.kernel_signature names it), and
-# the check of test_gpu_mirror_chains.py that ties it to an exact multi-bounce answer, or why it is left out ---------------
+# the check of test_gpu_mirror_chains.py that ties it to an exact multi-bounce answer, or why it is left out. The fast
+# (k_fast_*) instances it drives are also each tied to the sample replay by test_gpu_sample_replay.py ----------------------
 _Q = [(128, 6, 0), (128, 6, 1), (128, 6, 2), (128, 6, 3), (128, 6, 4), (128, 8, 2), (128, 8, 4),
       (768, 1, 0), (768, 1, 1), (768, 1, 2), (768, 1, 3)]
 _S = [(128, 6, 0), (128, 6, 1), (128, 6, 2), (128, 6, 3), (128, 8, 2), (768, 1, 0), (768, 1, 1), (768, 1, 2), (768, 1, 3)]
