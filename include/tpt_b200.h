@@ -62,8 +62,9 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
  * set, every path of a TPT_MODE_FAST tpt_draw (all fast variants), tpt_trace_rays, tpt_trace_irradiance,
  * tpt_draw_samples and tpt_trace_samples that leaves the scene adds the map's radiance in its direction instead of the
  * reference's gradient sky or "mitsuba_compare"'s constant sky ("mitsuba_compare"'s zero Metal roughness still applies).
- * The map is reached by bounce rays only, like the sky: it is not light-sampled, so "light_sampling" on and off both
- * stay unbiased. tpt_draw_aovs and tpt_trace_aovs are unaffected (a miss stays zeros and id -1). tpt_draw in
+ * By default the map is reached by bounce rays only, like the sky, so "light_sampling" on and off both stay unbiased;
+ * "environment_sampling" (tpt_set_option) adds an importance-sampled direction towards it at Lambert vertices, for which
+ * this call also builds the map's sampling tables. tpt_draw_aovs and tpt_trace_aovs are unaffected (a miss stays zeros and id -1). tpt_draw in
  * TPT_MODE_EXACT, TPT_MODE_REFGPU and TPT_MODE_REFGPU_FAST is refused while a map is set: those modes reproduce the
  * reference, which has no environment.
  *   rgba      width * height float4 texels, row-major, row 0 at the zenith (+y): an image stored top row first is
@@ -84,7 +85,10 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
  *   texel (i, j) has its centre at (i + 1/2, j + 1/2); bilinear filtering, columns wrap, rows clamp; every blend is
  *   a + f * (b - a), so a constant map returns its constant exactly.
  * The map's centre column lies along -z (where the reference camera looks), +x to its right: the reference view shows the
- * map unmirrored
+ * map unmirrored.
+ * Memory: each of the two device copies holds the texels and the sampling tables behind them, 24 * width * height +
+ * 8 * height bytes (the texels' alpha carries each cell's sampling probability; toypathtracer_b200/csrc/tpt_env_tables.h
+ * pins the tables).
  * While a map is set, the slab queue runs its 6-CTA instances where it would pick the 8-CTA ones (long draws and caller
  * calls, "fast_variant" 9): those have no lookup, which would make them spill at 64 registers. */
 int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int height, int onDevice);
@@ -134,7 +138,20 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * tpt_set_scene: no explicit light sampling at Lambert vertices (no light draws, no shadow rays, Test.cpp:95-133) and
  * every hit adds its emission (the doMaterialE suppression of Test.cpp:209-215 is off). Exact and reference-GPU strict
  * modes stay bit-identical to the reference built that way. The flag is part of the scene: toggling it re-uploads the
- * scene and invalidates the exact_lookahead cache). */
+ * scene and invalidates the exact_lookahead cache),
+ * "environment_sampling" (default 0; any non-zero value is 1: fast calls importance-sample tpt_set_environment's map at
+ * light-sampled Lambert vertices. After the light cones, such a vertex draws one direction from the map's tables
+ * (proportional to sin theta times the brightest texel the bilinear filter can blend into each cell) and traces its
+ * shadow ray, and the vertex's bounce, when it leaves the scene, is weighted against it with the power heuristic. An
+ * estimator switch like "light_sampling", not a speed path: both are unbiased and their outputs differ. Read by each
+ * call when it is issued, like the map, not a scene flag: toggling it uploads nothing. Active for a call only with the
+ * option on, a map set, "light_sampling" on and a map with some non-zero weight; a call where it is not active runs
+ * exactly as without it. While active: only the slab queue's reference-form (sweep form 0) instances sample, and every
+ * fast call runs them (measured: the sampling code in the packed-sweep instances cost map-less draws 20 %); tpt_draw's
+ * auto variant is 3 (never 7 or 8;
+ * host-buffer draws stage through the slab queue instead of storing into page-locked memory), 9 runs the 6-CTA
+ * instance, and an explicit "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused; Metal and glass vertices, Lambert
+ * vertices hit from inside their sphere, the AOV calls and the exact and reference-GPU modes do not sample it). */
 int tpt_set_option(tpt_context* ctx, const char* key, int value);
 
 /* Replaces DrawTest() (Test.cpp:344-367) for frames [frameCount, frameCount+numFrames) — numFrames*spp samples

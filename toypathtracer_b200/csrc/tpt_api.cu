@@ -5,6 +5,7 @@
 #include "tpt_scene_pack.h"
 #include "tpt_device_utils.cuh"
 #include "tpt_integrator.cuh"
+#include "tpt_env_tables.h"
 #include <cuda.h>      // types only: cuStreamWaitValue32 is resolved at run time (cudaGetDriverEntryPoint), libcuda is not linked
 #include <string>
 #include <vector>
@@ -58,6 +59,8 @@ struct tpt_context
     int curEnv = 1;                               // the first map goes into slot 0
     bool haveEnv = false;
     int envW = 0, envH = 0;                       // of the current slot
+    bool envSampleable = false;                   // the current slot's map has sampling tables (some weight is not zero)
+    int envSampling = 0;                          // "environment_sampling"
     cudaEvent_t envUploadDone[2] = {nullptr, nullptr};
     cudaEvent_t envLastUse[2] = {nullptr, nullptr};
 
@@ -414,6 +417,7 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     if (!strcmp(key, "fast_alpha_zero")) { ctx->fastAlphaZero = value ? 1 : 0; return 0; }
     if (!strcmp(key, "scene_upload_always")) { ctx->sceneUploadAlways = value ? 1 : 0; return 0; }
     if (!strcmp(key, "mitsuba_compare")) { ctx->sceneFlags = value ? (ctx->sceneFlags | kSceneMitsuba) : (ctx->sceneFlags & ~(uint32_t)kSceneMitsuba); return 0; }
+    if (!strcmp(key, "environment_sampling")) { ctx->envSampling = value ? 1 : 0; return 0; }
     if (!strcmp(key, "light_sampling")) { ctx->sceneFlags = value ? (ctx->sceneFlags & ~(uint32_t)kSceneNoLightSampling) : (ctx->sceneFlags | kSceneNoLightSampling); return 0; }
     if (!strcmp(key, "host_progress")) { ctx->hostProgress = value ? 1 : 0; return 0; }
     if (!strcmp(key, "host_zero_copy")) { ctx->hostZeroCopy = value ? 1 : 0; return 0; }
@@ -453,6 +457,9 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
         scene->layout.envHi = (uint32_t)(env >> 32);
         scene->layout.envW = ctx->envW;
         scene->layout.envH = ctx->envH;
+        // "environment_sampling" is read here, per call, like the map: not a scene flag, so toggling it uploads nothing
+        if (ctx->envSampling && ctx->envSampleable && !(scene->layout.flags & kSceneNoLightSampling))
+            scene->layout.flags |= kSceneEnvSampling;
     }
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
@@ -828,6 +835,12 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
+    // only the slab queue's 6-CTA and 768-thread instances sample the environment
+    const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
+    if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).samplesEnvironment)
+        return fail_msgf(ctx, "tpt_draw: \"environment_sampling\" is active (option on, a map with non-zero weight, light "
+                              "sampling on), and fast_variant %d does not sample the environment: use -1 (auto), 3 or 9",
+                         ctx->fastVariant);
 
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);
@@ -838,7 +851,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     // being traced — no staging image, no device-to-host copy after the kernel.
     bool zeroCopy = false;
     cudaPointerAttributes attr{};
-    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy &&
+    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && !envSampling &&
         (ctx->fastVariant < 0 || fast_variant_info(ctx->fastVariant).writesFinalPixels))
     {
         zeroCopy = prevWeight == 0.0f && numFrames <= kMaxFramesPerDraw && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
@@ -1140,8 +1153,10 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
                                      fn, i, i % width, i / width, c == 0 ? "R" : c == 1 ? "G" : "B", rgba[4 * i + c]);
     // The slot that is not current: the calls issued since the last tpt_set_environment read the other one. The upload
     // waits on the device for the slot's last reader (issued before the previous tpt_set_environment).
+    // The slot holds the texels, each cell's sampling probability in their alpha, and the alias tables behind them
+    // (tpt_env_tables.h): 24 W H + 8 H bytes, built here on the host.
     const int slot = ctx->curEnv ^ 1;
-    const size_t bytes = (size_t)n * 16;
+    const size_t bytes = env_slot_bytes(width, height);
     if (bytes > ctx->envCap[slot])
     {
         CK(cudaEventSynchronize(ctx->envLastUse[slot]), "sync before environment realloc");
@@ -1151,31 +1166,40 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
     }
     cudaStream_t s = ctx->uploadStream;
     CK(cudaStreamWaitEvent(s, ctx->envLastUse[slot], 0), "environment upload waits for the slot's readers");
+    std::vector<float> host((bytes + 3) / 4);
+    float* tex = host.data();
     if (onDevice)
     {
         // R, G and B of every texel packed into the slot's first 12 n bytes, then checked as 3 n int32 in [0, +Inf's bits)
-        // by the caller-list check (entry = channel index); the texels themselves are copied over them afterwards
+        // by the caller-list check (entry = channel index), and copied back for the table build
         CK(cudaMemcpy2DAsync(ctx->dEnv[slot], 12, rgba, 16, 12, (size_t)n, cudaMemcpyDefault, s), "pack environment RGB");
         CK(launch_list_check((const int*)ctx->dEnv[slot], 3 * n, kEnvBitsLimit, ctx->dBadPixel, ctx->numSMs, s),
            "environment check launch");
         CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s), "D2H environment check");
+        CK(cudaMemcpy2DAsync(tex, 16, ctx->dEnv[slot], 12, 12, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H environment RGB");
+        // A refused map leaves the current environment as it was.
+        CK(cudaStreamSynchronize(s), "environment check sync");
+        if (*ctx->hBadPixel != ~0ull)
+        {
+            const long long k = (long long)(*ctx->hBadPixel >> 32), i = k / 3;
+            uint32_t bits = (uint32_t)*ctx->hBadPixel;
+            float v;
+            memcpy(&v, &bits, 4);
+            return fail_msgf(ctx, "%s: texel %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative", fn, i,
+                             i % width, i / width, k % 3 == 0 ? "R" : k % 3 == 1 ? "G" : "B", v);
+        }
     }
-    CK(cudaMemcpyAsync(ctx->dEnv[slot], rgba, bytes, onDevice ? cudaMemcpyDefault : cudaMemcpyHostToDevice, s), "environment upload");
+    else
+        memcpy(tex, rgba, (size_t)n * 16);
+    EnvAlias* rows = reinterpret_cast<EnvAlias*>(tex + 4 * n);
+    const bool sampleable = env_build_tables(tex, width, height, rows, rows + height);
+    CK(cudaMemcpyAsync(ctx->dEnv[slot], tex, bytes, cudaMemcpyHostToDevice, s), "environment upload");
     CK(cudaEventRecord(ctx->envUploadDone[slot], s), "environment upload event");
-    // A set-up call: it returns once the caller's texels have been read (the caller may then free or reuse its buffer) and,
-    // for a device map, checked. A refused map leaves the current environment as it was.
+    // A set-up call: it returns once the caller's texels have been read (the caller may then free or reuse its buffer).
     CK(cudaStreamSynchronize(s), "environment upload sync");
-    if (onDevice && *ctx->hBadPixel != ~0ull)
-    {
-        const long long k = (long long)(*ctx->hBadPixel >> 32), i = k / 3;
-        uint32_t bits = (uint32_t)*ctx->hBadPixel;
-        float v;
-        memcpy(&v, &bits, 4);
-        return fail_msgf(ctx, "%s: texel %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative", fn, i,
-                         i % width, i / width, k % 3 == 0 ? "R" : k % 3 == 1 ? "G" : "B", v);
-    }
     ctx->curEnv = slot;
     ctx->haveEnv = true;
+    ctx->envSampleable = sampleable;
     ctx->envW = width;
     ctx->envH = height;
     return 0;

@@ -890,28 +890,6 @@ __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 n
     return m * omega * (1.0f / TPT_PI);
 }
 
-// The rest of a Lambert vertex after its shadow ray towards light lightFrom - 1 (or, lightFrom = 0, after the vertex's
-// own shading): the next light the vertex samples, its cone and shadow ray, or, when none is left, the bounce along
-// st.nextDir with throughput st.thrAlb. Without light sampling (kLsOff) there are no lights to sample: the bounce.
-template <int LS>
-__device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom)
-{
-    const int j = LS == kLsOff ? sc.nLights : next_light(sc, lightFrom, st.mid);
-    if (j < sc.nLights)
-    {
-        st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
-        st.kind = 1 + j;
-    }
-    else
-    {
-        st.d = st.nextDir;
-        st.thr = st.thrAlb;
-        st.kind = 0;
-        st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
-        ++st.depth;
-    }
-}
-
 // Metal bounce direction (Test.cpp:137-150); the path goes on when dot(result, normal) > 0. With roughness == 0 the
 // unit-sphere sample has zero weight, so the fast mode skips drawing it (the exact mode must draw it: it advances the
 // shared RNG stream).
@@ -926,7 +904,10 @@ __device__ __forceinline__ V3 metal_dir(V3 d, V3 normal, float roughness, uint32
 // phi = atan2(d.x, -d.z), theta = acos(d.y); continuous texel coordinates u = (phi + pi) / 2pi * W, v = theta / pi * H,
 // texel (i, j) centred at (i + 1/2, j + 1/2), row 0 at the zenith; bilinear, columns wrapping, rows clamped. Every blend is
 // a + f * (b - a), so a constant map returns its constant bit for bit. Four 128-bit read-only loads.
-__device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d)
+// CELL: also the sampling probability P of the cell [i, i+1) x [j, j+1) that holds (u + 1/2, v + 1/2), from the alpha of
+// whichever of the four texels that is (tpt_env_tables.h).
+template <bool CELL = false>
+__device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d, float* cellP = nullptr)
 {
     constexpr float kPi = 3.14159265358979f;
     const int W = sc.envW, H = sc.envH;
@@ -947,6 +928,7 @@ __device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d)
     const float4* row1 = env + (size_t)y1 * W;
     const float4 a = __ldg(row0 + x0), b = __ldg(row0 + x1), c = __ldg(row1 + x0), e = __ldg(row1 + x1);
     auto lerp = [](float p, float q, float f) { return p + f * (q - p); };
+    if constexpr (CELL) *cellP = tv < 0.5f ? (tu < 0.5f ? a.w : b.w) : (tu < 0.5f ? c.w : e.w);
     const V3 top = v3(lerp(a.x, b.x, tu), lerp(a.y, b.y, tu), lerp(a.z, b.z, tu));
     const V3 bot = v3(lerp(c.x, e.x, tu), lerp(c.y, e.y, tu), lerp(c.z, e.z, tu));
     return v3(lerp(top.x, bot.x, tv), lerp(top.y, bot.y, tv), lerp(top.z, bot.z, tv));
@@ -959,11 +941,108 @@ __device__ __forceinline__ V3 fast_sky(V3 d, const SceneView& sc)
     return (sc.flags & kSceneEnvironment) ? env_radiance(sc, d) : sky(d, sc);
 }
 
+// ---- environment sampling ("environment_sampling", kSceneEnvSampling; tpt_env_tables.h pins tables, draws, density)
+constexpr float kEnvPdfScale = 1.0f / (2.0f * TPT_PI * TPT_PI);      // pdf_e = P * W * H / (2 pi^2 sin theta)
+constexpr int kKindEnv = -1;                                         // QPath::kind of an environment sample's shadow ray
+
+// Power-heuristic weight of a bounce against the environment sampler, pdf_b^2 / (pdf_b^2 + pdf_e^2); 1 where the sampler
+// has no density (pdf_e zero or not a number: P = 0 at a pole).
+__device__ __forceinline__ float env_bounce_weight(float pb, float pe)
+{
+    const float b2 = pb * pb, e2 = pe * pe;
+    return e2 > 0.0f ? b2 / (b2 + e2) : 1.0f;
+}
+
+// One environment sample at a Lambert vertex whose bounce is cosine-distributed about nl: six draws (row, row alias test,
+// column, column alias test, in-cell u and v offsets), the direction into l, and true when its shadow ray is traced
+// (c = l.nl > 0 and sin theta > 0), with pend = (c / pi) pdf_e / (pdf_e^2 + pdf_b^2), pdf_b = c / pi: the ray adds
+// thrAlb * L(l) * pend when it leaves the scene. The tables are read through the read-only path.
+__device__ __forceinline__ bool sample_env(const SceneView& sc, V3 nl, uint32_t& rng, V3& l, float& pend)
+{
+    const uint32_t W = (uint32_t)sc.envW, H = (uint32_t)sc.envH;
+    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
+    const float2* rows = reinterpret_cast<const float2*>(tex + (size_t)W * H);
+    const float2* cols = rows + H;
+    uint32_t j = __umulhi((XorShift32(rng) & 0xFFFFFFu) << 8, H);          // (k * H) >> 24
+    const float2 er = __ldg(rows + j);
+    if (!(RandomFloat01(rng) < er.x)) j = (uint32_t)__float_as_int(er.y);
+    const float2* crow = cols + (size_t)j * W;
+    uint32_t i = __umulhi((XorShift32(rng) & 0xFFFFFFu) << 8, W);
+    const float2 ec = __ldg(crow + i);
+    if (!(RandomFloat01(rng) < ec.x)) i = (uint32_t)__float_as_int(ec.y);
+    const float P = __ldg(&tex[(size_t)j * W + i].w);
+    const float u = (float)i + RandomFloat01(rng);
+    const float v = (float)j + RandomFloat01(rng);
+    const float fW = (float)W, fH = (float)H;
+    float sp, cp, s, c;
+    __sincosf(__fdividef(u, fW) * (2.0f * TPT_PI) - TPT_PI, &sp, &cp);
+    __sincosf(__fdividef(v, fH) * TPT_PI, &s, &c);
+    l = v3(s * sp, c, -s * cp);
+    const float cn = dot(l, nl);
+    if (!(cn > 0.0f && s > 0.0f)) return false;
+    const float pe = P * (fW * fH * kEnvPdfScale) / s;
+    const float pb = cn * (1.0f / TPT_PI);
+    pend = pb * pe / (pe * pe + pb * pb);
+    return true;
+}
+
+// The miss of a path in the sampling instances: fast_sky's radiance, and for the bounce of a Lambert vertex that took an
+// environment sample (doMaterialE false, pend = the bounce's pdf_b >= 0) that radiance times env_bounce_weight. Camera
+// rays, Metal and glass bounces (doMaterialE true) and vertices without a sample (pend -1) keep full weight.
+__device__ __forceinline__ V3 fast_sky_mis(const SceneView& sc, const QPath& st)
+{
+    if (!(sc.flags & kSceneEnvSampling)) return fast_sky(st.d, sc);
+    float P;
+    const V3 L = env_radiance<true>(sc, st.d, &P);
+    if (st.doMaterialE || !(st.pend >= 0.0f)) return L;
+    const float s = M<false>::sqrt_(fmaxf(fmaf(-st.d.y, st.d.y, 1.0f), 0.0f));
+    const float pe = P * ((float)sc.envW * (float)sc.envH * kEnvPdfScale) / s;
+    return L * env_bounce_weight(st.pend, pe);
+}
+
+// The rest of a Lambert vertex after its shadow ray towards light lightFrom - 1 (or, lightFrom = 0, after the vertex's
+// own shading): the next light the vertex samples, its cone and shadow ray, or, when none is left, the bounce along
+// st.nextDir with throughput st.thrAlb. Without light sampling (kLsOff) there are no lights to sample: the bounce.
+// ENVM 2 with kSceneEnvSampling: after the lights (lightFrom <= nLights), one environment sample at a vertex hit from
+// outside (st.doMaterialE, path_step) and its shadow ray, which comes back with lightFrom = nLights + 1; then the
+// bounce, which keeps its pdf_b in pend for its miss (fast_sky_mis), or -1 where the vertex took no sample.
+template <int LS, int ENVM = 1>
+__device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom)
+{
+    const int j = LS == kLsOff ? sc.nLights : next_light(sc, lightFrom, st.mid);
+    if (j < sc.nLights)
+    {
+        st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
+        st.kind = 1 + j;
+    }
+    else
+    {
+        bool envSampled = false;
+        if constexpr (ENVM == 2)
+        {
+            envSampled = (sc.flags & kSceneEnvSampling) && st.doMaterialE;
+            if (envSampled && lightFrom <= sc.nLights && sample_env(sc, st.nl, st.rng, st.d, st.pend))
+            {
+                st.kind = kKindEnv;
+                return;
+            }
+        }
+        st.d = st.nextDir;
+        st.thr = st.thrAlb;
+        st.kind = 0;
+        if constexpr (ENVM == 2) st.pend = envSampled ? fmaxf(dot(st.nextDir, st.nl), 0.0f) * (1.0f / TPT_PI) : -1.0f;
+        st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
+        ++st.depth;
+    }
+}
+
 // One iteration of the per-lane path state machine every fast kernel shades with: intersect the lane's current ray
 // (path or shadow) against all spheres, then shade. Returns true when the lane's path has ended (st.col is final).
-// ENV = false: the miss sees the reference sky only (the slab queue's 64-register 8-CTA instances, which a lookup made
-// spill; pick_queue does not choose them while an environment is set).
-template <int LS, bool ENV = true, class Hitter>
+// ENVM, the environment mode: 0 the miss sees the reference sky only (the slab queue's 64-register 8-CTA instances, which
+// a lookup made spill; pick_queue does not choose them while an environment is set); 1 fast_sky; 2 fast_sky plus, where
+// the call's kSceneEnvSampling is set, environment sampling at light-sampled Lambert vertices (the slab queue's 6-CTA and
+// 768-thread light-sampling instances).
+template <int LS, int ENVM = 1, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
@@ -981,7 +1060,8 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         {
             if (id < 0)
             {
-                if constexpr (ENV) st.col = st.col + st.thr * fast_sky(st.d, sc);
+                if constexpr (ENVM == 2) st.col = st.col + st.thr * fast_sky_mis(sc, st);
+                else if constexpr (ENVM == 1) st.col = st.col + st.thr * fast_sky(st.d, sc);
                 else st.col = st.col + st.thr * sky(st.d, sc);
                 finished = true;
             }
@@ -1011,6 +1091,9 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     st.nextDir = M<false>::normalize(target);
                     st.thrAlb = st.thr * mat.albedo;
                     st.nl = dot(normal, st.d) < 0.0f ? normal : neg(normal);
+                    // until the bounce, doMaterialE says whether the vertex takes an environment sample: only when hit from
+                    // outside, where the bounce's axis (normal) is nl
+                    if constexpr (ENVM == 2) st.doMaterialE = dot(normal, st.d) < 0.0f;
                     st.mid = mid;
                     st.o = pos;
                     wantLight = true; lightFrom = 0;
@@ -1042,6 +1125,12 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 }
             }
         }
+        else if (ENVM == 2 && st.kind == kKindEnv)
+        {
+            // the environment sample's shadow ray (sample_env); after it, the bounce
+            if (id < 0) st.col = st.col + (st.thrAlb * env_radiance(sc, st.d)) * st.pend;
+            wantLight = true; lightFrom = sc.nLights + 1;
+        }
         else
         {
             const int j = st.kind - 1;
@@ -1050,7 +1139,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             wantLight = true; lightFrom = j + 1;
         }
     }
-    if (LS != kLsOff && wantLight) lambert_next<LS>(sc, st, lightFrom);
+    if (LS != kLsOff && wantLight) lambert_next<LS, ENVM>(sc, st, lightFrom);
     return finished;
 }
 
@@ -1058,14 +1147,14 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
 // Lambert vertex at p whose facing normal is n, as if a camera ray had just hit it: the bounce direction drawn first, then
 // lambert_next picks the first light (or the bounce). No emission of its own (doMaterialE is not looked at before the
 // next hit); depth 0, so the path keeps a camera path's budget. `mid`: the sphere the point lies on, or -1.
-template <int LS>
+template <int LS, int ENVM = 1>
 __device__ __forceinline__ void begin_vertex(const SceneView& sc, QPath& st, int mid)
 {
     st.nl = st.d;
     st.nextDir = M<false>::normalize(st.d + RandomUnitVector<false>(st.rng));
     st.thrAlb = v3(1, 1, 1);
     st.mid = mid;
-    lambert_next<LS>(sc, st, 0);
+    lambert_next<LS, ENVM>(sc, st, 0);     // (begin_path left doMaterialE true: the point takes an environment sample)
 }
 
 // The sphere id of point entry `tag` (tpt_trace_irradiance, tpt_trace_samples): ids are per input, so an entry of a list
@@ -1230,7 +1319,7 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
 // MOMENTS, (col^2, 0) to p.sq4[entry].
 enum QueueSource { kSrcCamera = 0, kSrcRays = 1, kSrcPixels = 2 };
-template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false, bool ENV = true>
+template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false, int ENVM = 1>
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
@@ -1329,7 +1418,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             if constexpr (SRC == kSrcRays && kStartInDeal)
                 if (pointStart)
                 {
-                    begin_vertex<LS>(sc, st, point_id(pointIds, entries, tag));
+                    begin_vertex<LS, ENVM>(sc, st, point_id(pointIds, entries, tag));
                     st.weight *= TPT_PI;
                 }
             if constexpr (SRC == kSrcRays && !kStartInDeal) fresh = true;
@@ -1337,7 +1426,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if constexpr (SRC == kSrcRays && !kStartInDeal)
             if (pointStart && fresh)
             {
-                begin_vertex<LS>(sc, st, point_id(pointIds, entries, st.pixOff));
+                begin_vertex<LS, ENVM>(sc, st, point_id(pointIds, entries, st.pixOff));
                 st.weight *= TPT_PI;
                 fresh = false;
             }
@@ -1348,7 +1437,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if (exhausted) { if (!trDry) trDry = gtimer(); ++trDryTrips; trDryLanes += (unsigned)__popc(__ballot_sync(0xffffffffu, st.active)); }
 #endif
 
-        if (path_step<LS, ENV>(sc, st, rc, hitter))
+        if (path_step<LS, ENVM>(sc, st, rc, hitter))
         {
             if constexpr (SRC == kSrcPixels)
             {
@@ -1388,13 +1477,21 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
 #endif
 }
 
+// path_step's environment mode of a light-sampling slab-queue instance with MINB CTAs per SM and sweep form KFORM: the
+// reference-form (KFORM 0) 6-CTA and 768-thread instances sample the environment (pick_queue runs them while it is
+// sampled), the other 6-CTA, 768-thread and 7-CTA ones only look it up, the 8-CTA ones have no lookup. Measured on an
+// H100 (700 W): the sampling code in the packed-sweep instance bench.py runs (k_fast_queue<128, 6, 4>) cost its
+// map-less 720p draw 20 % (23 200 -> 18 400 Mray/s) at the same 80 registers and no stack, so it is kept out of the
+// instances the default sweep forms run.
+__host__ __device__ constexpr int env_mode(int minb, int kform) { return minb == 8 ? 0 : minb == 7 || kform != 0 ? 1 : 2; }
+
 template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
 k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
              uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
              uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcCamera, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcCamera, false, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // DO_LIGHT_SAMPLING 0 (scene flag kSceneNoLightSampling): the same kernel without the light-sampling half of the state
@@ -1405,7 +1502,7 @@ k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, Scene
                      uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                      uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcCamera, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcCamera, false, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_trace_rays: the slab queue on caller rays (RAYS = true), with the same launch shapes as k_fast_queue and the
@@ -1416,7 +1513,7 @@ k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
             uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays, false, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 template <int THREADS, int MINB, int KFORM>
@@ -1425,7 +1522,7 @@ k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneB
                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                     uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays, false, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays, false, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_draw_samples: the slab queue on a pixel list (SRC = kSrcPixels), per-entry sums and, with MOMENTS, sums of squares.
@@ -1436,7 +1533,7 @@ k_fast_samples(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLa
                uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                  mtilesPerBand, raysOffset, pp);
 }
 
@@ -1446,7 +1543,7 @@ k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, Sce
                        uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone,
                        uint32_t mtilesPerBand, uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS, MINB != 8>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                   mtilesPerBand, raysOffset, pp);
 }
 
@@ -2099,6 +2196,9 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
 {
     QueuePick q;
     q.kform = fast_queue_kform(sc);
+    // the environment-sampling instances sweep in the reference form (env_mode)
+    const bool envSampling = (sc.layout.flags & kSceneEnvSampling) != 0;
+    if (envSampling) q.kform = 0;
     // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
     // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2). The same
     // instances run form 5 (the half-precision pass 1) when the parameter says so (sc.pairs.half, begin_call).
@@ -2400,7 +2500,7 @@ int fast_slab_pixels() { return kSlabPix; }
 FastVariantInfo fast_variant_info(int variant)
 {
     const bool queue = variant == 3 || variant == 4 || variant == 9;
-    return {variant == 8, queue || (variant >= 5 && variant <= 7), queue};
+    return {variant == 8, queue || (variant >= 5 && variant <= 7), queue, variant == 3 || variant == 9};
 }
 
 // The block wavefront (variants 6/7) indexes its paths in 31 bits, over whole 128-pixel slabs (tail pixels are skipped),
@@ -2411,12 +2511,14 @@ static bool wave_fits(const SceneDev& sc, long long regionPix, long long S)
     return wave_paths(regionPix, S) <= 0x7fffffffLL && sc.nLights < kKindFree;
 }
 
-// The slab queue (3), except: a draw into mapped host memory runs the group queue (8), which stores its finished pixels
+// The slab queue (3), always while the environment is sampled (tpt_draw then never stores into mapped host memory),
+// except: a draw into mapped host memory runs the group queue (8), which stores its finished pixels
 // itself; and where the sweep dwarfs everything else (>= 1024 spheres) and the slab queue cannot run a packed-pair sweep
 // (pair array does not fit, or "fast_kform" < 2), the block wavefront that sorts its paths by material before Scatter()
 // is faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312).
 int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy)
 {
+    if (sc.layout.flags & kSceneEnvSampling) return 3;       // the slab queue alone samples the environment
     if (zeroCopy) return 8;
     const long long S = (long long)spp * (numFrames < kMaxFramesPerDraw ? numFrames : kMaxFramesPerDraw);   // first launch
     return sc.count >= 1024 && fast_queue_kform(sc) < 2 && wave_fits(sc, regionPix, S) ? 7 : 3;

@@ -39,6 +39,7 @@ struct FastVariantInfo
     bool writesFinalPixels;   // the trace kernel stores finished pixels itself (no L2 reductions), also into mapped host memory
     bool rowBands;            // a draw can be split into row bands, one launch per band
     bool progressCounters;    // the trace kernel can publish per-band completion counters (launch_fast's bandDone)
+    bool samplesEnvironment;  // runs the slab queue's environment-sampling instances ("environment_sampling")
 };
 FastVariantInfo fast_variant_info(int variant);
 // The variant a draw with "fast_variant" -1 runs over regionPix pixels of numFrames frames at spp; zeroCopy: the draw

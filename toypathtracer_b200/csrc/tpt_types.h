@@ -48,7 +48,8 @@ struct SceneView
     uint32_t flags;       // kScene* bits
     uint32_t sphShared;   // device: 32-bit shared-memory address of sph[] (always staged), for ld.shared.v4
     uint32_t envLo, envHi; // kSceneEnvironment: address of the envW x envH RGBA texels of the lat-long environment (row 0 =
-    int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it
+    int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it; its sampling tables follow
+                           // the texels (tpt_env_tables.h)
 };
 
 // Blob layout in global memory (one contiguous, 16 B-aligned allocation so a single bulk copy stages it
@@ -75,7 +76,10 @@ struct SceneBlobLayout
 // emission rule (emission_after_lambert()).
 // An environment set with tpt_set_environment: a lat-long radiance map replaces the sky at the fast kernels' miss sites
 // (fast_sky) for the calls issued while it is set; the mitsuba constant sky included, its zero Metal roughness not.
-enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u };
+// kSceneEnvSampling ("environment_sampling" active for the call, set by begin_call with kSceneEnvironment): the slab
+// queue's sampling instances take one environment sample per light-sampled Lambert vertex (sample_env), with the map's
+// tables behind its texels (tpt_env_tables.h).
+enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u };
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.
