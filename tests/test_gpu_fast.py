@@ -86,15 +86,16 @@ def same_sample_draws(ctx, light_sampling):
 def test_variants_trace_the_same_samples(gpu_ctx, light_sampling):
     """Every variant shades with path_step, so on the same streams and sweep form they trace the same paths: only FMA
     contraction, which differs between kernel instances, can flip a decision now and then. Measured against variant 3 on
-    an H100 80GB HBM3 (700 W): relL2 <= 1.4e-7 and equal ray counts, except variants 6/7 without light sampling, relL2
-    8.3e-6 and 5.3e-8 more rays (about 3 rays in 5e7). The bars, 1e-4 and 1e-6, are ~12x and ~19x those. Copies of the
-    estimator that draw or weigh samples differently land above them: measured 8.8e-4 for a wavefront with its own
-    light-cone basis, 2e-2 and 4e-5 fewer rays for variants 0-2 with their own light and roughness sampling."""
+    an H100 80GB HBM3 (700 W): relL2 <= 1.4e-7 and equal ray counts for every variant, light sampling on and off. The
+    bars, 2e-6 and 1e-7, are ~14x the image figure and about 5 rays in the 5e7 of a draw. Copies of the estimator that
+    draw or weigh samples differently land above the image bar: measured 8.3e-6 (and 5.3e-8 more rays without light
+    sampling) for a wavefront with its own copy of the shading, 8.8e-4 for one with its own light-cone basis, 2e-2 and
+    4e-5 fewer rays for variants 0-2 with their own light and roughness sampling."""
     out = same_sample_draws(gpu_ctx, light_sampling)
     ref, ref_rays = out[3]
     for v, (img, rays) in out.items():
-        assert rel_l2(img, ref) <= 1e-4, (v, rel_l2(img, ref))
-        assert abs(rays / ref_rays - 1) <= 1e-6, (v, rays, ref_rays)
+        assert rel_l2(img, ref) <= 2e-6, (v, rel_l2(img, ref))
+        assert abs(rays / ref_rays - 1) <= 1e-7, (v, rays, ref_rays)
 
 
 def test_variants_and_sharding_consistent(gpu_ctx):

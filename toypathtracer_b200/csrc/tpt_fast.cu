@@ -4,8 +4,8 @@
 // same rays/sample), not bitwise — bitwise parity is the exact mode's job (tpt_exact.cu).
 //
 // The estimator is written once, as path_step (one step of a per-lane path state machine on a QPath): every variant and
-// entry point shades with it, and the block wavefront (variants 6/7) calls its pieces phase by phase. The variants differ
-// in how they deal work and write pixels:
+// entry point shades with it; the block wavefront (variants 6/7) runs its last part, lambert_next, in a phase of its own.
+// The variants differ in how they deal work and write pixels:
 // variant 0  "megakernel": one thread per pixel, loops over frames x spp with one stream per pixel and frame (what
 //            the reference's own GPU shaders do, Cpp/Windows/ComputeShader.hlsl:353-395). Baseline for the
 //            persistent design.
@@ -1042,7 +1042,9 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // a lookup made spill; pick_queue does not choose them while an environment is set); 1 fast_sky; 2 fast_sky plus, where
 // the call's kSceneEnvSampling is set, environment sampling at light-sampled Lambert vertices (the slab queue's 6-CTA and
 // 768-thread light-sampling instances).
-template <int LS, int ENVM = 1, class Hitter>
+// NEXT false: stop before lambert_next, for a caller that runs it later (the block wavefront). A Lambert vertex just shaded
+// and a returning shadow ray then leave the light to go on from in st.kind.
+template <int LS, int ENVM = 1, bool NEXT = true, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
@@ -1139,7 +1141,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
             wantLight = true; lightFrom = j + 1;
         }
     }
-    if (LS != kLsOff && wantLight) lambert_next<LS, ENVM>(sc, st, lightFrom);
+    if (NEXT && LS != kLsOff && wantLight) lambert_next<LS, ENVM>(sc, st, lightFrom);
     return finished;
 }
 
@@ -1789,27 +1791,79 @@ k_fast_tileq(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
 
 // ---- variant 6 ------------------------------------------------------------------------------------------------
 // "block wavefront": the persistent design of the north star taken literally. A CTA keeps kWaveSlots path slots in
-// SHARED memory (9 float4 per slot) and runs every iteration in three phases separated by block barriers:
+// SHARED memory (a QPath and the hit of its last sweep, 8 float4 per slot) and runs every iteration in four phases
+// separated by block barriers:
 //   sweep     thread i regenerates slot i if it is free (next path of the CTA's chunk) and intersects slot i's
 //             ray (path or shadow) against all spheres -> every lane has a ray, no divergence outside pass 2;
 //   sort      the slot is classified {miss, lambert, metal, dielectric, shadow-return, terminal} and appended to
 //             that type's index list with warp __ballot_sync + prefix popcount (one shared atomic per warp per type);
-//   scatter   the lists are cut into 32-entry chunks and dealt to the warps: every warp shades entries of ONE
-//             material type (Scatter(), Test.cpp:83-193, without divergence); Lambert vertices and returning
-//             shadow rays append themselves to the light list, processed the same way in a third phase
-//             (explicit light sampling, Test.cpp:96-133).
-// The shading is path_step's, phase by phase: the same metal bounce, light choice and light-cone sample, and the same
-// scalar shadow-ray weight. Radiance leaves through the same 128-bit vector reductions as variant 3.
+//   scatter   the lists are cut into 32-entry chunks and dealt to the warps: every warp runs path_step on the stored
+//             hits of ONE type, so it takes one branch of Scatter() (Test.cpp:83-193) without divergence; Lambert
+//             vertices and returning shadow rays append themselves to the light list;
+//   light     lambert_next for every slot on the light list: its next shadow ray or its bounce (explicit light
+//             sampling, Test.cpp:96-133).
+// So the shading is path_step's, with its lambert_next in a phase of its own: inlined into the scatter phase, where the
+// slot's QPath and the chunk walk are live, it made the 64-register instance spill. Radiance leaves through the same
+// 128-bit vector reductions as variant 3.
 constexpr int kWaveThreads = 256;
 constexpr int kWaveSlots = 256;        // one slot per thread
-constexpr int kWaveFields = 9;
+constexpr int kWaveFields = 8;
 constexpr int kWaveChunk = 4096;       // paths taken from the global counter at a time
-// WF_NL.w: the weight m * omega / pi of the slot's shadow ray in flight (QPath::pend)
-enum { WF_O = 0, WF_D, WF_THR, WF_COL, WF_NEXT, WF_THRALB, WF_NL, WF_POS, WF_NRM };
+// A slot's fields: the path's {o, rng} {d, state word} {thr, pend} {col, -}; its Lambert vertex's {nextDir, mid}
+// {thrAlb, -} {nl, -}; and {t, id} of the hit its last sweep found, with the path's {pixOff, weight}, which regeneration
+// writes and a finished path reads.
+enum { WF_O = 0, WF_D, WF_THR, WF_COL, WF_NEXT, WF_THRALB, WF_NL, WF_HIT };
 enum { WT_MISS = 0, WT_LAMBERT, WT_METAL, WT_DIEL, WT_SHADOW, WT_TERMINAL, WT_COUNT };
 // a slot's state word (WF_D.w): bits 0-15 kind (0 path ray, 1 + j shadow ray of light j, kKindFree), bits 16-23 depth,
 // bit 24 doMaterialE. The launcher refuses nLights >= kKindFree.
 constexpr int kKindFree = 0xffff;
+constexpr unsigned kWavePath = 1u << WF_O | 1u << WF_D | 1u << WF_THR | 1u << WF_COL;
+constexpr unsigned kWaveVertex = 1u << WF_NEXT | 1u << WF_THRALB | 1u << WF_NL;
+
+// The QPath fields held by the slot's fields in `fields` (bit f: field f); the others are left undefined. Each phase loads
+// only what it reads and stores only what it writes: a field loaded and stored back unchanged stays live in a register
+// through the shading, and k_fast_wave<4> has none to spare.
+__device__ __forceinline__ QPath wave_load(const float4* pool, int slot, unsigned fields)
+{
+    const float4* f = pool + slot;
+    QPath st;
+    st.active = true;
+    if (fields & 1u << WF_O) { const float4 v = f[WF_O * kWaveSlots]; st.o = v3(v.x, v.y, v.z); st.rng = __float_as_uint(v.w); }
+    if (fields & 1u << WF_D)
+    {
+        const float4 v = f[WF_D * kWaveSlots];
+        const int w = __float_as_int(v.w);
+        st.d = v3(v.x, v.y, v.z);
+        st.kind = w & 0xffff; st.depth = (w >> 16) & 0xff; st.doMaterialE = (w >> 24) & 1;
+    }
+    if (fields & 1u << WF_THR) { const float4 v = f[WF_THR * kWaveSlots]; st.thr = v3(v.x, v.y, v.z); st.pend = v.w; }
+    if (fields & 1u << WF_COL) { const float4 v = f[WF_COL * kWaveSlots]; st.col = v3(v.x, v.y, v.z); }
+    if (fields & 1u << WF_NEXT) { const float4 v = f[WF_NEXT * kWaveSlots]; st.nextDir = v3(v.x, v.y, v.z); st.mid = __float_as_int(v.w); }
+    if (fields & 1u << WF_THRALB) { const float4 v = f[WF_THRALB * kWaveSlots]; st.thrAlb = v3(v.x, v.y, v.z); }
+    if (fields & 1u << WF_NL) { const float4 v = f[WF_NL * kWaveSlots]; st.nl = v3(v.x, v.y, v.z); }
+    return st;
+}
+__device__ __forceinline__ void wave_store(float4* pool, int slot, const QPath& st, unsigned fields)
+{
+    float4* f = pool + slot;
+    if (fields & 1u << WF_O) f[WF_O * kWaveSlots] = make_float4(st.o.x, st.o.y, st.o.z, __uint_as_float(st.rng));
+    if (fields & 1u << WF_D)
+        f[WF_D * kWaveSlots] = make_float4(st.d.x, st.d.y, st.d.z, __int_as_float(st.kind | st.depth << 16 | (int)st.doMaterialE << 24));
+    if (fields & 1u << WF_THR) f[WF_THR * kWaveSlots] = make_float4(st.thr.x, st.thr.y, st.thr.z, st.pend);
+    if (fields & 1u << WF_COL) f[WF_COL * kWaveSlots] = make_float4(st.col.x, st.col.y, st.col.z, 0.0f);
+    if (fields & 1u << WF_NEXT) f[WF_NEXT * kWaveSlots] = make_float4(st.nextDir.x, st.nextDir.y, st.nextDir.z, __int_as_float(st.mid));
+    if (fields & 1u << WF_THRALB) f[WF_THRALB * kWaveSlots] = make_float4(st.thrAlb.x, st.thrAlb.y, st.thrAlb.z, 0.0f);
+    if (fields & 1u << WF_NL) f[WF_NL * kWaveSlots] = make_float4(st.nl.x, st.nl.y, st.nl.z, 0.0f);
+}
+__device__ __forceinline__ void wave_free(float4* pool, int slot) { pool[WF_D * kWaveSlots + slot].w = __int_as_float(kKindFree); }
+
+// The hitter of the scatter phase: the hit the sweep phase stored for the slot.
+struct StoredHit
+{
+    int id;
+    float t;
+    __device__ __forceinline__ int hit(const SceneView&, V3, V3, float, float, float& tOut) const { tOut = t; return id; }
+};
 
 struct WaveArgs
 {
@@ -1833,18 +1887,17 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
     __shared__ int sExhausted, sLive;
     stage_blob(smem, blob, stagedBytes, &bar);
     float4* pool = reinterpret_cast<float4*>(smem + poolOffset);
-#define WFLD(f, slot) pool[(f) * kWaveSlots + (slot)]
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const unsigned ltMask = (1u << lane) - 1u;
     if (tid == 0)
     {
         float wp; blend_weights(p, sW, wp);
+        for (int fi = 0; fi < p.numFrames; ++fi) sW[fi] *= 1.0f / (float)p.spp;     // the weight of one path of frame fi
         sNextPath = 0; sEndPath = 0; sExhausted = 0; sLive = 0; sLightCount = 0;
         for (int t = 0; t < WT_COUNT; ++t) sCount[t] = 0;
     }
-    WFLD(WF_D, tid) = make_float4(0, 0, 0, __int_as_float(kKindFree));
+    wave_free(pool, tid);
     SceneView sc = make_view(smem, blob, L, stagedBytes, count, nLights);
-    const float invSpp = 1.0f / (float)p.spp;
     SerialHitter<false> hitter;
     unsigned rc = 0;
     __syncthreads();
@@ -1866,18 +1919,17 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         __syncthreads();
 
         // ---- phase 1: regenerate own slot if free, then sweep
-        float4 fd = WFLD(WF_D, tid);
-        int misc = __float_as_int(fd.w);
-        int kind = misc & 0xffff;
+        int type = -1;
         {
-            const unsigned need = __ballot_sync(0xffffffffu, kind == kKindFree);
+            QPath st = wave_load(pool, tid, 1u << WF_O | 1u << WF_D);
+            const unsigned need = __ballot_sync(0xffffffffu, st.kind == kKindFree);
             if (need)
             {
                 uint32_t base = 0;
                 if (lane == 0) base = atomicAdd(&sNextPath, (uint32_t)__popc(need));
                 base = __shfl_sync(0xffffffffu, base, 0);
                 const uint32_t idx = base + (uint32_t)__popc(need & ltMask);
-                if (kind == kKindFree && idx < sEndPath)
+                if (st.kind == kKindFree && idx < sEndPath)
                 {
                     const uint32_t slab = idx >> 7, q = idx & 127u;
                     const uint32_t mtile = fdiv(slab, wa.divS), s = slab - mtile * wa.S;
@@ -1889,39 +1941,29 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                         const uint32_t fi = fdiv(s, wa.divSpp), ss = s - fi * (uint32_t)p.spp;
                         const int y = p.row0 + (int)ri * p.rowStep;
                         uint32_t rng = pixel_seed((uint32_t)(y * p.width + (int)x) * (uint32_t)p.spp + ss, (uint32_t)p.frame0 + fi);
-                        Ray r = fast_camera_ray(p, (int)x, y, rng);
-                        kind = 0; misc = 0 | (0 << 16) | (1 << 24);
-                        fd = make_float4(r.dir.x, r.dir.y, r.dir.z, __int_as_float(misc));
-                        WFLD(WF_O, tid) = make_float4(r.orig.x, r.orig.y, r.orig.z, 0.0f);
-                        WFLD(WF_D, tid) = fd;
-                        WFLD(WF_THR, tid) = make_float4(1, 1, 1, __uint_as_float(rng));
-                        WFLD(WF_COL, tid) = make_float4(0, 0, 0, __uint_as_float((uint32_t)((p.packed ? (int)ri : y) * p.width + (int)x)));
-                        WFLD(WF_NEXT, tid) = make_float4(0, 0, 0, invSpp * sW[fi]);
+                        const Ray r = fast_camera_ray(p, (int)x, y, rng);
+                        st = QPath{};
+                        begin_path(st, r, rng);
+                        wave_store(pool, tid, st, kWavePath);
+                        float4& h = pool[WF_HIT * kWaveSlots + tid];
+                        h.z = __uint_as_float((uint32_t)((p.packed ? (int)ri : y) * p.width + (int)x));    // pixOff
+                        h.w = sW[fi];                                                                       // weight
                     }
                 }
             }
-        }
-        int type = -1;
-        if (kind != kKindFree)
-        {
-            const float4 fo = WFLD(WF_O, tid);
-            const V3 o = v3(fo.x, fo.y, fo.z), d = v3(fd.x, fd.y, fd.z);
-            float t;
-            const int id = hitter.hit(sc, o, d, TPT_MIN_T, TPT_MAX_T, t);
-            ++rc;
-            if (kind != 0) { type = WT_SHADOW; WFLD(WF_POS, tid).w = __int_as_float(id); }
-            else if (id < 0) type = WT_MISS;
-            else
+            if (st.kind != kKindFree)
             {
-                const Q4 s = ld_sph(sc, id);
-                const V3 pos = o + d * t;
-                const V3 normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];
-                const int mid = id < sc.count ? id : sc.count;
-                const int depth = (misc >> 16) & 0xff;
-                const int mtype = f_as_i(sc.matA[mid].w);
-                type = depth >= TPT_MAX_DEPTH ? WT_TERMINAL : (mtype == kLambert ? WT_LAMBERT : (mtype == kMetal ? WT_METAL : WT_DIEL));
-                WFLD(WF_POS, tid) = make_float4(pos.x, pos.y, pos.z, __int_as_float(mid));
-                WFLD(WF_NRM, tid) = make_float4(normal.x, normal.y, normal.z, 0.0f);
+                float t;
+                const int id = hitter.hit(sc, st.o, st.d, TPT_MIN_T, TPT_MAX_T, t);
+                pool[WF_HIT * kWaveSlots + tid].x = t;
+                pool[WF_HIT * kWaveSlots + tid].y = __int_as_float(id);
+                if (st.kind != 0) type = WT_SHADOW;
+                else if (id < 0) type = WT_MISS;
+                else
+                {
+                    const int mtype = f_as_i(sc.matA[id < sc.count ? id : sc.count].w);
+                    type = st.depth >= TPT_MAX_DEPTH ? WT_TERMINAL : (mtype == kLambert ? WT_LAMBERT : (mtype == kMetal ? WT_METAL : WT_DIEL));
+                }
             }
         }
         // ---- phase 2: sort slots by type (ballot + prefix)
@@ -1941,7 +1983,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         const int live = sCount[0] + sCount[1] + sCount[2] + sCount[3] + sCount[4] + sCount[5];
         if (live == 0 && sExhausted) break;
 
-        // ---- phase 3: Scatter() per material type, 32-entry chunks dealt to the warps
+        // ---- phase 3: path_step per type, 32-entry chunks dealt to the warps (path_step counts the ray the sweep traced)
         {
             int chunk = warp;               // chunk ids over the concatenation of the type lists
             int T = 0, first = 0;           // `first` = chunk id of type T's first chunk
@@ -1952,85 +1994,19 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                 const int k = ((chunk - first) << 5) + lane;
                 const bool on = k < sCount[T];
                 const int slot = on ? sList[T][k] : 0;
-                bool wantLight = false, finished = false;
-                float4 fcol, fthr;
+                const bool wantLight = on && (T == WT_LAMBERT || T == WT_SHADOW);     // they go on in phase 4
                 if (on)
                 {
-                    fcol = WFLD(WF_COL, slot);
-                    fthr = WFLD(WF_THR, slot);
-                    float4 fdd = WFLD(WF_D, slot);
-                    int m2 = __float_as_int(fdd.w);
-                    V3 col = v3(fcol.x, fcol.y, fcol.z), thr = v3(fthr.x, fthr.y, fthr.z);
-                    uint32_t rng = __float_as_uint(fthr.w);
-                    const V3 d = v3(fdd.x, fdd.y, fdd.z);
-                    const bool doMatE = (m2 >> 24) & 1;
-                    if (T == WT_MISS) { col = col + thr * fast_sky(d, sc); finished = true; }
-                    else if (T == WT_SHADOW)
+                    QPath st = wave_load(pool, slot, kWavePath | (T == WT_SHADOW ? 1u << WF_THRALB : 0u));
+                    const float4* h = pool + WF_HIT * kWaveSlots + slot;
+                    if (path_step<kLsRuntime, 1, false>(sc, st, rc, StoredHit{__float_as_int(h->y), h->x}))
                     {
-                        const int j = (m2 & 0xffff) - 1;
-                        const int hid = __float_as_int(WFLD(WF_POS, slot).w);
-                        const LightRec& Lj = sc.lights[j];
-                        if (hid == Lj.id)
-                        {
-                            const float4 ta = WFLD(WF_THRALB, slot);
-                            col = col + (v3(ta.x, ta.y, ta.z) * v3(Lj.ex, Lj.ey, Lj.ez)) * WFLD(WF_NL, slot).w;
-                        }
-                        wantLight = true;   // next light index = j + 1, kept in kind
+                        const uint32_t pixOff = __float_as_uint(h->z);
+                        const float w = h->w;
+                        red_add_f4(p.image + (size_t)pixOff * 4, st.col.x * w, st.col.y * w, st.col.z * w);
+                        wave_free(pool, slot);
                     }
-                    else
-                    {
-                        const float4 fp = WFLD(WF_POS, slot), fn = WFLD(WF_NRM, slot);
-                        const V3 pos = v3(fp.x, fp.y, fp.z), normal = v3(fn.x, fn.y, fn.z);
-                        const int mid = __float_as_int(fp.w);
-                        const Mat mat = load_mat(sc, mid);
-                        if (T == WT_TERMINAL) { col = col + thr * mat.emissive; finished = true; }
-                        else if (T == WT_LAMBERT)
-                        {
-                            if (doMatE) col = col + thr * mat.emissive;
-                            const V3 target = normal + RandomUnitVector<false>(rng);
-                            const V3 nextDir = M<false>::normalize(target);
-                            const V3 nl = dot(normal, d) < 0.0f ? normal : neg(normal);
-                            const V3 thrAlb = thr * mat.albedo;
-                            WFLD(WF_NEXT, slot) = make_float4(nextDir.x, nextDir.y, nextDir.z, WFLD(WF_NEXT, slot).w);
-                            WFLD(WF_THRALB, slot) = make_float4(thrAlb.x, thrAlb.y, thrAlb.z, __int_as_float(mid));
-                            WFLD(WF_NL, slot) = make_float4(nl.x, nl.y, nl.z, 0.0f);
-                            WFLD(WF_O, slot) = make_float4(pos.x, pos.y, pos.z, 0.0f);
-                            m2 = (m2 & ~0xffff) | 0;    // kind := "before light 0" (light phase advances it)
-                            wantLight = true;
-                        }
-                        else
-                        {
-                            V3 att, outDir;
-                            bool ok;
-                            if (T == WT_METAL)
-                            {
-                                outDir = metal_dir(d, normal, mat.roughness, rng);
-                                att = mat.albedo;
-                                ok = dot(outDir, normal) > 0.0f;
-                            }
-                            else ok = scatter_specular<false>(mat, d, pos, normal, rng, att, outDir);
-                            if (!ok) { col = col + thr * mat.emissive; finished = true; }
-                            else
-                            {
-                                if (doMatE) col = col + thr * mat.emissive;
-                                thr = thr * att;
-                                const int depth = ((m2 >> 16) & 0xff) + 1;
-                                m2 = 0 | (depth << 16) | (1 << 24);
-                                WFLD(WF_O, slot) = make_float4(pos.x, pos.y, pos.z, 0.0f);
-                                fdd = make_float4(outDir.x, outDir.y, outDir.z, 0.0f);
-                            }
-                        }
-                    }
-                    if (finished)
-                    {
-                        const float w = WFLD(WF_NEXT, slot).w;
-                        red_add_f4(p.image + (size_t)__float_as_uint(fcol.w) * 4, col.x * w, col.y * w, col.z * w);
-                        m2 = kKindFree;
-                    }
-                    fdd.w = __int_as_float(m2);
-                    WFLD(WF_D, slot) = fdd;
-                    WFLD(WF_COL, slot) = make_float4(col.x, col.y, col.z, fcol.w);
-                    WFLD(WF_THR, slot) = make_float4(thr.x, thr.y, thr.z, __uint_as_float(rng));
+                    else wave_store(pool, slot, st, kWavePath | (T == WT_LAMBERT ? kWaveVertex : 0u));
                 }
                 const unsigned lm = __ballot_sync(0xffffffffu, wantLight);
                 if (lm)
@@ -2045,7 +2021,7 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
         }
         __syncthreads();
 
-        // ---- phase 4: explicit light sampling for Lambert vertices / returning shadow rays (Test.cpp:96-133)
+        // ---- phase 4: lambert_next for Lambert vertices / returning shadow rays (Test.cpp:96-133)
         {
             const int nL = sLightCount;
             for (int k = tid; k < ((nL + 31) & ~31); k += kWaveThreads)
@@ -2053,38 +2029,14 @@ k_fast_wave(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
                 if (k < nL)
                 {
                     const int slot = sLight[k];
-                    float4 fdd = WFLD(WF_D, slot);
-                    int m2 = __float_as_int(fdd.w);
-                    const float4 fta = WFLD(WF_THRALB, slot);
-                    // kind k = shadow ray of light k-1 just returned -> next is light k
-                    const int j = next_light(sc, m2 & 0xffff, __float_as_int(fta.w));
-                    if (j < sc.nLights)
-                    {
-                        const float4 fo = WFLD(WF_O, slot), fnl = WFLD(WF_NL, slot);
-                        uint32_t rng = __float_as_uint(WFLD(WF_THR, slot).w);
-                        V3 l;
-                        const float pend = sample_light_cone(sc.lights[j], v3(fo.x, fo.y, fo.z), v3(fnl.x, fnl.y, fnl.z), rng, l);
-                        WFLD(WF_NL, slot).w = pend;
-                        WFLD(WF_THR, slot).w = __uint_as_float(rng);
-                        m2 = (m2 & ~0xffff) | (1 + j);
-                        WFLD(WF_D, slot) = make_float4(l.x, l.y, l.z, __int_as_float(m2));
-                    }
-                    else
-                    {
-                        const float4 fnx = WFLD(WF_NEXT, slot);
-                        float4 fthr = WFLD(WF_THR, slot);
-                        const int depth = ((m2 >> 16) & 0xff) + 1;
-                        // doMaterialE = false after a Lambert vertex (Test.cpp:214), unless light sampling is off
-                        m2 = 0 | (depth << 16) | ((emission_after_lambert(sc) ? 1 : 0) << 24);
-                        WFLD(WF_D, slot) = make_float4(fnx.x, fnx.y, fnx.z, __int_as_float(m2));
-                        WFLD(WF_THR, slot) = make_float4(fta.x, fta.y, fta.z, fthr.w);
-                    }
+                    QPath st = wave_load(pool, slot, kWavePath & ~(1u << WF_COL) | kWaveVertex);
+                    lambert_next<kLsRuntime>(sc, st, st.kind);
+                    wave_store(pool, slot, st, kWavePath & ~(1u << WF_COL));
                 }
             }
         }
         __syncthreads();
     }
-#undef WFLD
     flush_ray_count(p.rayCounter, rc, lane);
 }
 
