@@ -92,6 +92,39 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
  * While a map is set, the slab queue runs its 6-CTA instances where it would pick the 8-CTA ones (long draws and caller
  * calls, "fast_variant" 9): those have no lookup, which would make them spill at 64 registers. */
 int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int height, int onDevice);
+/* Albedo textures for the fast mode: lat-long images bound to spheres by sphere id (which is also the material id). While
+ * they are set, every hit of a TPT_MODE_FAST tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples and
+ * tpt_trace_samples on a textured sphere uses albedo x T(n) wherever the untextured estimator uses the material's albedo:
+ * a Lambert vertex's throughput (its light cones, its environment sample and its bounce, with "light_sampling" on or off)
+ * and a Metal vertex's tint. Glass uses no albedo and emission is not textured. The lookup draws no random numbers, so
+ * every sample stream stays where it was. tpt_trace_irradiance's starting vertex stays white; later vertices on textured
+ * spheres are textured. tpt_draw_aovs and tpt_trace_aovs report the textured albedo for every material type.
+ *   n         the hit's shading normal (pos - centre) / radius.
+ *   T(n)      the bilinear lookup of the sphere's layer in the direction n, with the mapping tpt_set_environment pins:
+ *             phi = atan2f(n.x, -n.z), theta = acosf(clamp(n.y, -1, 1)), texel centres at (i + 1/2, j + 1/2), columns
+ *             wrap, rows clamp, every blend a + f * (b - a) (a constant layer returns its constant exactly). Row 0 is at the
+ *             sphere's +y pole, the centre column along -z and +x to its right.
+ *   rgba      layers * height * width float4 texels, layer-major, then row-major. All layers share width x height (resample
+ *             textures of other sizes). Alpha is ignored; R, G and B must be finite and not negative (-0 is refused too).
+ *             NULL removes the textures.
+ *   sphereLayers  numSpheres int32 in HOST memory: entry i is the layer of sphere i, or -1 for none. Sphere ids at or past
+ *             numSpheres, and the padding spheres of the sweep, are untextured.
+ *   onDevice  0: host texels; 1: device texels of the context's device, 16-byte aligned, complete when the call is made (a
+ *             small kernel checks them there). sphereLayers is host memory either way.
+ * Refused, with tpt_last_error text naming the offending value: width, height or layers below 1, width * height * layers
+ * >= 2^31, numSpheres < 0, a layer outside [-1, layers), a texel with a negative or non-finite R, G or B (the error names
+ * its layer, x and y), a misaligned device buffer or one on another device. A refused call leaves the textures as they were.
+ * Lifetime and ordering are tpt_set_environment's: a set-up call that may block and returns once the texels have been
+ * read; calls issued before it keep the textures they were issued with, even while in flight; tpt_set_scene keeps them,
+ * tpt_destroy frees them. Memory: two device copies of 16 * width * height * layers + 4 * numSpheres bytes at most.
+ * Kernels: only the slab queue's reference-form (sweep form 0) 6-CTA and 768-thread instances carry the lookup, so that no
+ * instance an untextured call runs does. While textures are set every fast call runs them: tpt_draw's auto variant is 3
+ * (host-buffer draws stage through the slab queue instead of storing into page-locked memory), 9 runs the 6-CTA instance,
+ * and an explicit "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused. tpt_draw in TPT_MODE_EXACT, TPT_MODE_REFGPU and
+ * TPT_MODE_REFGPU_FAST is refused: those modes reproduce the reference, which has no textures. Textures and
+ * "environment_sampling" run in the same instances and combine. */
+int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
+                     const int* sphereLayers, int numSpheres, int onDevice);
 /* Camera only (UpdateTest rebuilds it every frame from the aspect ratio, Test.cpp:341). */
 int tpt_set_camera(tpt_context* ctx, const void* camera88);
 

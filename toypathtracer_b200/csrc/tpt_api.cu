@@ -21,6 +21,21 @@ thread_local KernelRecord tpt::t_lastKernels = {};
 // tpt_tonemap_rgba8, tpt_trace_rays' out4 and tpt_draw_samples' sum4; the others hold the buffers they are named after.
 enum Staging { kStageImage, kStageRays, kStageAlbedo, kStageNormal, kStageIds, kStagePixels, kStageSq4, kNumStaging };
 
+// Set-up data that the calls read on the device (tpt_set_environment's map, tpt_set_textures' layers), in two device slots
+// with the scene blob's discipline: a new upload goes into the slot that is not current, on the upload stream after that
+// slot's last use (slot_begin_upload, slot_finish_upload); calls wait on the current slot's upload and mark its last use
+// (begin_call and finish_call through slot_use and slot_used). So a call keeps the data it was issued with, even while
+// it is in flight, and the caller never synchronises.
+struct DeviceSlots
+{
+    void* ptr[2] = {nullptr, nullptr};
+    size_t cap[2] = {0, 0};
+    int cur = 1;                                  // the first upload goes into slot 0
+    bool have = false;                            // the calls issued from now on read slot `cur`
+    cudaEvent_t uploadDone[2] = {nullptr, nullptr};
+    cudaEvent_t lastUse[2] = {nullptr, nullptr};
+};
+
 struct tpt_context
 {
     int device = 0;
@@ -51,18 +66,14 @@ struct tpt_context
     bool haveScene = false;
     int spp = 4;
 
-    // environment (tpt_set_environment): two device slots with the scene blob's discipline. A new map goes into the slot
-    // that is not current, on the upload stream after that slot's last use; calls wait on the current slot's upload and
-    // mark its last use. It belongs to the context, not to the scene: tpt_set_scene leaves it alone.
-    Q4* dEnv[2] = {nullptr, nullptr};
-    size_t envCap[2] = {0, 0};
-    int curEnv = 1;                               // the first map goes into slot 0
-    bool haveEnv = false;
+    // environment (tpt_set_environment) and textures (tpt_set_textures): each in its own DeviceSlots. They belong to the
+    // context, not to the scene: tpt_set_scene leaves them alone.
+    DeviceSlots env;
     int envW = 0, envH = 0;                       // of the current slot
     bool envSampleable = false;                   // the current slot's map has sampling tables (some weight is not zero)
     int envSampling = 0;                          // "environment_sampling"
-    cudaEvent_t envUploadDone[2] = {nullptr, nullptr};
-    cudaEvent_t envLastUse[2] = {nullptr, nullptr};
+    DeviceSlots tex;                              // [layers x texH x texW float4 texels][texSpheres int32 layers]
+    int texW = 0, texH = 0, texLayers = 0, texSpheres = 0;   // of the current slot
 
     // options
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
@@ -236,8 +247,11 @@ int tpt_create(int device, tpt_context** out)
     {
         e = cudaEventCreateWithFlags(&ctx->uploadDone[i], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->blobLastUse[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->envUploadDone[i], cudaEventDisableTiming);
-        if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->envLastUse[i], cudaEventDisableTiming);
+        for (DeviceSlots* s : {&ctx->env, &ctx->tex})
+        {
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->uploadDone[i], cudaEventDisableTiming);
+            if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->lastUse[i], cudaEventDisableTiming);
+        }
     }
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->lastDraw, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->forkEvent, cudaEventDisableTiming);
@@ -281,9 +295,12 @@ void tpt_destroy(tpt_context* ctx)
         if (ctx->hBlob[i]) cudaFreeHost(ctx->hBlob[i]);
         if (ctx->uploadDone[i]) cudaEventDestroy(ctx->uploadDone[i]);
         if (ctx->blobLastUse[i]) cudaEventDestroy(ctx->blobLastUse[i]);
-        cudaFree(ctx->dEnv[i]);
-        if (ctx->envUploadDone[i]) cudaEventDestroy(ctx->envUploadDone[i]);
-        if (ctx->envLastUse[i]) cudaEventDestroy(ctx->envLastUse[i]);
+        for (DeviceSlots* s : {&ctx->env, &ctx->tex})
+        {
+            cudaFree(s->ptr[i]);
+            if (s->uploadDone[i]) cudaEventDestroy(s->uploadDone[i]);
+            if (s->lastUse[i]) cudaEventDestroy(s->lastUse[i]);
+        }
     }
     if (ctx->uploadStream) cudaStreamDestroy(ctx->uploadStream);
     if (ctx->lastDraw) cudaEventDestroy(ctx->lastDraw);
@@ -437,6 +454,51 @@ static int ensure(tpt_context* ctx, void** p, size_t* cap, size_t bytes, const c
     return 0;
 }
 
+// The slot a new upload of `bytes` goes into (*slot): the one that is not current, grown when it is too small (after its
+// last reader, issued before the previous upload, has finished), with the upload stream ordered after that reader.
+// `what` names the data in error texts.
+static int slot_begin_upload(tpt_context* ctx, DeviceSlots& s, size_t bytes, const char* what, int* slot)
+{
+    const std::string w = what;
+    *slot = s.cur ^ 1;
+    if (bytes > s.cap[*slot])
+    {
+        CK(cudaEventSynchronize(s.lastUse[*slot]), ("sync before " + w + " realloc").c_str());
+        cudaFree(s.ptr[*slot]); s.ptr[*slot] = nullptr; s.cap[*slot] = 0;
+        CK(cudaMalloc(&s.ptr[*slot], bytes), ("cudaMalloc " + w).c_str());
+        s.cap[*slot] = bytes;
+    }
+    CK(cudaStreamWaitEvent(ctx->uploadStream, s.lastUse[*slot], 0), (w + " upload waits for the slot's readers").c_str());
+    return 0;
+}
+
+// After the upload's copies into `slot` were enqueued on the upload stream: the slot becomes current once they have been
+// read (a set-up call: it returns once the caller's data has been read, so the caller may then free or reuse it).
+static int slot_finish_upload(tpt_context* ctx, DeviceSlots& s, int slot, const char* what)
+{
+    const std::string w = what;
+    CK(cudaEventRecord(s.uploadDone[slot], ctx->uploadStream), (w + " upload event").c_str());
+    CK(cudaStreamSynchronize(ctx->uploadStream), (w + " upload sync").c_str());
+    s.cur = slot;
+    s.have = true;
+    return 0;
+}
+
+// begin_call: the call reads the current slot, once its upload has landed; its address into *addr.
+static int slot_use(tpt_context* ctx, const DeviceSlots& s, cudaStream_t stream, const char* what, uint64_t* addr)
+{
+    CK(cudaStreamWaitEvent(stream, s.uploadDone[s.cur], 0), (std::string("wait for ") + what + " upload").c_str());
+    *addr = (uint64_t)(uintptr_t)s.ptr[s.cur];
+    return 0;
+}
+
+// finish_call: the next upload into the call's slot waits for this call.
+static int slot_used(tpt_context* ctx, const DeviceSlots& s, cudaStream_t stream, const char* what)
+{
+    if (s.have) CK(cudaEventRecord(s.lastUse[s.cur], stream), (std::string(what) + " last-use event").c_str());
+    return 0;
+}
+
 // Prologue of a call that traces (tpt_draw, tpt_trace_rays). One context = one scene blob, one set of counters: calls are
 // ordered in issue order even across streams, and the scene they read must have landed (tpt_set_scene uploads
 // asynchronously on its own stream). Returns the call's stream and the scene with the context's sweep-form option applied.
@@ -447,11 +509,11 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
     if (ctx->haveLastDraw && ctx->lastDrawStream != *stream) CK(cudaStreamWaitEvent(*stream, ctx->lastDraw, 0), "order after previous draw");
     CK(cudaStreamWaitEvent(*stream, ctx->uploadDone[ctx->curBlob], 0), "wait for scene upload");
     *scene = ctx->scene;
-    if (ctx->haveEnv)
+    if (ctx->env.have)
     {
         // the call reads the environment that is current now, in its slot, once that slot's upload has landed
-        CK(cudaStreamWaitEvent(*stream, ctx->envUploadDone[ctx->curEnv], 0), "wait for environment upload");
-        const uint64_t env = (uint64_t)(uintptr_t)ctx->dEnv[ctx->curEnv];
+        uint64_t env = 0;
+        if (int r = slot_use(ctx, ctx->env, *stream, "environment", &env)) return r;
         scene->layout.flags |= kSceneEnvironment;
         scene->layout.envLo = (uint32_t)env;
         scene->layout.envHi = (uint32_t)(env >> 32);
@@ -460,6 +522,21 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
         // "environment_sampling" is read here, per call, like the map: not a scene flag, so toggling it uploads nothing
         if (ctx->envSampling && ctx->envSampleable && !(scene->layout.flags & kSceneNoLightSampling))
             scene->layout.flags |= kSceneEnvSampling;
+    }
+    if (ctx->tex.have)
+    {
+        uint64_t tex = 0;
+        if (int r = slot_use(ctx, ctx->tex, *stream, "textures", &tex)) return r;
+        const uint64_t tab = tex + (uint64_t)16 * ctx->texW * ctx->texH * ctx->texLayers;
+        scene->layout.flags |= kSceneTextures;
+        scene->layout.texLo = (uint32_t)tex;
+        scene->layout.texHi = (uint32_t)(tex >> 32);
+        scene->layout.tabLo = (uint32_t)tab;
+        scene->layout.tabHi = (uint32_t)(tab >> 32);
+        scene->layout.texW = ctx->texW;
+        scene->layout.texH = ctx->texH;
+        // sphere ids past the scene's count are padding spheres, which are never textured
+        scene->layout.texSpheres = ctx->texSpheres < scene->count ? ctx->texSpheres : scene->count;
     }
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
@@ -510,7 +587,8 @@ static int finish_call(tpt_context* ctx, cudaStream_t stream, int n, bool hostBu
 {
     CK(cudaEventRecord(ctx->lastDraw, stream), "draw end event");
     CK(cudaEventRecord(ctx->blobLastUse[ctx->curBlob], stream), "scene last-use event");
-    if (ctx->haveEnv) CK(cudaEventRecord(ctx->envLastUse[ctx->curEnv], stream), "environment last-use event");
+    if (int r = slot_used(ctx, ctx->env, stream, "environment")) return r;
+    if (int r = slot_used(ctx, ctx->tex, stream, "textures")) return r;
     ctx->lastDrawStream = stream; ctx->haveLastDraw = true;
     if (outRayCount || outPerFrame)
     {
@@ -826,21 +904,28 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode != TPT_MODE_EXACT && mode != TPT_MODE_FAST && mode != TPT_MODE_REFGPU && mode != TPT_MODE_REFGPU_FAST)
         return fail_msg(ctx, "tpt_draw: unknown mode");
     // the parity modes reproduce the reference, which has no environment to be bit-identical to
-    if (mode != TPT_MODE_FAST && ctx->haveEnv)
+    if (mode != TPT_MODE_FAST && ctx->env.have)
         return fail_msg(ctx, "tpt_draw: an environment is set, and only TPT_MODE_FAST draws use one (clear it with "
                              "tpt_set_environment(ctx, NULL, 0, 0, 0) for exact and reference-GPU draws)");
+    if (mode != TPT_MODE_FAST && ctx->tex.have)
+        return fail_msg(ctx, "tpt_draw: textures are set, and only TPT_MODE_FAST draws use them (clear them with "
+                             "tpt_set_textures(ctx, NULL, 0, 0, 0, NULL, 0, 0) for exact and reference-GPU draws)");
     // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
     if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    // only the slab queue's 6-CTA and 768-thread instances sample the environment
+    // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment and look up textures
     const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
-    if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).samplesEnvironment)
+    const bool textured = (scene.layout.flags & kSceneTextures) != 0;
+    if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
         return fail_msgf(ctx, "tpt_draw: \"environment_sampling\" is active (option on, a map with non-zero weight, light "
                               "sampling on), and fast_variant %d does not sample the environment: use -1 (auto), 3 or 9",
                          ctx->fastVariant);
+    if (textured && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
+        return fail_msgf(ctx, "tpt_draw: textures are set (tpt_set_textures), and fast_variant %d does not look them up: "
+                              "use -1 (auto), 3 or 9", ctx->fastVariant);
 
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);
@@ -851,7 +936,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     // being traced — no staging image, no device-to-host copy after the kernel.
     bool zeroCopy = false;
     cudaPointerAttributes attr{};
-    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && !envSampling &&
+    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && !envSampling && !textured &&
         (ctx->fastVariant < 0 || fast_variant_info(ctx->fastVariant).writesFinalPixels))
     {
         zeroCopy = prevWeight == 0.0f && numFrames <= kMaxFramesPerDraw && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&
@@ -1134,7 +1219,7 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
     static const char* fn = "tpt_set_environment";
     if (!ctx) return (int)cudaErrorInvalidValue;
     // NULL: the calls issued from now on see the reference sky; those in flight keep reading their slot
-    if (!rgba) { ctx->haveEnv = false; return 0; }
+    if (!rgba) { ctx->env.have = false; return 0; }
     if (width < 1 || height < 1) return fail_msgf(ctx, "%s: width and height must be >= 1 (got %d x %d)", fn, width, height);
     const long long n = (long long)width * height;
     if (n >= (1LL << 31)) return fail_msgf(ctx, "%s: width * height must be below 2^31 (got %lld)", fn, n);
@@ -1151,32 +1236,25 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
                 if (!env_channel_ok(rgba[4 * i + c]))
                     return fail_msgf(ctx, "%s: texel %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative",
                                      fn, i, i % width, i / width, c == 0 ? "R" : c == 1 ? "G" : "B", rgba[4 * i + c]);
-    // The slot that is not current: the calls issued since the last tpt_set_environment read the other one. The upload
-    // waits on the device for the slot's last reader (issued before the previous tpt_set_environment).
+    // The slot that is not current: the calls issued since the last tpt_set_environment read the other one.
     // The slot holds the texels, each cell's sampling probability in their alpha, and the alias tables behind them
     // (tpt_env_tables.h): 24 W H + 8 H bytes, built here on the host.
-    const int slot = ctx->curEnv ^ 1;
     const size_t bytes = env_slot_bytes(width, height);
-    if (bytes > ctx->envCap[slot])
-    {
-        CK(cudaEventSynchronize(ctx->envLastUse[slot]), "sync before environment realloc");
-        cudaFree(ctx->dEnv[slot]); ctx->dEnv[slot] = nullptr; ctx->envCap[slot] = 0;
-        CK(cudaMalloc(&ctx->dEnv[slot], bytes), "cudaMalloc environment");
-        ctx->envCap[slot] = bytes;
-    }
+    int slot = 0;
+    if (int r = slot_begin_upload(ctx, ctx->env, bytes, "environment", &slot)) return r;
+    Q4* dst = (Q4*)ctx->env.ptr[slot];
     cudaStream_t s = ctx->uploadStream;
-    CK(cudaStreamWaitEvent(s, ctx->envLastUse[slot], 0), "environment upload waits for the slot's readers");
     std::vector<float> host((bytes + 3) / 4);
     float* tex = host.data();
     if (onDevice)
     {
         // R, G and B of every texel packed into the slot's first 12 n bytes, then checked as 3 n int32 in [0, +Inf's bits)
         // by the caller-list check (entry = channel index), and copied back for the table build
-        CK(cudaMemcpy2DAsync(ctx->dEnv[slot], 12, rgba, 16, 12, (size_t)n, cudaMemcpyDefault, s), "pack environment RGB");
-        CK(launch_list_check((const int*)ctx->dEnv[slot], 3 * n, kEnvBitsLimit, ctx->dBadPixel, ctx->numSMs, s),
+        CK(cudaMemcpy2DAsync(dst, 12, rgba, 16, 12, (size_t)n, cudaMemcpyDefault, s), "pack environment RGB");
+        CK(launch_list_check((const int*)dst, 3 * n, kEnvBitsLimit, ctx->dBadPixel, ctx->numSMs, s),
            "environment check launch");
         CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s), "D2H environment check");
-        CK(cudaMemcpy2DAsync(tex, 16, ctx->dEnv[slot], 12, 12, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H environment RGB");
+        CK(cudaMemcpy2DAsync(tex, 16, dst, 12, 12, (size_t)n, cudaMemcpyDeviceToHost, s), "D2H environment RGB");
         // A refused map leaves the current environment as it was.
         CK(cudaStreamSynchronize(s), "environment check sync");
         if (*ctx->hBadPixel != ~0ull)
@@ -1193,15 +1271,87 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
         memcpy(tex, rgba, (size_t)n * 16);
     EnvAlias* rows = reinterpret_cast<EnvAlias*>(tex + 4 * n);
     const bool sampleable = env_build_tables(tex, width, height, rows, rows + height);
-    CK(cudaMemcpyAsync(ctx->dEnv[slot], tex, bytes, cudaMemcpyHostToDevice, s), "environment upload");
-    CK(cudaEventRecord(ctx->envUploadDone[slot], s), "environment upload event");
-    // A set-up call: it returns once the caller's texels have been read (the caller may then free or reuse its buffer).
-    CK(cudaStreamSynchronize(s), "environment upload sync");
-    ctx->curEnv = slot;
-    ctx->haveEnv = true;
+    CK(cudaMemcpyAsync(dst, tex, bytes, cudaMemcpyHostToDevice, s), "environment upload");
+    if (int r = slot_finish_upload(ctx, ctx->env, slot, "environment")) return r;
     ctx->envSampleable = sampleable;
     ctx->envW = width;
     ctx->envH = height;
+    return 0;
+}
+
+int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
+                     const int* sphereLayers, int numSpheres, int onDevice)
+{
+    static const char* fn = "tpt_set_textures";
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    // NULL: the calls issued from now on see every sphere untextured; those in flight keep reading their slot
+    if (!rgba) { ctx->tex.have = false; return 0; }
+    if (width < 1 || height < 1 || layers < 1)
+        return fail_msgf(ctx, "%s: width, height and layers must be >= 1 (got %d x %d x %d)", fn, width, height, layers);
+    const long long plane = (long long)width * height, n = plane * layers;
+    if (n >= (1LL << 31)) return fail_msgf(ctx, "%s: width * height * layers must be below 2^31 (got %lld)", fn, n);
+    if (numSpheres < 0) return fail_msgf(ctx, "%s: numSpheres must be >= 0 (got %d)", fn, numSpheres);
+    if (numSpheres > 0 && !sphereLayers) return fail_msgf(ctx, "%s: sphereLayers is NULL for %d spheres", fn, numSpheres);
+    for (int i = 0; i < numSpheres; ++i)
+        if (sphereLayers[i] < -1 || sphereLayers[i] >= layers)
+            return fail_msgf(ctx, "%s: sphereLayers[%d] = %d is outside [-1, %d)", fn, i, sphereLayers[i], layers);
+    auto bad_texel = [&](long long i, int c, float v) {
+        return fail_msgf(ctx, "%s: texel of layer %lld (x %lld, y %lld) has %s = %g: RGB must be finite and not negative", fn,
+                         i / plane, i % width, i % plane / width, c == 0 ? "R" : c == 1 ? "G" : "B", v);
+    };
+    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+    if (onDevice)
+    {
+        if ((uintptr_t)rgba & 15) return fail_msgf(ctx, "%s: device rgba is not 16-byte aligned", fn);
+        if (int r = check_device_buffer(ctx, fn, rgba, "rgba")) return r;
+        if (int r = ensure_index_check(ctx)) return r;
+    }
+    else
+        for (long long i = 0; i < n; ++i)
+            for (int c = 0; c < 3; ++c)
+                if (!env_channel_ok(rgba[4 * i + c])) return bad_texel(i, c, rgba[4 * i + c]);
+    // The slot that is not current: the calls issued since the last tpt_set_textures read the other one. It holds the
+    // texels and the sphere table behind them: 16 W H L + 4 numSpheres bytes.
+    const size_t texBytes = (size_t)n * 16, bytes = texBytes + (size_t)numSpheres * 4;
+    int slot = 0;
+    if (int r = slot_begin_upload(ctx, ctx->tex, bytes, "textures", &slot)) return r;
+    unsigned char* dst = (unsigned char*)ctx->tex.ptr[slot];
+    cudaStream_t s = ctx->uploadStream;
+    if (onDevice)
+    {
+        // As tpt_set_environment checks a device map: R, G and B packed into the slot, checked as int32 bits by the
+        // caller-list check (entry = channel index), in chunks whose entry indices fit the check's 32 bits. Then the
+        // texels themselves, alpha included (never read).
+        const long long kChunk = 1LL << 30;
+        for (long long c0 = 0; c0 < n; c0 += kChunk)
+        {
+            const long long m = n - c0 < kChunk ? n - c0 : kChunk;
+            CK(cudaMemcpy2DAsync(dst, 12, rgba + 4 * c0, 16, 12, (size_t)m, cudaMemcpyDefault, s), "pack texture RGB");
+            CK(launch_list_check((const int*)dst, 3 * m, kEnvBitsLimit, ctx->dBadPixel, ctx->numSMs, s), "texture check launch");
+            CK(cudaMemcpyAsync(ctx->hBadPixel, ctx->dBadPixel, sizeof(unsigned long long), cudaMemcpyDeviceToHost, s),
+               "D2H texture check");
+            // A refused texel leaves the current textures as they were.
+            CK(cudaStreamSynchronize(s), "texture check sync");
+            if (*ctx->hBadPixel != ~0ull)
+            {
+                const long long k = (long long)(*ctx->hBadPixel >> 32);
+                uint32_t bits = (uint32_t)*ctx->hBadPixel;
+                float v;
+                memcpy(&v, &bits, 4);
+                return bad_texel(c0 + k / 3, (int)(k % 3), v);
+            }
+        }
+        CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyDeviceToDevice, s), "texture upload");
+    }
+    else
+        CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyHostToDevice, s), "texture upload");
+    if (numSpheres > 0)
+        CK(cudaMemcpyAsync(dst + texBytes, sphereLayers, (size_t)numSpheres * 4, cudaMemcpyHostToDevice, s), "sphere layer upload");
+    if (int r = slot_finish_upload(ctx, ctx->tex, slot, "textures")) return r;
+    ctx->texW = width;
+    ctx->texH = height;
+    ctx->texLayers = layers;
+    ctx->texSpheres = numSpheres;
     return 0;
 }
 

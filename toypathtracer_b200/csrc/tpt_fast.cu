@@ -900,17 +900,19 @@ __device__ __forceinline__ V3 metal_dir(V3 d, V3 normal, float roughness, uint32
     return M<false>::normalize(refl);
 }
 
-// Radiance of tpt_set_environment's lat-long map in the unit direction d (include/tpt_b200.h pins the mapping):
-// phi = atan2(d.x, -d.z), theta = acos(d.y); continuous texel coordinates u = (phi + pi) / 2pi * W, v = theta / pi * H,
-// texel (i, j) centred at (i + 1/2, j + 1/2), row 0 at the zenith; bilinear, columns wrapping, rows clamped. Every blend is
-// a + f * (b - a), so a constant map returns its constant bit for bit. Four 128-bit read-only loads.
+// Bilinear lookup of the W x H lat-long image of RGBA texels at `tex` (global memory) in the direction d
+// (include/tpt_b200.h pins the mapping): phi = atan2(d.x, -d.z), theta = acos(d.y); continuous texel coordinates
+// u = (phi + pi) / 2pi * W, v = theta / pi * H, texel (i, j) centred at (i + 1/2, j + 1/2), row 0 at +y; columns wrapping,
+// rows clamped. Every blend is a + f * (b - a), so a constant image returns its constant bit for bit. Four 128-bit
+// read-only loads; RGB: twelve 32-bit ones of R, G and B only, at 32-bit texel offsets (fewer registers live: the texture
+// instances stay at 80 without spilling). The environment map (env_radiance) and the sphere textures (textured_albedo)
+// both read through it.
 // CELL: also the sampling probability P of the cell [i, i+1) x [j, j+1) that holds (u + 1/2, v + 1/2), from the alpha of
 // whichever of the four texels that is (tpt_env_tables.h).
-template <bool CELL = false>
-__device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d, float* cellP = nullptr)
+template <bool CELL = false, bool RGB = false>
+__device__ __forceinline__ V3 latlong_lookup(const float4* tex, int W, int H, V3 d, float* cellP = nullptr)
 {
     constexpr float kPi = 3.14159265358979f;
-    const int W = sc.envW, H = sc.envH;
     const float phi = atan2f(d.x, -d.z);
     const float theta = acosf(fminf(fmaxf(d.y, -1.0f), 1.0f));
     const float u = (phi + kPi) * (0.5f / kPi) * (float)W - 0.5f;
@@ -923,15 +925,47 @@ __device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d, float* cel
     const int x1 = x0 + 1 == W ? 0 : x0 + 1;
     const int y1 = min(max(y0 + 1, 0), H - 1);
     y0 = min(max(y0, 0), H - 1);
-    const float4* env = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
-    const float4* row0 = env + (size_t)y0 * W;
-    const float4* row1 = env + (size_t)y1 * W;
-    const float4 a = __ldg(row0 + x0), b = __ldg(row0 + x1), c = __ldg(row1 + x0), e = __ldg(row1 + x1);
     auto lerp = [](float p, float q, float f) { return p + f * (q - p); };
+    if constexpr (RGB)
+    {
+        auto ld = [&](int x, int y) {
+            const float* f = reinterpret_cast<const float*>(tex + (uint32_t)(y * W + x));
+            return v3(__ldg(f), __ldg(f + 1), __ldg(f + 2));
+        };
+        const V3 a = ld(x0, y0), b = ld(x1, y0), c = ld(x0, y1), e = ld(x1, y1);
+        const V3 top = v3(lerp(a.x, b.x, tu), lerp(a.y, b.y, tu), lerp(a.z, b.z, tu));
+        const V3 bot = v3(lerp(c.x, e.x, tu), lerp(c.y, e.y, tu), lerp(c.z, e.z, tu));
+        return v3(lerp(top.x, bot.x, tv), lerp(top.y, bot.y, tv), lerp(top.z, bot.z, tv));
+    }
+    const float4* row0 = tex + (size_t)y0 * W;
+    const float4* row1 = tex + (size_t)y1 * W;
+    const float4 a = __ldg(row0 + x0), b = __ldg(row0 + x1), c = __ldg(row1 + x0), e = __ldg(row1 + x1);
     if constexpr (CELL) *cellP = tv < 0.5f ? (tu < 0.5f ? a.w : b.w) : (tu < 0.5f ? c.w : e.w);
     const V3 top = v3(lerp(a.x, b.x, tu), lerp(a.y, b.y, tu), lerp(a.z, b.z, tu));
     const V3 bot = v3(lerp(c.x, e.x, tu), lerp(c.y, e.y, tu), lerp(c.z, e.z, tu));
     return v3(lerp(top.x, bot.x, tv), lerp(top.y, bot.y, tv), lerp(top.z, bot.z, tv));
+}
+
+// Radiance of tpt_set_environment's lat-long map in the unit direction d (row 0 at the zenith).
+template <bool CELL = false>
+__device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d, float* cellP = nullptr)
+{
+    const float4* env = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
+    return latlong_lookup<CELL>(env, sc.envW, sc.envH, d, cellP);
+}
+
+// tpt_set_textures (kSceneTextures, the caller checks the flag): the albedo of a hit on sphere `id` with shading normal n
+// ((pos - centre) / r): albedo x the lookup of the sphere's layer at n, or albedo itself for a sphere without a layer
+// (-1, or an id at or past texSpheres, which begin_call keeps at most the scene's count: padding spheres have none).
+// Draws no random numbers.
+__device__ __forceinline__ V3 textured_albedo(const SceneView& sc, int id, V3 albedo, V3 n)
+{
+    if (id >= sc.texSpheres) return albedo;
+    const int* tab = reinterpret_cast<const int*>(((uint64_t)sc.tabHi << 32) | sc.tabLo);
+    const int layer = __ldg(tab + id);
+    if (layer < 0) return albedo;
+    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)sc.texHi << 32) | sc.texLo);
+    return albedo * latlong_lookup<false, true>(tex + (uint32_t)(layer * sc.texW * sc.texH), sc.texW, sc.texH, n);
 }
 
 // What a fast path sees when it leaves the scene: the caller's environment while one is set, else the reference sky
@@ -1044,7 +1078,9 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // 768-thread light-sampling instances).
 // NEXT false: stop before lambert_next, for a caller that runs it later (the block wavefront). A Lambert vertex just shaded
 // and a returning shadow ray then leave the light to go on from in st.kind.
-template <int LS, int ENVM = 1, bool NEXT = true, class Hitter>
+// TEX: where the call's kSceneTextures is set, Lambert and Metal hits take textured_albedo for the material's albedo (the
+// slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while textures are set).
+template <int LS, int ENVM = 1, bool NEXT = true, bool TEX = false, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
@@ -1077,6 +1113,9 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 // the compiler turns a three-way test of mat.type into a jump table (LDC from the constant bank + BRX: two
                 // long-latency steps in front of every shading branch); keeping the second test opaque keeps it two branches
                 int mtype = mat.type;
+                // Lambert and Metal use the albedo (glass does not): with textures, the textured one
+                if constexpr (TEX)
+                    if ((sc.flags & kSceneTextures) && mtype != kDielectric) mat.albedo = textured_albedo(sc, id, mat.albedo, normal);
                 if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
                 else if (LS == kLsOff && mtype == kLambert)
                 {
@@ -1321,7 +1360,7 @@ __device__ __forceinline__ unsigned long long gtimer() { unsigned long long t; a
 // slab being 64 consecutive entries x one sample index, finished paths adding (col, 1) to p.image[entry] and, with
 // MOMENTS, (col^2, 0) to p.sq4[entry].
 enum QueueSource { kSrcCamera = 0, kSrcRays = 1, kSrcPixels = 2 };
-template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false, int ENVM = 1>
+template <int THREADS, int KFORM, int LS, int SRC = kSrcCamera, bool MOMENTS = false, int ENVM = 1, bool TEX = false>
 __device__ __forceinline__ void
 fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayout L, int count, int nLights,
                 uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
@@ -1439,7 +1478,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if (exhausted) { if (!trDry) trDry = gtimer(); ++trDryTrips; trDryLanes += (unsigned)__popc(__ballot_sync(0xffffffffu, st.active)); }
 #endif
 
-        if (path_step<LS, ENVM>(sc, st, rc, hitter))
+        if (path_step<LS, ENVM, true, TEX>(sc, st, rc, hitter))
         {
             if constexpr (SRC == kSrcPixels)
             {
@@ -1486,6 +1525,10 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
 // map-less 720p draw 20 % (23 200 -> 18 400 Mray/s) at the same 80 registers and no stack, so it is kept out of the
 // instances the default sweep forms run.
 __host__ __device__ constexpr int env_mode(int minb, int kform) { return minb == 8 ? 0 : minb == 7 || kform != 0 ? 1 : 2; }
+// path_step's TEX of a slab-queue instance, light sampling on or off: the same reference-form 6-CTA and 768-thread
+// instances look up textures (pick_queue runs them while textures are set), so no instance a default call runs carries
+// the lookup.
+__host__ __device__ constexpr bool tex_mode(int minb, int kform) { return env_mode(minb, kform) == 2; }
 
 template <int THREADS, int MINB, int KFORM>
 __global__ void __launch_bounds__(THREADS, MINB)
@@ -1493,7 +1536,7 @@ k_fast_queue(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayo
              uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
              uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcCamera, false, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcCamera, false, env_mode(MINB, KFORM), tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // DO_LIGHT_SAMPLING 0 (scene flag kSceneNoLightSampling): the same kernel without the light-sampling half of the state
@@ -1504,7 +1547,7 @@ k_fast_queue_nolight(DrawParams p, const unsigned char* __restrict__ blob, Scene
                      uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                      uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcCamera, false, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcCamera, false, MINB != 8 ? 1 : 0, tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_trace_rays: the slab queue on caller rays (RAYS = true), with the same launch shapes as k_fast_queue and the
@@ -1515,7 +1558,7 @@ k_fast_rays(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLayou
             uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
             uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays, false, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcRays, false, env_mode(MINB, KFORM), tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 template <int THREADS, int MINB, int KFORM>
@@ -1524,7 +1567,7 @@ k_fast_rays_nolight(DrawParams p, const unsigned char* __restrict__ blob, SceneB
                     uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                     uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays, false, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcRays, false, MINB != 8 ? 1 : 0, tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone, mtilesPerBand, raysOffset, pp);
 }
 
 // tpt_draw_samples: the slab queue on a pixel list (SRC = kSrcPixels), per-entry sums and, with MOMENTS, sums of squares.
@@ -1535,7 +1578,7 @@ k_fast_samples(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobLa
                uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone, uint32_t mtilesPerBand,
                uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS, env_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOn, kSrcPixels, MOMENTS, env_mode(MINB, KFORM), tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                  mtilesPerBand, raysOffset, pp);
 }
 
@@ -1545,7 +1588,7 @@ k_fast_samples_nolight(DrawParams p, const unsigned char* __restrict__ blob, Sce
                        uint32_t stagedBytes, uint32_t numSlabs, uint32_t S, unsigned int* __restrict__ bandDone,
                        uint32_t mtilesPerBand, uint32_t raysOffset, const __grid_constant__ ParamPairs pp)
 {
-    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS, MINB != 8 ? 1 : 0>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
+    fast_queue_body<THREADS, KFORM, kLsOff, kSrcPixels, MOMENTS, MINB != 8 ? 1 : 0, tex_mode(MINB, KFORM)>(p, blob, L, count, nLights, stagedBytes, numSlabs, S, bandDone,
                                                                   mtilesPerBand, raysOffset, pp);
 }
 
@@ -2148,9 +2191,9 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
 {
     QueuePick q;
     q.kform = fast_queue_kform(sc);
-    // the environment-sampling instances sweep in the reference form (env_mode)
-    const bool envSampling = (sc.layout.flags & kSceneEnvSampling) != 0;
-    if (envSampling) q.kform = 0;
+    // the environment-sampling and texture instances sweep in the reference form (env_mode, tex_mode)
+    const bool refInstances = (sc.layout.flags & (kSceneEnvSampling | kSceneTextures)) != 0;
+    if (refInstances) q.kform = 0;
     // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
     // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2). The same
     // instances run form 5 (the half-precision pass 1) when the parameter says so (sc.pairs.half, begin_call).
@@ -2160,8 +2203,9 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     const bool big = fast_smem(sc.stagedBytes, smem_pair_bytes(sc, q.kform), 4 * 2048).bytes > 36 * 1024 ||
                      sc.stagedBytes != sc.layout.totalBytes;
     const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
-    // the 8-CTA instances have no environment lookup (at 64 registers it made them spill): with one set, the 6-CTA ones run
-    const bool eight = !(sc.layout.flags & kSceneEnvironment) && (variant == 9 || (variant == 3 && slabsPerWarp >= 48));
+    // the 8-CTA instances have no environment lookup (at 64 registers it made them spill) and no texture lookup: with
+    // either set, the 6-CTA ones run
+    const bool eight = !(sc.layout.flags & (kSceneEnvironment | kSceneTextures)) && (variant == 9 || (variant == 3 && slabsPerWarp >= 48));
     q.threads = big ? TPT_BIG_THREADS : 128;
     if (big) q.kern = queue_kernel<SRC, MOMENTS, TPT_BIG_THREADS, 1>(sc, q.kform);
     else if (q.kform == 4)
@@ -2340,6 +2384,8 @@ __device__ __forceinline__ int aov_sample(const SceneView& sc, const Hitter& hit
     a.normal = (pos - v3(s.x, s.y, s.z)) * sc.invRadius[id];     // path_step's normal: not flipped, not renormalised
     const Q4 m = sc.matA[id < sc.count ? id : sc.count];         // a padded sphere (form 0) has the all-zero material
     a.albedo = v3(m.x, m.y, m.z);
+    // the textured albedo for every material type (this kernel is not on a draw's path: a runtime branch is enough)
+    if (sc.flags & kSceneTextures) a.albedo = textured_albedo(sc, id, a.albedo, a.normal);
     a.cov = 1.0f; a.t = t;
     return id;
 }
@@ -2463,14 +2509,16 @@ static bool wave_fits(const SceneDev& sc, long long regionPix, long long S)
     return wave_paths(regionPix, S) <= 0x7fffffffLL && sc.nLights < kKindFree;
 }
 
-// The slab queue (3), always while the environment is sampled (tpt_draw then never stores into mapped host memory),
+// The slab queue (3), always while the environment is sampled or textures are set (tpt_draw then never stores into
+// mapped host memory),
 // except: a draw into mapped host memory runs the group queue (8), which stores its finished pixels
 // itself; and where the sweep dwarfs everything else (>= 1024 spheres) and the slab queue cannot run a packed-pair sweep
 // (pair array does not fit, or "fast_kform" < 2), the block wavefront that sorts its paths by material before Scatter()
 // is faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312).
 int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy)
 {
-    if (sc.layout.flags & kSceneEnvSampling) return 3;       // the slab queue alone samples the environment
+    if (sc.layout.flags & (kSceneEnvSampling | kSceneTextures)) return 3;   // the slab queue alone samples the environment
+                                                                             // and looks up textures
     if (zeroCopy) return 8;
     const long long S = (long long)spp * (numFrames < kMaxFramesPerDraw ? numFrames : kMaxFramesPerDraw);   // first launch
     return sc.count >= 1024 && fast_queue_kform(sc) < 2 && wave_fits(sc, regionPix, S) ? 7 : 3;

@@ -39,7 +39,8 @@ struct FastVariantInfo
     bool writesFinalPixels;   // the trace kernel stores finished pixels itself (no L2 reductions), also into mapped host memory
     bool rowBands;            // a draw can be split into row bands, one launch per band
     bool progressCounters;    // the trace kernel can publish per-band completion counters (launch_fast's bandDone)
-    bool samplesEnvironment;  // runs the slab queue's environment-sampling instances ("environment_sampling")
+    bool referenceQueue;      // runs the slab queue's reference-form instances, which alone sample the environment
+                              // ("environment_sampling") and look up textures (tpt_set_textures)
 };
 FastVariantInfo fast_variant_info(int variant);
 // The variant a draw with "fast_variant" -1 runs over regionPix pixels of numFrames frames at spp; zeroCopy: the draw
@@ -69,8 +70,8 @@ cudaError_t launch_fast_rays(const DrawParams& p, const SceneDev& sc, long long 
 cudaError_t launch_fast_samples(const DrawParams& p, const SceneDev& sc, unsigned long long* badPixel, int numSMs,
                                 cudaStream_t stream);
 // The check of n int32 `list` against [0, limit) that the caller lists get before their trace kernel: the smallest
-// (entry << 32 | value) of an entry outside lands in *bad (device; ~0 when there is none). tpt_set_environment checks a
-// device map's channels with it, as their bits.
+// (entry << 32 | value) of an entry outside lands in *bad (device; ~0 when there is none). tpt_set_environment and
+// tpt_set_textures check device texels' channels with it, as their bits.
 cudaError_t launch_list_check(const int* list, long long n, long long limit, unsigned long long* bad, int numSMs,
                               cudaStream_t stream);
 // tpt_draw_aovs (rays = false: the region of p, frames [p.frame0, p.frame0 + p.numFrames) at p.spp, blended over the outputs

@@ -50,6 +50,9 @@ struct SceneView
     uint32_t envLo, envHi; // kSceneEnvironment: address of the envW x envH RGBA texels of the lat-long environment (row 0 =
     int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it; its sampling tables follow
                            // the texels (tpt_env_tables.h)
+    uint32_t texLo, texHi; // kSceneTextures: the texW x texH RGBA texels of tpt_set_textures' layers, layer-major (row 0 =
+    uint32_t tabLo, tabHi; // the +y pole, global memory), and the int32 layer of each sphere id below texSpheres (-1: none)
+    int texW, texH, texSpheres;
 };
 
 // Blob layout in global memory (one contiguous, 16 B-aligned allocation so a single bulk copy stages it
@@ -65,6 +68,13 @@ struct SceneBlobLayout
     // Not part of the blob: each call's copy of the layout gets them (begin_call).
     uint32_t envLo, envHi;
     int envW, envH;
+    // tpt_set_textures' layers (kSceneTextures), the same way: the texel and layer-table addresses in halves, the layer size,
+    // and the number of sphere ids the table covers (at most the scene's count, so padding spheres are never textured).
+    uint32_t texLo, texHi, tabLo, tabHi;
+    int texW, texH, texSpheres;
+    // unused: keeps the texture fields a multiple of 8 bytes, so the kernel parameters behind the layout keep the
+    // 8-byte pairing of their constant-bank loads (an odd number of added words changed untextured kernels' SASS)
+    uint32_t texPad;
 };
 
 // DO_MITSUBA_COMPARE (Config.h:25) as a runtime switch: constant sky (Test.cpp:226-227) and zero Metal roughness
@@ -79,7 +89,10 @@ struct SceneBlobLayout
 // kSceneEnvSampling ("environment_sampling" active for the call, set by begin_call with kSceneEnvironment): the slab
 // queue's sampling instances take one environment sample per light-sampled Lambert vertex (sample_env), with the map's
 // tables behind its texels (tpt_env_tables.h).
-enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u };
+// kSceneTextures (tpt_set_textures, set by begin_call): the slab queue's reference-form instances and the AOV kernel
+// multiply the albedo of a hit on a textured sphere by its layer's lat-long lookup at the hit's normal (textured_albedo).
+enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
+                             kSceneTextures = 16u };
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.
