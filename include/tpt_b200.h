@@ -96,8 +96,8 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
  * they are set, every hit of a TPT_MODE_FAST tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples and
  * tpt_trace_samples on a textured sphere uses albedo x T(n) wherever the untextured estimator uses the material's albedo:
  * a Lambert vertex's throughput (its light cones, its environment sample and its bounce, with "light_sampling" on or off)
- * and a Metal vertex's tint. Glass uses no albedo and emission is not textured. The lookup draws no random numbers, so
- * every sample stream stays where it was. tpt_trace_irradiance's starting vertex stays white; later vertices on textured
+ * and a Metal vertex's tint. Glass uses no albedo; emission has textures of its own (tpt_set_emission_textures). The
+ * lookup draws no random numbers, so every sample stream stays where it was. tpt_trace_irradiance's starting vertex stays white; later vertices on textured
  * spheres are textured. tpt_draw_aovs and tpt_trace_aovs report the textured albedo for every material type.
  *   n         the hit's shading normal (pos - centre) / radius.
  *   T(n)      the bilinear lookup of the sphere's layer in the direction n, with the mapping tpt_set_environment pins:
@@ -125,6 +125,32 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
  * "environment_sampling" run in the same instances and combine. */
 int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
                      const int* sphereLayers, int numSpheres, int onDevice);
+/* Emission textures for the fast mode: lat-long images bound to spheres by sphere id, the matching half of
+ * tpt_set_textures. While they are set, the emitted radiance of a hit on sphere id with shading normal n is
+ * emissive[id] x T(n), with T(n) the same bilinear lookup (mapping, orientation, blends) as tpt_set_textures' layers.
+ * It applies wherever a TPT_MODE_FAST tpt_draw, tpt_trace_rays, tpt_trace_irradiance, tpt_draw_samples and
+ * tpt_trace_samples add emission: a camera or caller ray's first hit, hits after Metal and glass bounces, Lambert hits
+ * with "light_sampling" 0, the ends of a path absorbed by Metal or failed by glass, the depth cap, and a light cone's
+ * shadow ray that reaches its light. There T is evaluated at the normal of the point where the shadow ray meets the
+ * light (not at the cone's axis or the sampled direction). The products are taken in that order: emissive x T first,
+ * then the throughput times that (on a light's shadow ray (throughput x albedo x (emissive x T)) x the cone's weight), so
+ * a constant layer c gives the bits of the untextured scene whose emission is emissive x c rounded to float.
+ * A sphere whose material emission is zero stays dark whatever its layer: the light list, and with it the set of spheres
+ * light sampling aims at, stays the one tpt_set_scene made, so the estimator stays unbiased with cone sampling left as it
+ * is (uniform in the light's subtended cone; only its variance depends on the texture). The lookup draws no random
+ * numbers, so every sample stream stays where it was. Spheres without a layer (-1), ids at or past numSpheres and the
+ * padding spheres of the sweep keep emissive[id]. tpt_draw_aovs and tpt_trace_aovs do not change, nor do
+ * tpt_trace_irradiance's self-skip rule and environment sampling. Albedo and emission textures on one sphere combine, each
+ * acting on its own term.
+ * Arguments, refusals (with the same error texts, headed tpt_set_emission_textures), NULL to remove, lifetime, ordering,
+ * memory (two device copies of 16 * width * height * layers + 4 * numSpheres bytes at most) and kernels are those of
+ * tpt_set_textures, and the two calls are independent: each has its own size, layers and sphere table, and either can
+ * be made without the other. While emission textures are set every fast call runs the instances that carry the lookups:
+ * tpt_draw's auto variant is 3 (host-buffer draws stage through the slab queue), 9 runs the 6-CTA instance, an explicit
+ * "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused, and tpt_draw in TPT_MODE_EXACT, TPT_MODE_REFGPU and
+ * TPT_MODE_REFGPU_FAST is refused. */
+int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
+                              const int* sphereLayers, int numSpheres, int onDevice);
 /* Camera only (UpdateTest rebuilds it every frame from the aspect ratio, Test.cpp:341). */
 int tpt_set_camera(tpt_context* ctx, const void* camera88);
 

@@ -88,6 +88,7 @@ def _load_lib():
     L.tpt_trace_samples.restype = ci
     L.tpt_set_environment.argtypes = [vp, vp, ci, ci, ci]; L.tpt_set_environment.restype = ci
     L.tpt_set_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_textures.restype = ci
+    L.tpt_set_emission_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_emission_textures.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -395,49 +396,63 @@ class Context:
         textured sphere uses albedo x the layer's lookup at its normal. None removes the textures. Refused here: other
         shapes and dtypes, negative (-0 included) or non-finite RGB values, and layers outside [-1, L). See
         include/tpt_b200.h for which calls and kernels use them."""
+        self._set_texture_set("set_textures", textures, sphere_layers)
+
+    def set_emission_textures(self, textures, sphere_layers=None):
+        """tpt_set_emission_textures: lat-long emission textures on spheres for the fast mode, independent of
+        set_textures. Takes the same inputs as set_textures and refuses the same ones. The emitted radiance of a hit on
+        a sphere with a layer is its material's emission x the layer's lookup at the hit's normal, also where a light
+        sampling shadow ray meets the light; a sphere with zero emission stays dark. None removes the textures. See
+        include/tpt_b200.h for where the estimator applies it."""
+        self._set_texture_set("set_emission_textures", textures, sphere_layers)
+
+    def _set_texture_set(self, name, textures, sphere_layers):
+        """set_textures and set_emission_textures (`name`): checks and stages their inputs for tpt_<name>, which is looked
+        up only once they pass."""
+        cname = "tpt_" + name
         if textures is None:
-            self._check(self._L.tpt_set_textures(self._h, None, 0, 0, 0, None, 0, 0), "tpt_set_textures")
+            self._check(getattr(self._L, cname)(self._h, None, 0, 0, 0, None, 0, 0), cname)
             return
         if not isinstance(textures, np.ndarray) and not hasattr(textures, "data_ptr"):
-            raise TptError("set_textures: textures must be a numpy array or a torch tensor")
+            raise TptError(f"{name}: textures must be a numpy array or a torch tensor")
         shape = tuple(textures.shape)
         if len(shape) != 4 or shape[3] not in (3, 4) or 0 in shape:
-            raise TptError(f"set_textures: textures must have shape (L, H, W, 3) or (L, H, W, 4) with L, H, W >= 1, not {shape}")
+            raise TptError(f"{name}: textures must have shape (L, H, W, 3) or (L, H, W, 4) with L, H, W >= 1, not {shape}")
         if sphere_layers is None:
-            raise TptError("set_textures: sphere_layers is required with textures")
+            raise TptError(f"{name}: sphere_layers is required with textures")
         layers = np.asarray(sphere_layers.cpu() if hasattr(sphere_layers, "cpu") else sphere_layers)
         if layers.ndim != 1 or layers.dtype.kind not in "iu":
-            raise TptError(f"set_textures: sphere_layers must be a 1-D integer array, not {layers.dtype} of shape {layers.shape}")
+            raise TptError(f"{name}: sphere_layers must be a 1-D integer array, not {layers.dtype} of shape {layers.shape}")
         bad = np.nonzero((layers < -1) | (layers >= shape[0]))[0]
         if bad.size:
             i = int(bad[0])
-            raise TptError(f"set_textures: sphere_layers[{i}] = {int(layers[i])} is outside [-1, {shape[0]})")
+            raise TptError(f"{name}: sphere_layers[{i}] = {int(layers[i])} is outside [-1, {shape[0]})")
         layers = np.ascontiguousarray(layers, dtype=np.int32)
         if isinstance(textures, np.ndarray):
             if textures.dtype != np.float32:
-                raise TptError(f"set_textures: textures must be float32, not {textures.dtype}")
+                raise TptError(f"{name}: textures must be float32, not {textures.dtype}")
             rgb = textures[..., :3]
             if not np.isfinite(rgb).all() or np.signbit(rgb).any():
-                raise TptError("set_textures: RGB values must be finite and not negative (-0 included)")
+                raise TptError(f"{name}: RGB values must be finite and not negative (-0 included)")
             rgba = np.zeros(shape[:3] + (4,), np.float32)
             rgba[..., :shape[3]] = textures
             addr, on_dev = rgba.ctypes.data, False
         else:
             import torch
             if textures.dtype != torch.float32:
-                raise TptError(f"set_textures: textures must be float32, not {textures.dtype}")
+                raise TptError(f"{name}: textures must be float32, not {textures.dtype}")
             rgb = textures[..., :3]
             if not bool(torch.isfinite(rgb).all()) or bool(torch.signbit(rgb).any()):
-                raise TptError("set_textures: RGB values must be finite and not negative (-0 included)")
+                raise TptError(f"{name}: RGB values must be finite and not negative (-0 included)")
             rgba = torch.zeros(shape[:3] + (4,), dtype=torch.float32, device=textures.device)
             rgba[..., :shape[3]] = textures
             on_dev = bool(rgba.is_cuda)
             if on_dev:
                 torch.cuda.current_stream(rgba.device).synchronize()   # the library reads it on its own stream
             addr = int(rgba.data_ptr())
-        self._check(self._L.tpt_set_textures(self._h, ctypes.c_void_p(addr), shape[2], shape[1], shape[0],
-                                             layers.ctypes.data if layers.size else None, int(layers.size),
-                                             1 if on_dev else 0), "tpt_set_textures")
+        self._check(getattr(self._L, cname)(self._h, ctypes.c_void_p(addr), shape[2], shape[1], shape[0],
+                                            layers.ctypes.data if layers.size else None, int(layers.size),
+                                            1 if on_dev else 0), cname)
 
     def set_camera(self, camera: np.ndarray):
         camera = np.ascontiguousarray(camera)

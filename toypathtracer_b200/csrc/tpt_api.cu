@@ -21,7 +21,8 @@ thread_local KernelRecord tpt::t_lastKernels = {};
 // tpt_tonemap_rgba8, tpt_trace_rays' out4 and tpt_draw_samples' sum4; the others hold the buffers they are named after.
 enum Staging { kStageImage, kStageRays, kStageAlbedo, kStageNormal, kStageIds, kStagePixels, kStageSq4, kNumStaging };
 
-// Set-up data that the calls read on the device (tpt_set_environment's map, tpt_set_textures' layers), in two device slots
+// Set-up data that the calls read on the device (tpt_set_environment's map, tpt_set_textures' and
+// tpt_set_emission_textures' layers), in two device slots
 // with the scene blob's discipline: a new upload goes into the slot that is not current, on the upload stream after that
 // slot's last use (slot_begin_upload, slot_finish_upload); calls wait on the current slot's upload and mark its last use
 // (begin_call and finish_call through slot_use and slot_used). So a call keeps the data it was issued with, even while
@@ -34,6 +35,14 @@ struct DeviceSlots
     bool have = false;                            // the calls issued from now on read slot `cur`
     cudaEvent_t uploadDone[2] = {nullptr, nullptr};
     cudaEvent_t lastUse[2] = {nullptr, nullptr};
+};
+
+// One set of sphere textures (tpt_set_textures' albedo, tpt_set_emission_textures' emission): its slots, each
+// [layers x h x w float4 texels][spheres int32 layers], and the sizes of the current one.
+struct TextureSlots
+{
+    DeviceSlots slots;
+    int w = 0, h = 0, layers = 0, spheres = 0;
 };
 
 struct tpt_context
@@ -66,14 +75,14 @@ struct tpt_context
     bool haveScene = false;
     int spp = 4;
 
-    // environment (tpt_set_environment) and textures (tpt_set_textures): each in its own DeviceSlots. They belong to the
-    // context, not to the scene: tpt_set_scene leaves them alone.
+    // environment (tpt_set_environment), albedo textures (tpt_set_textures) and emission textures
+    // (tpt_set_emission_textures): each in its own DeviceSlots. They belong to the context, not to the scene:
+    // tpt_set_scene leaves them alone.
     DeviceSlots env;
     int envW = 0, envH = 0;                       // of the current slot
     bool envSampleable = false;                   // the current slot's map has sampling tables (some weight is not zero)
     int envSampling = 0;                          // "environment_sampling"
-    DeviceSlots tex;                              // [layers x texH x texW float4 texels][texSpheres int32 layers]
-    int texW = 0, texH = 0, texLayers = 0, texSpheres = 0;   // of the current slot
+    TextureSlots tex, emit;
 
     // options
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
@@ -247,7 +256,7 @@ int tpt_create(int device, tpt_context** out)
     {
         e = cudaEventCreateWithFlags(&ctx->uploadDone[i], cudaEventDisableTiming);
         if (e == cudaSuccess) e = cudaEventCreateWithFlags(&ctx->blobLastUse[i], cudaEventDisableTiming);
-        for (DeviceSlots* s : {&ctx->env, &ctx->tex})
+        for (DeviceSlots* s : {&ctx->env, &ctx->tex.slots, &ctx->emit.slots})
         {
             if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->uploadDone[i], cudaEventDisableTiming);
             if (e == cudaSuccess) e = cudaEventCreateWithFlags(&s->lastUse[i], cudaEventDisableTiming);
@@ -295,7 +304,7 @@ void tpt_destroy(tpt_context* ctx)
         if (ctx->hBlob[i]) cudaFreeHost(ctx->hBlob[i]);
         if (ctx->uploadDone[i]) cudaEventDestroy(ctx->uploadDone[i]);
         if (ctx->blobLastUse[i]) cudaEventDestroy(ctx->blobLastUse[i]);
-        for (DeviceSlots* s : {&ctx->env, &ctx->tex})
+        for (DeviceSlots* s : {&ctx->env, &ctx->tex.slots, &ctx->emit.slots})
         {
             cudaFree(s->ptr[i]);
             if (s->uploadDone[i]) cudaEventDestroy(s->uploadDone[i]);
@@ -499,6 +508,27 @@ static int slot_used(tpt_context* ctx, const DeviceSlots& s, cudaStream_t stream
     return 0;
 }
 
+// begin_call's part for one texture set, while it is set: the call reads its current slot (slot_use), sees `flag` and
+// gets the slot's addresses and sizes in *out.
+static int use_textures(tpt_context* ctx, const TextureSlots& ts, cudaStream_t stream, const char* what, uint32_t flag,
+                        SceneDev* scene, TexSet* out)
+{
+    if (!ts.slots.have) return 0;
+    uint64_t tex = 0;
+    if (int r = slot_use(ctx, ts.slots, stream, what, &tex)) return r;
+    const uint64_t tab = tex + (uint64_t)16 * ts.w * ts.h * ts.layers;
+    scene->layout.flags |= flag;
+    out->texLo = (uint32_t)tex;
+    out->texHi = (uint32_t)(tex >> 32);
+    out->tabLo = (uint32_t)tab;
+    out->tabHi = (uint32_t)(tab >> 32);
+    out->W = ts.w;
+    out->H = ts.h;
+    // sphere ids past the scene's count are padding spheres, which are never textured
+    out->spheres = ts.spheres < scene->count ? ts.spheres : scene->count;
+    return 0;
+}
+
 // Prologue of a call that traces (tpt_draw, tpt_trace_rays). One context = one scene blob, one set of counters: calls are
 // ordered in issue order even across streams, and the scene they read must have landed (tpt_set_scene uploads
 // asynchronously on its own stream). Returns the call's stream and the scene with the context's sweep-form option applied.
@@ -523,21 +553,9 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
         if (ctx->envSampling && ctx->envSampleable && !(scene->layout.flags & kSceneNoLightSampling))
             scene->layout.flags |= kSceneEnvSampling;
     }
-    if (ctx->tex.have)
-    {
-        uint64_t tex = 0;
-        if (int r = slot_use(ctx, ctx->tex, *stream, "textures", &tex)) return r;
-        const uint64_t tab = tex + (uint64_t)16 * ctx->texW * ctx->texH * ctx->texLayers;
-        scene->layout.flags |= kSceneTextures;
-        scene->layout.texLo = (uint32_t)tex;
-        scene->layout.texHi = (uint32_t)(tex >> 32);
-        scene->layout.tabLo = (uint32_t)tab;
-        scene->layout.tabHi = (uint32_t)(tab >> 32);
-        scene->layout.texW = ctx->texW;
-        scene->layout.texH = ctx->texH;
-        // sphere ids past the scene's count are padding spheres, which are never textured
-        scene->layout.texSpheres = ctx->texSpheres < scene->count ? ctx->texSpheres : scene->count;
-    }
+    if (int r = use_textures(ctx, ctx->tex, *stream, "textures", kSceneTextures, scene, &scene->layout.tex)) return r;
+    if (int r = use_textures(ctx, ctx->emit, *stream, "emission textures", kSceneEmissionTextures, scene, &scene->layout.emit))
+        return r;
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
     scene->pairs.half = scene->halfOk && scene->kformOk && ctx->fastKForm == 2;
@@ -588,7 +606,8 @@ static int finish_call(tpt_context* ctx, cudaStream_t stream, int n, bool hostBu
     CK(cudaEventRecord(ctx->lastDraw, stream), "draw end event");
     CK(cudaEventRecord(ctx->blobLastUse[ctx->curBlob], stream), "scene last-use event");
     if (int r = slot_used(ctx, ctx->env, stream, "environment")) return r;
-    if (int r = slot_used(ctx, ctx->tex, stream, "textures")) return r;
+    if (int r = slot_used(ctx, ctx->tex.slots, stream, "textures")) return r;
+    if (int r = slot_used(ctx, ctx->emit.slots, stream, "emission textures")) return r;
     ctx->lastDrawStream = stream; ctx->haveLastDraw = true;
     if (outRayCount || outPerFrame)
     {
@@ -907,9 +926,13 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode != TPT_MODE_FAST && ctx->env.have)
         return fail_msg(ctx, "tpt_draw: an environment is set, and only TPT_MODE_FAST draws use one (clear it with "
                              "tpt_set_environment(ctx, NULL, 0, 0, 0) for exact and reference-GPU draws)");
-    if (mode != TPT_MODE_FAST && ctx->tex.have)
-        return fail_msg(ctx, "tpt_draw: textures are set, and only TPT_MODE_FAST draws use them (clear them with "
-                             "tpt_set_textures(ctx, NULL, 0, 0, 0, NULL, 0, 0) for exact and reference-GPU draws)");
+    if (mode != TPT_MODE_FAST && (ctx->tex.slots.have || ctx->emit.slots.have))
+    {
+        const bool albedo = ctx->tex.slots.have;
+        return fail_msgf(ctx, "tpt_draw: %s are set, and only TPT_MODE_FAST draws use them (clear them with "
+                              "%s(ctx, NULL, 0, 0, 0, NULL, 0, 0) for exact and reference-GPU draws)",
+                         albedo ? "textures" : "emission textures", albedo ? "tpt_set_textures" : "tpt_set_emission_textures");
+    }
     // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
     if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
@@ -918,14 +941,18 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
     // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment and look up textures
     const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
-    const bool textured = (scene.layout.flags & kSceneTextures) != 0;
+    const bool textured = (scene.layout.flags & kSceneAnyTextures) != 0;
     if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
         return fail_msgf(ctx, "tpt_draw: \"environment_sampling\" is active (option on, a map with non-zero weight, light "
                               "sampling on), and fast_variant %d does not sample the environment: use -1 (auto), 3 or 9",
                          ctx->fastVariant);
     if (textured && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
-        return fail_msgf(ctx, "tpt_draw: textures are set (tpt_set_textures), and fast_variant %d does not look them up: "
-                              "use -1 (auto), 3 or 9", ctx->fastVariant);
+    {
+        const bool albedo = (scene.layout.flags & kSceneTextures) != 0;
+        return fail_msgf(ctx, "tpt_draw: %s are set (%s), and fast_variant %d does not look them up: use -1 (auto), 3 or 9",
+                         albedo ? "textures" : "emission textures", albedo ? "tpt_set_textures" : "tpt_set_emission_textures",
+                         ctx->fastVariant);
+    }
 
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);
@@ -1279,13 +1306,13 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
     return 0;
 }
 
-int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
-                     const int* sphereLayers, int numSpheres, int onDevice)
+// tpt_set_textures and tpt_set_emission_textures: the checks, the upload into one set's slots and its sizes. `fn` heads
+// the error texts, `what` names the set in those of CUDA failures.
+static int set_textures(tpt_context* ctx, TextureSlots& ts, const char* fn, const char* what, const float* rgba, int width,
+                        int height, int layers, const int* sphereLayers, int numSpheres, int onDevice)
 {
-    static const char* fn = "tpt_set_textures";
-    if (!ctx) return (int)cudaErrorInvalidValue;
-    // NULL: the calls issued from now on see every sphere untextured; those in flight keep reading their slot
-    if (!rgba) { ctx->tex.have = false; return 0; }
+    // NULL: the calls issued from now on see every sphere without this set; those in flight keep reading their slot
+    if (!rgba) { ts.slots.have = false; return 0; }
     if (width < 1 || height < 1 || layers < 1)
         return fail_msgf(ctx, "%s: width, height and layers must be >= 1 (got %d x %d x %d)", fn, width, height, layers);
     const long long plane = (long long)width * height, n = plane * layers;
@@ -1310,12 +1337,12 @@ int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height,
         for (long long i = 0; i < n; ++i)
             for (int c = 0; c < 3; ++c)
                 if (!env_channel_ok(rgba[4 * i + c])) return bad_texel(i, c, rgba[4 * i + c]);
-    // The slot that is not current: the calls issued since the last tpt_set_textures read the other one. It holds the
+    // The slot that is not current: the calls issued since the set's last upload read the other one. It holds the
     // texels and the sphere table behind them: 16 W H L + 4 numSpheres bytes.
     const size_t texBytes = (size_t)n * 16, bytes = texBytes + (size_t)numSpheres * 4;
     int slot = 0;
-    if (int r = slot_begin_upload(ctx, ctx->tex, bytes, "textures", &slot)) return r;
-    unsigned char* dst = (unsigned char*)ctx->tex.ptr[slot];
+    if (int r = slot_begin_upload(ctx, ts.slots, bytes, what, &slot)) return r;
+    unsigned char* dst = (unsigned char*)ts.slots.ptr[slot];
     cudaStream_t s = ctx->uploadStream;
     if (onDevice)
     {
@@ -1347,12 +1374,28 @@ int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height,
         CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyHostToDevice, s), "texture upload");
     if (numSpheres > 0)
         CK(cudaMemcpyAsync(dst + texBytes, sphereLayers, (size_t)numSpheres * 4, cudaMemcpyHostToDevice, s), "sphere layer upload");
-    if (int r = slot_finish_upload(ctx, ctx->tex, slot, "textures")) return r;
-    ctx->texW = width;
-    ctx->texH = height;
-    ctx->texLayers = layers;
-    ctx->texSpheres = numSpheres;
+    if (int r = slot_finish_upload(ctx, ts.slots, slot, what)) return r;
+    ts.w = width;
+    ts.h = height;
+    ts.layers = layers;
+    ts.spheres = numSpheres;
     return 0;
+}
+
+int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
+                     const int* sphereLayers, int numSpheres, int onDevice)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    return set_textures(ctx, ctx->tex, "tpt_set_textures", "textures", rgba, width, height, layers, sphereLayers, numSpheres,
+                        onDevice);
+}
+
+int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
+                              const int* sphereLayers, int numSpheres, int onDevice)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    return set_textures(ctx, ctx->emit, "tpt_set_emission_textures", "emission textures", rgba, width, height, layers,
+                        sphereLayers, numSpheres, onDevice);
 }
 
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStreamArg, long long* outRays)

@@ -110,13 +110,8 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     v.envHi = L.envHi;
     v.envW = L.envW;
     v.envH = L.envH;
-    v.texLo = L.texLo;
-    v.texHi = L.texHi;
-    v.tabLo = L.tabLo;
-    v.tabHi = L.tabHi;
-    v.texW = L.texW;
-    v.texH = L.texH;
-    v.texSpheres = L.texSpheres;
+    v.tex = L.tex;
+    v.emit = L.emit;
     return v;
 }
 

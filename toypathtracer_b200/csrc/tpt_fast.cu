@@ -905,7 +905,7 @@ __device__ __forceinline__ V3 metal_dir(V3 d, V3 normal, float roughness, uint32
 // u = (phi + pi) / 2pi * W, v = theta / pi * H, texel (i, j) centred at (i + 1/2, j + 1/2), row 0 at +y; columns wrapping,
 // rows clamped. Every blend is a + f * (b - a), so a constant image returns its constant bit for bit. Four 128-bit
 // read-only loads; RGB: twelve 32-bit ones of R, G and B only, at 32-bit texel offsets (fewer registers live: the texture
-// instances stay at 80 without spilling). The environment map (env_radiance) and the sphere textures (textured_albedo)
+// instances stay at 80 without spilling). The environment map (env_radiance) and the sphere textures (sphere_texture)
 // both read through it.
 // CELL: also the sampling probability P of the cell [i, i+1) x [j, j+1) that holds (u + 1/2, v + 1/2), from the alpha of
 // whichever of the four texels that is (tpt_env_tables.h).
@@ -954,18 +954,32 @@ __device__ __forceinline__ V3 env_radiance(const SceneView& sc, V3 d, float* cel
     return latlong_lookup<CELL>(env, sc.envW, sc.envH, d, cellP);
 }
 
-// tpt_set_textures (kSceneTextures, the caller checks the flag): the albedo of a hit on sphere `id` with shading normal n
-// ((pos - centre) / r): albedo x the lookup of the sphere's layer at n, or albedo itself for a sphere without a layer
-// (-1, or an id at or past texSpheres, which begin_call keeps at most the scene's count: padding spheres have none).
-// Draws no random numbers.
-__device__ __forceinline__ V3 textured_albedo(const SceneView& sc, int id, V3 albedo, V3 n)
+// The layer of sphere `id` in the texture set ts (sc.tex: tpt_set_textures' albedo; sc.emit: tpt_set_emission_textures'
+// emission; the caller checks the set's flag), or -1 for a sphere without one (-1 in the table, or an id at or past
+// ts.spheres, which begin_call keeps at most the scene's count: padding spheres have none).
+__device__ __forceinline__ int sphere_layer(const TexSet& ts, int id)
 {
-    if (id >= sc.texSpheres) return albedo;
-    const int* tab = reinterpret_cast<const int*>(((uint64_t)sc.tabHi << 32) | sc.tabLo);
-    const int layer = __ldg(tab + id);
-    if (layer < 0) return albedo;
-    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)sc.texHi << 32) | sc.texLo);
-    return albedo * latlong_lookup<false, true>(tex + (uint32_t)(layer * sc.texW * sc.texH), sc.texW, sc.texH, n);
+    if (id >= ts.spheres) return -1;
+    return __ldg(reinterpret_cast<const int*>(((uint64_t)ts.tabHi << 32) | ts.tabLo) + id);
+}
+
+// base x the lookup of layer `layer` (>= 0) of ts at the shading normal n ((pos - centre) / r): the texture's product
+// comes first, so a constant layer c gives base x c rounded once. Draws no random numbers.
+__device__ __forceinline__ V3 sphere_texture_layer(const TexSet& ts, int layer, V3 base, V3 n)
+{
+    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)ts.texHi << 32) | ts.texLo);
+    return base * latlong_lookup<false, true>(tex + (uint32_t)(layer * ts.W * ts.H), ts.W, ts.H, n);
+}
+
+// The textured value of a hit on sphere `id` with shading normal n: base (the material's albedo or emission) x the
+// lookup of the sphere's layer in ts at n, or base itself for a sphere without a layer (sphere_layer's test, as early
+// returns: the AOV kernel's code stays what it was before emission textures).
+__device__ __forceinline__ V3 sphere_texture(const TexSet& ts, int id, V3 base, V3 n)
+{
+    if (id >= ts.spheres) return base;
+    const int layer = __ldg(reinterpret_cast<const int*>(((uint64_t)ts.tabHi << 32) | ts.tabLo) + id);
+    if (layer < 0) return base;
+    return sphere_texture_layer(ts, layer, base, n);
 }
 
 // What a fast path sees when it leaves the scene: the caller's environment while one is set, else the reference sky
@@ -1078,8 +1092,10 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // 768-thread light-sampling instances).
 // NEXT false: stop before lambert_next, for a caller that runs it later (the block wavefront). A Lambert vertex just shaded
 // and a returning shadow ray then leave the light to go on from in st.kind.
-// TEX: where the call's kSceneTextures is set, Lambert and Metal hits take textured_albedo for the material's albedo (the
-// slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while textures are set).
+// TEX: where the call's kSceneTextures is set, Lambert and Metal hits take the textured albedo for the material's albedo,
+// and where its kSceneEmissionTextures is set, every hit takes the textured emission for the material's emission and a
+// light's shadow ray that reaches it the light's emission x its layer's lookup at the normal where the ray meets it (the
+// slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while either is set).
 template <int LS, int ENVM = 1, bool NEXT = true, bool TEX = false, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
@@ -1115,7 +1131,11 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 int mtype = mat.type;
                 // Lambert and Metal use the albedo (glass does not): with textures, the textured one
                 if constexpr (TEX)
-                    if ((sc.flags & kSceneTextures) && mtype != kDielectric) mat.albedo = textured_albedo(sc, id, mat.albedo, normal);
+                {
+                    if ((sc.flags & kSceneTextures) && mtype != kDielectric) mat.albedo = sphere_texture(sc.tex, id, mat.albedo, normal);
+                    // every emission this hit adds below is mat.emissive: with emission textures, the textured one
+                    if (sc.flags & kSceneEmissionTextures) mat.emissive = sphere_texture(sc.emit, id, mat.emissive, normal);
+                }
                 if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
                 else if (LS == kLsOff && mtype == kLambert)
                 {
@@ -1176,7 +1196,19 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         {
             const int j = st.kind - 1;
             const LightRec& Lj = sc.lights[j];
-            if (id == Lj.id) st.col = st.col + (st.thrAlb * v3(Lj.ex, Lj.ey, Lj.ez)) * st.pend;
+            if (id == Lj.id)
+            {
+                V3 e = v3(Lj.ex, Lj.ey, Lj.ez);
+                // an emission-textured light: its layer's lookup at the normal of the point where the shadow ray meets it
+                if constexpr (TEX)
+                    if (sc.flags & kSceneEmissionTextures)
+                    {
+                        const int layer = sphere_layer(sc.emit, id);
+                        if (layer >= 0)
+                            e = sphere_texture_layer(sc.emit, layer, e, (st.o + st.d * t - v3(Lj.cx, Lj.cy, Lj.cz)) * sc.invRadius[id]);
+                    }
+                st.col = st.col + (st.thrAlb * e) * st.pend;
+            }
             wantLight = true; lightFrom = j + 1;
         }
     }
@@ -2192,7 +2224,7 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     QueuePick q;
     q.kform = fast_queue_kform(sc);
     // the environment-sampling and texture instances sweep in the reference form (env_mode, tex_mode)
-    const bool refInstances = (sc.layout.flags & (kSceneEnvSampling | kSceneTextures)) != 0;
+    const bool refInstances = (sc.layout.flags & (kSceneEnvSampling | kSceneAnyTextures)) != 0;
     if (refInstances) q.kform = 0;
     // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
     // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2). The same
@@ -2205,7 +2237,7 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
     const long long slabsPerWarp = ((regionPix + kSlabPix - 1) / kSlabPix) * samples / ((long long)numSMs * 32);
     // the 8-CTA instances have no environment lookup (at 64 registers it made them spill) and no texture lookup: with
     // either set, the 6-CTA ones run
-    const bool eight = !(sc.layout.flags & (kSceneEnvironment | kSceneTextures)) && (variant == 9 || (variant == 3 && slabsPerWarp >= 48));
+    const bool eight = !(sc.layout.flags & (kSceneEnvironment | kSceneAnyTextures)) && (variant == 9 || (variant == 3 && slabsPerWarp >= 48));
     q.threads = big ? TPT_BIG_THREADS : 128;
     if (big) q.kern = queue_kernel<SRC, MOMENTS, TPT_BIG_THREADS, 1>(sc, q.kform);
     else if (q.kform == 4)
@@ -2385,7 +2417,7 @@ __device__ __forceinline__ int aov_sample(const SceneView& sc, const Hitter& hit
     const Q4 m = sc.matA[id < sc.count ? id : sc.count];         // a padded sphere (form 0) has the all-zero material
     a.albedo = v3(m.x, m.y, m.z);
     // the textured albedo for every material type (this kernel is not on a draw's path: a runtime branch is enough)
-    if (sc.flags & kSceneTextures) a.albedo = textured_albedo(sc, id, a.albedo, a.normal);
+    if (sc.flags & kSceneTextures) a.albedo = sphere_texture(sc.tex, id, a.albedo, a.normal);
     a.cov = 1.0f; a.t = t;
     return id;
 }
@@ -2517,7 +2549,7 @@ static bool wave_fits(const SceneDev& sc, long long regionPix, long long S)
 // is faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312).
 int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy)
 {
-    if (sc.layout.flags & (kSceneEnvSampling | kSceneTextures)) return 3;   // the slab queue alone samples the environment
+    if (sc.layout.flags & (kSceneEnvSampling | kSceneAnyTextures)) return 3;   // the slab queue alone samples the environment
                                                                              // and looks up textures
     if (zeroCopy) return 8;
     const long long S = (long long)spp * (numFrames < kMaxFramesPerDraw ? numFrames : kMaxFramesPerDraw);   // first launch

@@ -28,9 +28,7 @@ inline SceneBlobLayout scene_blob_layout(int count, int nLights)
     L.flags = 0;
     L.envLo = L.envHi = 0;
     L.envW = L.envH = 0;
-    L.texLo = L.texHi = L.tabLo = L.tabHi = 0;
-    L.texW = L.texH = L.texSpheres = 0;
-    L.texPad = 0;
+    L.tex = L.emit = TexSet{};
     return L;
 }
 
@@ -180,8 +178,7 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.sphShared = 0;
     v.envLo = v.envHi = 0;     // host views never look up an environment
     v.envW = v.envH = 0;
-    v.texLo = v.texHi = v.tabLo = v.tabHi = 0;     // nor textures
-    v.texW = v.texH = v.texSpheres = 0;
+    v.tex = v.emit = TexSet{};     // nor textures
     return v;
 }
 

@@ -30,6 +30,20 @@ struct alignas(16) LightRec
     int id;
 };
 
+// One set of lat-long sphere textures as the kernels see it (tpt_set_textures, tpt_set_emission_textures): the address
+// of its W x H RGBA texels, layer-major (row 0 = the +y pole, global memory) and of the int32 layer of each sphere id below
+// `spheres` (-1: none; begin_call keeps `spheres` at most the scene's count, so padding spheres are never textured). The
+// addresses travel as 32-bit halves, which keeps the struct 4-byte aligned (an 8-byte aligned kernel parameter changes
+// how the compiler loads the fields around it). `pad` is unused: it keeps the struct a multiple of 8 bytes, so the kernel
+// parameters behind SceneBlobLayout keep the 8-byte pairing of their constant-bank loads (an odd number of added words
+// changed untextured kernels' SASS).
+struct TexSet
+{
+    uint32_t texLo, texHi, tabLo, tabHi;
+    int W, H, spheres;
+    uint32_t pad;
+};
+
 // Device-side scene, SoA, padded like the reference's SpheresSoA (Maths.h:368-404):
 //   sph[i]  = {centerX, centerY, centerZ, sqRadius}, i < simdCount, entries >= count are the
 //             "impossible" spheres (centre 10000, r^2 = 0, invRadius 0)
@@ -50,9 +64,8 @@ struct SceneView
     uint32_t envLo, envHi; // kSceneEnvironment: address of the envW x envH RGBA texels of the lat-long environment (row 0 =
     int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it; its sampling tables follow
                            // the texels (tpt_env_tables.h)
-    uint32_t texLo, texHi; // kSceneTextures: the texW x texH RGBA texels of tpt_set_textures' layers, layer-major (row 0 =
-    uint32_t tabLo, tabHi; // the +y pole, global memory), and the int32 layer of each sphere id below texSpheres (-1: none)
-    int texW, texH, texSpheres;
+    TexSet tex;            // kSceneTextures: tpt_set_textures' albedo layers
+    TexSet emit;           // kSceneEmissionTextures: tpt_set_emission_textures' emission layers
 };
 
 // Blob layout in global memory (one contiguous, 16 B-aligned allocation so a single bulk copy stages it
@@ -68,13 +81,9 @@ struct SceneBlobLayout
     // Not part of the blob: each call's copy of the layout gets them (begin_call).
     uint32_t envLo, envHi;
     int envW, envH;
-    // tpt_set_textures' layers (kSceneTextures), the same way: the texel and layer-table addresses in halves, the layer size,
-    // and the number of sphere ids the table covers (at most the scene's count, so padding spheres are never textured).
-    uint32_t texLo, texHi, tabLo, tabHi;
-    int texW, texH, texSpheres;
-    // unused: keeps the texture fields a multiple of 8 bytes, so the kernel parameters behind the layout keep the
-    // 8-byte pairing of their constant-bank loads (an odd number of added words changed untextured kernels' SASS)
-    uint32_t texPad;
+    // tpt_set_textures' albedo layers (kSceneTextures) and tpt_set_emission_textures' emission layers
+    // (kSceneEmissionTextures), the same way.
+    TexSet tex, emit;
 };
 
 // DO_MITSUBA_COMPARE (Config.h:25) as a runtime switch: constant sky (Test.cpp:226-227) and zero Metal roughness
@@ -90,9 +99,13 @@ struct SceneBlobLayout
 // queue's sampling instances take one environment sample per light-sampled Lambert vertex (sample_env), with the map's
 // tables behind its texels (tpt_env_tables.h).
 // kSceneTextures (tpt_set_textures, set by begin_call): the slab queue's reference-form instances and the AOV kernel
-// multiply the albedo of a hit on a textured sphere by its layer's lat-long lookup at the hit's normal (textured_albedo).
+// multiply the albedo of a hit on a textured sphere by its layer's lat-long lookup at the hit's normal (sphere_texture).
+// kSceneEmissionTextures (tpt_set_emission_textures, set by begin_call): the same instances multiply the emission of a hit
+// on a sphere with an emission layer, and that of a light where its shadow ray meets it, by the layer's lookup there.
 enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
-                             kSceneTextures = 16u };
+                             kSceneTextures = 16u, kSceneEmissionTextures = 32u };
+// Either texture set: the calls that have one run the instances that look textures up (pick_queue, fast_auto_variant).
+constexpr uint32_t kSceneAnyTextures = kSceneTextures | kSceneEmissionTextures;
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.
