@@ -142,9 +142,13 @@ int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height,
  * padding spheres of the sweep keep emissive[id]. tpt_draw_aovs and tpt_trace_aovs do not change, nor do
  * tpt_trace_irradiance's self-skip rule and environment sampling. Albedo and emission textures on one sphere combine, each
  * acting on its own term.
- * Arguments, refusals (with the same error texts, headed tpt_set_emission_textures), NULL to remove, lifetime, ordering,
- * memory (two device copies of 16 * width * height * layers + 4 * numSpheres bytes at most) and kernels are those of
- * tpt_set_textures, and the two calls are independent: each has its own size, layers and sphere table, and either can
+ * "emission_texture_sampling" (tpt_set_option) adds a sample drawn from a light's layer to its cone sample, from sampling
+ * tables this call builds on the host for every layer (device texels are copied back for it).
+ * Arguments, refusals (with the same error texts, headed tpt_set_emission_textures), NULL to remove, lifetime, ordering
+ * and kernels are those of tpt_set_textures. Memory: two device copies of 24 * width * height * layers +
+ * 8 * height * layers + 4 * numSpheres bytes (+ 4 when numSpheres is odd) at most: the texels (their alpha holds each
+ * cell's sampling probability), the sphere table and the sampling tables (toypathtracer_b200/csrc/tpt_env_tables.h). The
+ * two calls are independent: each has its own size, layers and sphere table, and either can
  * be made without the other. While emission textures are set every fast call runs the instances that carry the lookups:
  * tpt_draw's auto variant is 3 (host-buffer draws stage through the slab queue), 9 runs the 6-CTA instance, an explicit
  * "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused, and tpt_draw in TPT_MODE_EXACT, TPT_MODE_REFGPU and
@@ -210,7 +214,32 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * auto variant is 3 (never 7 or 8;
  * host-buffer draws stage through the slab queue instead of storing into page-locked memory), 9 runs the 6-CTA
  * instance, and an explicit "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused; Metal and glass vertices, Lambert
- * vertices hit from inside their sphere, the AOV calls and the exact and reference-GPU modes do not sample it). */
+ * vertices hit from inside their sphere, the AOV calls and the exact and reference-GPU modes do not sample it),
+ * "emission_texture_sampling" (default 0; any non-zero value is 1: fast calls importance-sample each light that has an
+ * emission layer by that layer; an estimator switch like "environment_sampling": unbiased, outputs differ from the default;
+ * read by each call when it is issued, not a scene flag, so toggling it uploads nothing. Active for a call (kSceneEmitSampling)
+ * only with the option on, emission textures set, "light_sampling" on and some layer with a non-zero weight; a call where
+ * it is not active runs exactly as without it (same kernel, streams and ray counts). At a light-sampled Lambert vertex o
+ * with facing normal nl, each light j it samples (never its own sphere) whose sphere has a sampleable layer gets, right
+ * after its cone sample (2 draws, its shadow ray traced as before), one texture sample: six draws in sample_env's order
+ * (row, row alias test, column, column alias test, u offset, v offset) from the layer's tables give the unit normal n_x by
+ * the inverse lat-long mapping and the point x = c + r n_x. Its shadow ray, along l = normalize(x - o), is traced (and
+ * counted in the call's rays) only when x faces o (n_x . (o - x) > 0), m = l . nl > 0 and sin theta_x > 0; the next light
+ * follows, then the environment sample, then the bounce. Densities in solid angle at o: the cone's pc = 1 / omega,
+ * omega = 2 pi (1 - cos_max) as the cone sampler computes it, and the texture sample's
+ * pt(x) = P_cell(n_x) W H / (2 pi^2 sin theta_x) / r^2 * |x - o|^2 / cos_x, cos_x = n_x . normalize(o - x), P_cell the
+ * realised probability of the layer cell that holds x's (u, v). Weights, the power heuristic with one sample each: a cone ray that reaches
+ * light j at x adds (throughput x albedo x (emissive x T(n_x))) x m omega / pi x pc^2 / (pc^2 + pt(x)^2); a texture ray
+ * that reaches it adds the same product, T at the normal where it meets the light, times (m / pi) pt / (pt^2 + pc^2),
+ * fixed when the sample is drawn (the kernels evaluate both with q = pt omega, which is the same value). A light without
+ * a layer, with layer -1, or with a layer whose weights are all zero draws nothing extra and its cone ray keeps full
+ * weight; so does every light at a vertex inside or on it (d <= r). Metal and glass vertices, "light_sampling" 0, the
+ * AOV calls and the exact and reference-GPU modes are unchanged; tpt_trace_irradiance, tpt_draw_samples and
+ * tpt_trace_samples sample as draws do. Tables: built by tpt_set_emission_textures for every layer whether or not the
+ * option is on, as tpt_set_environment builds the map's: the same weights (sin theta x the 3 x 3 maximum of mean RGB), alias
+ * tables and realised probabilities; they cost 8 * width * height * layers + 8 * height * layers bytes per device copy,
+ * plus 4 bytes of padding behind an odd sphere table. Kernels and routing are emission textures': the slab queue's
+ * reference-form 6-CTA and 768-thread instances). */
 int tpt_set_option(tpt_context* ctx, const char* key, int value);
 
 /* Replaces DrawTest() (Test.cpp:344-367) for frames [frameCount, frameCount+numFrames) — numFrames*spp samples

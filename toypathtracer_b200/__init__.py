@@ -403,7 +403,8 @@ class Context:
         set_textures. Takes the same inputs as set_textures and refuses the same ones. The emitted radiance of a hit on
         a sphere with a layer is its material's emission x the layer's lookup at the hit's normal, also where a light
         sampling shadow ray meets the light; a sphere with zero emission stays dark. None removes the textures. See
-        include/tpt_b200.h for where the estimator applies it."""
+        include/tpt_b200.h for where the estimator applies it. The option "emission_texture_sampling" (set_option)
+        importance-samples the textured lights by their layers, from tables this call builds."""
         self._set_texture_set("set_emission_textures", textures, sphere_layers)
 
     def _set_texture_set(self, name, textures, sphere_layers):

@@ -38,11 +38,14 @@ struct DeviceSlots
 };
 
 // One set of sphere textures (tpt_set_textures' albedo, tpt_set_emission_textures' emission): its slots, each
-// [layers x h x w float4 texels][spheres int32 layers], and the sizes of the current one.
+// [layers x h x w float4 texels][spheres int32 layers], with the emission set's sampling tables behind them
+// (tpt_env_tables.h), and the sizes of the current one.
 struct TextureSlots
 {
     DeviceSlots slots;
     int w = 0, h = 0, layers = 0, spheres = 0;
+    bool tables = false;       // the current slot has sampling tables (the emission set)
+    bool sampleable = false;   // ... and some layer with a non-zero weight
 };
 
 struct tpt_context
@@ -83,6 +86,7 @@ struct tpt_context
     bool envSampleable = false;                   // the current slot's map has sampling tables (some weight is not zero)
     int envSampling = 0;                          // "environment_sampling"
     TextureSlots tex, emit;
+    int emitSampling = 0;                         // "emission_texture_sampling"
 
     // options
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
@@ -444,6 +448,7 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     if (!strcmp(key, "scene_upload_always")) { ctx->sceneUploadAlways = value ? 1 : 0; return 0; }
     if (!strcmp(key, "mitsuba_compare")) { ctx->sceneFlags = value ? (ctx->sceneFlags | kSceneMitsuba) : (ctx->sceneFlags & ~(uint32_t)kSceneMitsuba); return 0; }
     if (!strcmp(key, "environment_sampling")) { ctx->envSampling = value ? 1 : 0; return 0; }
+    if (!strcmp(key, "emission_texture_sampling")) { ctx->emitSampling = value ? 1 : 0; return 0; }
     if (!strcmp(key, "light_sampling")) { ctx->sceneFlags = value ? (ctx->sceneFlags & ~(uint32_t)kSceneNoLightSampling) : (ctx->sceneFlags | kSceneNoLightSampling); return 0; }
     if (!strcmp(key, "host_progress")) { ctx->hostProgress = value ? 1 : 0; return 0; }
     if (!strcmp(key, "host_zero_copy")) { ctx->hostZeroCopy = value ? 1 : 0; return 0; }
@@ -526,6 +531,7 @@ static int use_textures(tpt_context* ctx, const TextureSlots& ts, cudaStream_t s
     out->H = ts.h;
     // sphere ids past the scene's count are padding spheres, which are never textured
     out->spheres = ts.spheres < scene->count ? ts.spheres : scene->count;
+    out->tabWords = ts.tables ? (uint32_t)emit_table_words(ts.spheres) : 0u;
     return 0;
 }
 
@@ -556,6 +562,9 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
     if (int r = use_textures(ctx, ctx->tex, *stream, "textures", kSceneTextures, scene, &scene->layout.tex)) return r;
     if (int r = use_textures(ctx, ctx->emit, *stream, "emission textures", kSceneEmissionTextures, scene, &scene->layout.emit))
         return r;
+    // "emission_texture_sampling", like "environment_sampling": read per call, not a scene flag
+    if (ctx->emitSampling && ctx->emit.slots.have && ctx->emit.sampleable && !(scene->layout.flags & kSceneNoLightSampling))
+        scene->layout.flags |= kSceneEmitSampling;
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
     scene->pairs.half = scene->halfOk && scene->kformOk && ctx->fastKForm == 2;
@@ -1307,9 +1316,10 @@ int tpt_set_environment(tpt_context* ctx, const float* rgba, int width, int heig
 }
 
 // tpt_set_textures and tpt_set_emission_textures: the checks, the upload into one set's slots and its sizes. `fn` heads
-// the error texts, `what` names the set in those of CUDA failures.
+// the error texts, `what` names the set in those of CUDA failures. `tables`: the slot also carries the layers' sampling
+// tables, built here on the host (the emission set, tpt_env_tables.h).
 static int set_textures(tpt_context* ctx, TextureSlots& ts, const char* fn, const char* what, const float* rgba, int width,
-                        int height, int layers, const int* sphereLayers, int numSpheres, int onDevice)
+                        int height, int layers, const int* sphereLayers, int numSpheres, int onDevice, bool tables)
 {
     // NULL: the calls issued from now on see every sphere without this set; those in flight keep reading their slot
     if (!rgba) { ts.slots.have = false; return 0; }
@@ -1338,12 +1348,15 @@ static int set_textures(tpt_context* ctx, TextureSlots& ts, const char* fn, cons
             for (int c = 0; c < 3; ++c)
                 if (!env_channel_ok(rgba[4 * i + c])) return bad_texel(i, c, rgba[4 * i + c]);
     // The slot that is not current: the calls issued since the set's last upload read the other one. It holds the
-    // texels and the sphere table behind them: 16 W H L + 4 numSpheres bytes.
-    const size_t texBytes = (size_t)n * 16, bytes = texBytes + (size_t)numSpheres * 4;
+    // texels and the sphere table behind them: 16 W H L + 4 numSpheres bytes; with tables, the padding and the tables
+    // behind those (emit_slot_bytes), uploaded from a host copy of the slot in which they are built.
+    const size_t texBytes = (size_t)n * 16;
+    const size_t bytes = tables ? emit_slot_bytes(width, height, layers, numSpheres) : texBytes + (size_t)numSpheres * 4;
     int slot = 0;
     if (int r = slot_begin_upload(ctx, ts.slots, bytes, what, &slot)) return r;
     unsigned char* dst = (unsigned char*)ts.slots.ptr[slot];
     cudaStream_t s = ctx->uploadStream;
+    std::vector<float> host(tables ? bytes / 4 : 0);
     if (onDevice)
     {
         // As tpt_set_environment checks a device map: R, G and B packed into the slot, checked as int32 bits by the
@@ -1367,14 +1380,33 @@ static int set_textures(tpt_context* ctx, TextureSlots& ts, const char* fn, cons
                 memcpy(&v, &bits, 4);
                 return bad_texel(c0 + k / 3, (int)(k % 3), v);
             }
+            // with tables: the checked chunk's RGB back for the build, as tpt_set_environment does
+            if (tables)
+            {
+                CK(cudaMemcpy2DAsync(host.data() + 4 * c0, 16, dst, 12, 12, (size_t)m, cudaMemcpyDeviceToHost, s), "D2H texture RGB");
+                CK(cudaStreamSynchronize(s), "texture RGB sync");
+            }
         }
-        CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyDeviceToDevice, s), "texture upload");
+        if (!tables) CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyDeviceToDevice, s), "texture upload");
     }
+    else if (tables)
+        memcpy(host.data(), rgba, texBytes);
     else
         CK(cudaMemcpyAsync(dst, rgba, texBytes, cudaMemcpyHostToDevice, s), "texture upload");
-    if (numSpheres > 0)
+    bool sampleable = false;
+    if (tables)
+    {
+        if (numSpheres > 0) memcpy(host.data() + 4 * n, sphereLayers, (size_t)numSpheres * 4);
+        EnvAlias* tab = reinterpret_cast<EnvAlias*>(reinterpret_cast<unsigned char*>(host.data()) +
+                                                    emit_table_offset(width, height, layers, numSpheres));
+        sampleable = emit_build_tables(host.data(), width, height, layers, tab);
+        CK(cudaMemcpyAsync(dst, host.data(), bytes, cudaMemcpyHostToDevice, s), "texture upload");
+    }
+    else if (numSpheres > 0)
         CK(cudaMemcpyAsync(dst + texBytes, sphereLayers, (size_t)numSpheres * 4, cudaMemcpyHostToDevice, s), "sphere layer upload");
     if (int r = slot_finish_upload(ctx, ts.slots, slot, what)) return r;
+    ts.tables = tables;
+    ts.sampleable = sampleable;
     ts.w = width;
     ts.h = height;
     ts.layers = layers;
@@ -1387,7 +1419,7 @@ int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height,
 {
     if (!ctx) return (int)cudaErrorInvalidValue;
     return set_textures(ctx, ctx->tex, "tpt_set_textures", "textures", rgba, width, height, layers, sphereLayers, numSpheres,
-                        onDevice);
+                        onDevice, false);
 }
 
 int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
@@ -1395,7 +1427,7 @@ int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, in
 {
     if (!ctx) return (int)cudaErrorInvalidValue;
     return set_textures(ctx, ctx->emit, "tpt_set_emission_textures", "emission textures", rgba, width, height, layers,
-                        sphereLayers, numSpheres, onDevice);
+                        sphereLayers, numSpheres, onDevice, true);
 }
 
 int tpt_read_ray_count(tpt_context* ctx, void* cudaStreamArg, long long* outRays)

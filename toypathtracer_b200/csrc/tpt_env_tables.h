@@ -1,5 +1,6 @@
-// Importance-sampling tables of tpt_set_environment's lat-long map ("environment_sampling"). Host-only, plain C++: the
-// library builds them in tpt_set_environment, and tests/host_sim/env_tables_check.cpp runs the same code under g++.
+// Importance-sampling tables of tpt_set_environment's lat-long map ("environment_sampling") and of
+// tpt_set_emission_textures' layers ("emission_texture_sampling", at the end). Host-only, plain C++: the library builds
+// them in those calls, and tests/host_sim/env_tables_check.cpp and emit_tables_check.cpp run the same code under g++.
 //
 // Weight of cell (i, j), the texel footprint [i, i+1) x [j, j+1) in the (u, v) of include/tpt_b200.h's mapping:
 //   w(i, j) = sin(theta_j) * max over di, dj in {-1, 0, 1} of (R + G + B) / 3 at texel (i + di wrapped, j + dj clamped),
@@ -141,4 +142,41 @@ inline bool env_build_tables(float* texels, int W, int H, EnvAlias* rows, EnvAli
         for (int i = 0; i < W; ++i) texels[4 * ((size_t)j * W + i) + 3] = (float)(pRow[j] * pCol[i]);
     }
     return true;
+}
+
+// ---- emission layers ("emission_texture_sampling") -----------------------------------------------------------------
+// tpt_set_emission_textures builds the same tables for each of its L layers of W x H texels, each layer alone, with
+// env_build_tables: the layers use the map's lat-long mapping, so a layer's sampler is sample_env's with the sphere's
+// normal for the direction. Slot layout (one device allocation per emission-texture slot, emit_slot_bytes):
+//   [L * W * H float4 texels: R, G, B, P] [S int32 sphere layers] [4 bytes of padding when S is odd]
+//   [L blocks of (H + W * H) EnvAlias: layer k's rows, then its columns, row-major]
+// i.e. 16 W H L + 4 S (+ 4) + 8 H L + 8 W H L bytes. The tables start emit_table_words(S) int32 words behind the sphere
+// table (S rounded up to even, keeping them 8-byte aligned); TexSet::tabWords carries that count to the kernels.
+// A layer whose weights are all zero has no tables: every entry of its block is the sentinel {prob 0, alias -1} (the
+// kernels test rows[0].alias < 0) and its texels' alpha is 0. Albedo textures (tpt_set_textures) build no tables and
+// keep their 16 W H L + 4 S byte slots.
+constexpr int32_t kEmitNoTables = -1;
+
+inline size_t emit_table_words(int S) { return ((size_t)S + 1) & ~(size_t)1; }
+inline size_t emit_table_offset(int W, int H, int L, int S) { return (size_t)W * H * L * 16 + emit_table_words(S) * 4; }
+inline size_t emit_slot_bytes(int W, int H, int L, int S)
+{
+    return emit_table_offset(W, H, L, S) + (size_t)L * ((size_t)H + (size_t)W * H) * 8;
+}
+
+// Tables of every layer into `tables` (L blocks of H + W * H entries) and the alpha of `texels` (L * W * H float4, R, G
+// and B read). Returns true when some layer has a non-zero weight.
+inline bool emit_build_tables(float* texels, int W, int H, int L, EnvAlias* tables)
+{
+    bool any = false;
+    const size_t plane = (size_t)W * H, block = (size_t)H + plane;
+    for (int k = 0; k < L; ++k)
+    {
+        float* t = texels + 4 * plane * k;
+        EnvAlias* rows = tables + block * k;
+        if (env_build_tables(t, W, H, rows, rows + H)) { any = true; continue; }
+        for (size_t e = 0; e < block; ++e) { rows[e].prob = 0.0f; rows[e].alias = kEmitNoTables; }
+        for (size_t i = 0; i < plane; ++i) t[4 * i + 3] = 0.0f;
+    }
+    return any;
 }

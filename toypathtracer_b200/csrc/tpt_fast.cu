@@ -862,13 +862,22 @@ __device__ __forceinline__ int next_light(const SceneView& sc, int j, int mid)
 // The shadow ray from o towards light Lr (Test.cpp:104-131, the facing normal nl already resolved): a direction l drawn
 // uniformly in the cone the light subtends, and the returned weight m * omega / pi. The ray adds thrAlb * E_light * weight
 // when it reaches its light.
-__device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l)
+// The cone from o that light Lr subtends: its unit axis sw, and the cosine of its half-angle as the return value (not
+// above 0 where o lies inside or on the light, d <= r).
+__device__ __forceinline__ float light_cone_cos(const LightRec& Lr, V3 o, V3& sw)
 {
     V3 scn = v3(Lr.cx, Lr.cy, Lr.cz);
     V3 pc = scn - o;
     float d2 = dot(pc, pc);
     float inv = __frsqrt_rn(d2);          // d2 is a squared distance between distinct spheres: never denormal
-    V3 sw = pc * inv;
+    sw = pc * inv;
+    return M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
+}
+
+__device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l)
+{
+    V3 sw;
+    const float cosAMax = light_cone_cos(Lr, o, sw);
     // any orthonormal (su, sv) around sw gives the same cone-sample distribution (phi is uniform): use the
     // branch-free basis of Duff et al. 2017 instead of normalize(cross(up, sw)), cross(sw, su) (Test.cpp:108-109)
     const float sgn = copysignf(1.0f, sw.z);
@@ -876,7 +885,6 @@ __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 n
     const float ob = sw.x * sw.y * oa;
     V3 su = v3(1.0f + sgn * sw.x * sw.x * oa, sgn * ob, -sgn * sw.x);
     V3 sv = v3(ob, sgn + sw.y * sw.y * oa, -sw.y);
-    float cosAMax = M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
     float eps1 = RandomFloat01(rng), eps2 = RandomFloat01(rng);
     float cosA = 1.0f - eps1 + eps1 * cosAMax;
     float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
@@ -933,6 +941,7 @@ __device__ __forceinline__ V3 latlong_lookup(const float4* tex, int W, int H, V3
             return v3(__ldg(f), __ldg(f + 1), __ldg(f + 2));
         };
         const V3 a = ld(x0, y0), b = ld(x1, y0), c = ld(x0, y1), e = ld(x1, y1);
+        if constexpr (CELL) *cellP = __ldg(reinterpret_cast<const float*>(tex + (uint32_t)((tv < 0.5f ? y0 : y1) * W + (tu < 0.5f ? x0 : x1))) + 3);
         const V3 top = v3(lerp(a.x, b.x, tu), lerp(a.y, b.y, tu), lerp(a.z, b.z, tu));
         const V3 bot = v3(lerp(c.x, e.x, tu), lerp(c.y, e.y, tu), lerp(c.z, e.z, tu));
         return v3(lerp(top.x, bot.x, tv), lerp(top.y, bot.y, tv), lerp(top.z, bot.z, tv));
@@ -963,12 +972,19 @@ __device__ __forceinline__ int sphere_layer(const TexSet& ts, int id)
     return __ldg(reinterpret_cast<const int*>(((uint64_t)ts.tabHi << 32) | ts.tabLo) + id);
 }
 
-// base x the lookup of layer `layer` (>= 0) of ts at the shading normal n ((pos - centre) / r): the texture's product
-// comes first, so a constant layer c gives base x c rounded once. Draws no random numbers.
-__device__ __forceinline__ V3 sphere_texture_layer(const TexSet& ts, int layer, V3 base, V3 n)
+// The W x H texels of layer `layer` of ts.
+__device__ __forceinline__ const float4* texture_layer(const TexSet& ts, int layer)
 {
-    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)ts.texHi << 32) | ts.texLo);
-    return base * latlong_lookup<false, true>(tex + (uint32_t)(layer * ts.W * ts.H), ts.W, ts.H, n);
+    return reinterpret_cast<const float4*>(((uint64_t)ts.texHi << 32) | ts.texLo) + (uint32_t)(layer * ts.W * ts.H);
+}
+
+// base x the lookup of layer `layer` (>= 0) of ts at the shading normal n ((pos - centre) / r): the texture's product
+// comes first, so a constant layer c gives base x c rounded once. Draws no random numbers. CELL: also the alpha of the
+// cell that holds n's (u, v) into *cellP (latlong_lookup).
+template <bool CELL = false>
+__device__ __forceinline__ V3 sphere_texture_layer(const TexSet& ts, int layer, V3 base, V3 n, float* cellP = nullptr)
+{
+    return base * latlong_lookup<CELL, true>(texture_layer(ts, layer), ts.W, ts.H, n, cellP);
 }
 
 // The textured value of a hit on sphere `id` with shading normal n: base (the material's albedo or emission) x the
@@ -1001,15 +1017,14 @@ __device__ __forceinline__ float env_bounce_weight(float pb, float pe)
     return e2 > 0.0f ? b2 / (b2 + e2) : 1.0f;
 }
 
-// One environment sample at a Lambert vertex whose bounce is cosine-distributed about nl: six draws (row, row alias test,
-// column, column alias test, in-cell u and v offsets), the direction into l, and true when its shadow ray is traced
-// (c = l.nl > 0 and sin theta > 0), with pend = (c / pi) pdf_e / (pdf_e^2 + pdf_b^2), pdf_b = c / pi: the ray adds
-// thrAlb * L(l) * pend when it leaves the scene. The tables are read through the read-only path.
-__device__ __forceinline__ bool sample_env(const SceneView& sc, V3 nl, uint32_t& rng, V3& l, float& pend)
+// One draw from the tables of a W x H lat-long image (the environment map or an emission layer): tex, its texels with
+// each cell's probability P in their alpha; rows, its H row entries followed by its W * H column entries
+// (tpt_env_tables.h). Six draws (row, row alias test, column, column alias test, in-cell u and v offsets); returns the
+// unit direction of the drawn (u, v) by the inverse of latlong_lookup's mapping, with P and s = sin theta. The tables
+// are read through the read-only path.
+__device__ __forceinline__ V3 latlong_sample(const float4* tex, const float2* rows, uint32_t W, uint32_t H, uint32_t& rng,
+                                             float& P, float& s)
 {
-    const uint32_t W = (uint32_t)sc.envW, H = (uint32_t)sc.envH;
-    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
-    const float2* rows = reinterpret_cast<const float2*>(tex + (size_t)W * H);
     const float2* cols = rows + H;
     uint32_t j = __umulhi((XorShift32(rng) & 0xFFFFFFu) << 8, H);          // (k * H) >> 24
     const float2 er = __ldg(rows + j);
@@ -1018,14 +1033,25 @@ __device__ __forceinline__ bool sample_env(const SceneView& sc, V3 nl, uint32_t&
     uint32_t i = __umulhi((XorShift32(rng) & 0xFFFFFFu) << 8, W);
     const float2 ec = __ldg(crow + i);
     if (!(RandomFloat01(rng) < ec.x)) i = (uint32_t)__float_as_int(ec.y);
-    const float P = __ldg(&tex[(size_t)j * W + i].w);
+    P = __ldg(&tex[(size_t)j * W + i].w);
     const float u = (float)i + RandomFloat01(rng);
     const float v = (float)j + RandomFloat01(rng);
+    float sp, cp, c;
+    __sincosf(__fdividef(u, (float)W) * (2.0f * TPT_PI) - TPT_PI, &sp, &cp);
+    __sincosf(__fdividef(v, (float)H) * TPT_PI, &s, &c);
+    return v3(s * sp, c, -s * cp);
+}
+
+// One environment sample at a Lambert vertex whose bounce is cosine-distributed about nl: latlong_sample's direction
+// into l, and true when its shadow ray is traced (c = l.nl > 0 and sin theta > 0), with pend = (c / pi) pdf_e /
+// (pdf_e^2 + pdf_b^2), pdf_b = c / pi: the ray adds thrAlb * L(l) * pend when it leaves the scene.
+__device__ __forceinline__ bool sample_env(const SceneView& sc, V3 nl, uint32_t& rng, V3& l, float& pend)
+{
+    const uint32_t W = (uint32_t)sc.envW, H = (uint32_t)sc.envH;
+    const float4* tex = reinterpret_cast<const float4*>(((uint64_t)sc.envHi << 32) | sc.envLo);
+    float P, s;
+    l = latlong_sample(tex, reinterpret_cast<const float2*>(tex + (size_t)W * H), W, H, rng, P, s);
     const float fW = (float)W, fH = (float)H;
-    float sp, cp, s, c;
-    __sincosf(__fdividef(u, fW) * (2.0f * TPT_PI) - TPT_PI, &sp, &cp);
-    __sincosf(__fdividef(v, fH) * TPT_PI, &s, &c);
-    l = v3(s * sp, c, -s * cp);
     const float cn = dot(l, nl);
     if (!(cn > 0.0f && s > 0.0f)) return false;
     const float pe = P * (fW * fH * kEnvPdfScale) / s;
@@ -1048,15 +1074,88 @@ __device__ __forceinline__ V3 fast_sky_mis(const SceneView& sc, const QPath& st)
     return L * env_bounce_weight(st.pend, pe);
 }
 
+// ---- emission texture sampling ("emission_texture_sampling", kSceneEmitSampling; tpt_env_tables.h pins the tables)
+// At a light-sampled Lambert vertex o, a light with a sampleable emission layer gets, after its cone sample, one texture
+// sample: latlong_sample's draw from its layer's tables gives the unit normal n and the point x = c + r n, of solid-angle
+// density at o
+//   pt(x) = P W H / (2 pi^2 sin theta) / r^2 * |x - o|^2 / cos_x,   cos_x = n . normalize(o - x),
+// against the cone's pc = 1 / omega. Both rays are weighted with the power heuristic, written with q = pt omega = pt / pc
+// (so that omega 0, P 0 and an overflowing pt stay finite): the cone's w_c = pc^2 / (pc^2 + pt^2) = 1 / (1 + q^2), the
+// texture sample's pend_t = (m / pi) pt / (pt^2 + pc^2) = (m / pi) omega / (q + 1 / q).
+constexpr int kKindEmit = -2;                // QPath::kind of light j's texture-sample shadow ray: kKindEmit - j
+
+// The sampling tables of emission layer `layer` (>= 0): its rows, then its columns; null when the layer has none (all
+// of its weights are zero: the sentinel alias kEmitNoTables in its first row).
+__device__ __forceinline__ const float2* emit_tables(const TexSet& ts, int layer)
+{
+    const float2* t = reinterpret_cast<const float2*>(reinterpret_cast<const int*>(((uint64_t)ts.tabHi << 32) | ts.tabLo) +
+                                                      ts.tabWords) + (size_t)layer * ((size_t)ts.H + (size_t)ts.W * ts.H);
+    return __float_as_int(__ldg(t).y) < 0 ? nullptr : t;
+}
+
+// q = pt(x) omega for a point x on light Lr with unit normal n, sin theta s and cell probability P, seen from o at
+// squared distance d2 with cos_x = cx.
+__device__ __forceinline__ float emit_q(const TexSet& ts, const LightRec& Lr, float P, float s, float d2, float cx, float omega)
+{
+    return __fdividef(P * ((float)ts.W * (float)ts.H * kEnvPdfScale) * d2 * omega, s * (Lr.radius * Lr.radius) * cx);
+}
+
+// The cone weight w_c of a cone ray from o that met light Lr (emission layer `layer`) at x with normal n, where the
+// lookup read cell probability P: 1 for a light without tables and for o inside or on the light (no texture sample).
+__device__ __forceinline__ float emit_cone_weight(const SceneView& sc, const LightRec& Lr, int layer, V3 o, V3 x, V3 n, float P)
+{
+    V3 sw;
+    const float cosAMax = light_cone_cos(Lr, o, sw);
+    if (!(cosAMax > 0.0f) || !emit_tables(sc.emit, layer)) return 1.0f;
+    const V3 ox = o - x;
+    const float d2 = dot(ox, ox);
+    const float s = M<false>::sqrt_(fmaxf(fmaf(-n.y, n.y, 1.0f), 0.0f));
+    const float q = emit_q(sc.emit, Lr, P, s, d2, dot(n, ox) * __frsqrt_rn(d2), 2.0f * TPT_PI * (1.0f - cosAMax));
+    return q > 0.0f ? __fdividef(1.0f, fmaf(q, q, 1.0f)) : 1.0f;
+}
+
+// The texture sample of light Lr at the vertex st.o (facing normal st.nl), after its cone sample: nothing, and no draws,
+// for a light without a sampleable layer or a vertex inside or on it; otherwise the six draws, and true when its shadow
+// ray is traced (x faces o, m = l . nl > 0 and sin theta > 0), with the direction in st.d and pend_t in st.pend.
+__device__ __forceinline__ bool sample_emit(const SceneView& sc, const LightRec& Lr, QPath& st)
+{
+    const int layer = sphere_layer(sc.emit, Lr.id);
+    if (layer < 0) return false;
+    const float2* tabs = emit_tables(sc.emit, layer);
+    V3 sw;
+    const float cosAMax = light_cone_cos(Lr, st.o, sw);
+    if (!tabs || !(cosAMax > 0.0f)) return false;
+    float P, s;
+    const V3 n = latlong_sample(texture_layer(sc.emit, layer), tabs, (uint32_t)sc.emit.W, (uint32_t)sc.emit.H, st.rng, P, s);
+    const V3 ox = st.o - (v3(Lr.cx, Lr.cy, Lr.cz) + n * Lr.radius);
+    const float d2 = dot(ox, ox), inv = __frsqrt_rn(d2);
+    const float cx = dot(n, ox) * inv;
+    st.d = neg(ox) * inv;
+    const float m = dot(st.d, st.nl);
+    if (!(cx > 0.0f && m > 0.0f && s > 0.0f)) return false;
+    const float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
+    const float q = emit_q(sc.emit, Lr, P, s, d2, cx, omega);
+    st.pend = m * (1.0f / TPT_PI) * __fdividef(omega, q + __fdividef(1.0f, q));
+    return true;
+}
+
 // The rest of a Lambert vertex after its shadow ray towards light lightFrom - 1 (or, lightFrom = 0, after the vertex's
 // own shading): the next light the vertex samples, its cone and shadow ray, or, when none is left, the bounce along
 // st.nextDir with throughput st.thrAlb. Without light sampling (kLsOff) there are no lights to sample: the bounce.
 // ENVM 2 with kSceneEnvSampling: after the lights (lightFrom <= nLights), one environment sample at a vertex hit from
 // outside (st.doMaterialE, path_step) and its shadow ray, which comes back with lightFrom = nLights + 1; then the
 // bounce, which keeps its pdf_b in pend for its miss (fast_sky_mis), or -1 where the vertex took no sample.
-template <int LS, int ENVM = 1>
-__device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom)
+// TEX with kSceneEmitSampling: after the cone ray of light coneOf (>= 0), that light's texture sample (sample_emit) and its
+// shadow ray, which comes back with lightFrom = coneOf + 1 and coneOf -1.
+template <int LS, int ENVM = 1, bool TEX = false>
+__device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom, int coneOf = -1)
 {
+    if constexpr (TEX)
+        if (coneOf >= 0 && (sc.flags & kSceneEmitSampling) && sample_emit(sc, sc.lights[coneOf], st))
+        {
+            st.kind = kKindEmit - coneOf;
+            return;
+        }
     const int j = LS == kLsOff ? sc.nLights : next_light(sc, lightFrom, st.mid);
     if (j < sc.nLights)
     {
@@ -1107,6 +1206,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
     // ---- shade
     bool wantLight = false;
     int lightFrom = 0;
+    int coneOf = -1;          // TEX: the light whose cone ray just returned
     bool finished = false;
     if (st.active)
     {
@@ -1194,25 +1294,41 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         }
         else
         {
-            const int j = st.kind - 1;
+            // a light's shadow ray: its cone's (kind 1 + j) or, with TEX, its texture sample's (kind kKindEmit - j)
+            const bool texRay = TEX && st.kind < kKindEnv;
+            const int j = texRay ? kKindEmit - st.kind : st.kind - 1;
             const LightRec& Lj = sc.lights[j];
             if (id == Lj.id)
             {
                 V3 e = v3(Lj.ex, Lj.ey, Lj.ez);
-                // an emission-textured light: its layer's lookup at the normal of the point where the shadow ray meets it
+                float pend = st.pend;
+                // an emission-textured light: its layer's lookup at the normal of the point where the shadow ray meets it,
+                // and with kSceneEmitSampling a cone ray's power-heuristic weight against the light's texture sample
                 if constexpr (TEX)
                     if (sc.flags & kSceneEmissionTextures)
                     {
                         const int layer = sphere_layer(sc.emit, id);
                         if (layer >= 0)
-                            e = sphere_texture_layer(sc.emit, layer, e, (st.o + st.d * t - v3(Lj.cx, Lj.cy, Lj.cz)) * sc.invRadius[id]);
+                        {
+                            const V3 x = st.o + st.d * t;
+                            const V3 n = (x - v3(Lj.cx, Lj.cy, Lj.cz)) * sc.invRadius[id];
+                            if (!texRay && (sc.flags & kSceneEmitSampling))
+                            {
+                                float P;
+                                e = sphere_texture_layer<true>(sc.emit, layer, e, n, &P);
+                                pend *= emit_cone_weight(sc, Lj, layer, st.o, x, n, P);
+                            }
+                            else
+                                e = sphere_texture_layer(sc.emit, layer, e, n);
+                        }
                     }
-                st.col = st.col + (st.thrAlb * e) * st.pend;
+                st.col = st.col + (st.thrAlb * e) * pend;
             }
             wantLight = true; lightFrom = j + 1;
+            if (!texRay) coneOf = j;
         }
     }
-    if (NEXT && LS != kLsOff && wantLight) lambert_next<LS, ENVM>(sc, st, lightFrom);
+    if (NEXT && LS != kLsOff && wantLight) lambert_next<LS, ENVM, TEX>(sc, st, lightFrom, coneOf);
     return finished;
 }
 
@@ -1220,14 +1336,14 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
 // Lambert vertex at p whose facing normal is n, as if a camera ray had just hit it: the bounce direction drawn first, then
 // lambert_next picks the first light (or the bounce). No emission of its own (doMaterialE is not looked at before the
 // next hit); depth 0, so the path keeps a camera path's budget. `mid`: the sphere the point lies on, or -1.
-template <int LS, int ENVM = 1>
+template <int LS, int ENVM = 1, bool TEX = false>
 __device__ __forceinline__ void begin_vertex(const SceneView& sc, QPath& st, int mid)
 {
     st.nl = st.d;
     st.nextDir = M<false>::normalize(st.d + RandomUnitVector<false>(st.rng));
     st.thrAlb = v3(1, 1, 1);
     st.mid = mid;
-    lambert_next<LS, ENVM>(sc, st, 0);     // (begin_path left doMaterialE true: the point takes an environment sample)
+    lambert_next<LS, ENVM, TEX>(sc, st, 0);     // (begin_path left doMaterialE true: the point takes an environment sample)
 }
 
 // The sphere id of point entry `tag` (tpt_trace_irradiance, tpt_trace_samples): ids are per input, so an entry of a list
@@ -1491,7 +1607,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
             if constexpr (SRC == kSrcRays && kStartInDeal)
                 if (pointStart)
                 {
-                    begin_vertex<LS, ENVM>(sc, st, point_id(pointIds, entries, tag));
+                    begin_vertex<LS, ENVM, TEX>(sc, st, point_id(pointIds, entries, tag));
                     st.weight *= TPT_PI;
                 }
             if constexpr (SRC == kSrcRays && !kStartInDeal) fresh = true;
@@ -1499,7 +1615,7 @@ fast_queue_body(DrawParams p, const unsigned char* __restrict__ blob, SceneBlobL
         if constexpr (SRC == kSrcRays && !kStartInDeal)
             if (pointStart && fresh)
             {
-                begin_vertex<LS, ENVM>(sc, st, point_id(pointIds, entries, st.pixOff));
+                begin_vertex<LS, ENVM, TEX>(sc, st, point_id(pointIds, entries, st.pixOff));
                 st.weight *= TPT_PI;
                 fresh = false;
             }

@@ -34,14 +34,15 @@ struct alignas(16) LightRec
 // of its W x H RGBA texels, layer-major (row 0 = the +y pole, global memory) and of the int32 layer of each sphere id below
 // `spheres` (-1: none; begin_call keeps `spheres` at most the scene's count, so padding spheres are never textured). The
 // addresses travel as 32-bit halves, which keeps the struct 4-byte aligned (an 8-byte aligned kernel parameter changes
-// how the compiler loads the fields around it). `pad` is unused: it keeps the struct a multiple of 8 bytes, so the kernel
+// how the compiler loads the fields around it). `tabWords` also keeps the struct a multiple of 8 bytes, so the kernel
 // parameters behind SceneBlobLayout keep the 8-byte pairing of their constant-bank loads (an odd number of added words
-// changed untextured kernels' SASS).
+// changed untextured kernels' SASS): for the emission set, the int32 words from the sphere table to the layers' sampling
+// tables (tpt_env_tables.h, emit_table_words of the uploaded table's length); 0 for the albedo set, which has none.
 struct TexSet
 {
     uint32_t texLo, texHi, tabLo, tabHi;
     int W, H, spheres;
-    uint32_t pad;
+    uint32_t tabWords;
 };
 
 // Device-side scene, SoA, padded like the reference's SpheresSoA (Maths.h:368-404):
@@ -102,8 +103,11 @@ struct SceneBlobLayout
 // multiply the albedo of a hit on a textured sphere by its layer's lat-long lookup at the hit's normal (sphere_texture).
 // kSceneEmissionTextures (tpt_set_emission_textures, set by begin_call): the same instances multiply the emission of a hit
 // on a sphere with an emission layer, and that of a light where its shadow ray meets it, by the layer's lookup there.
+// kSceneEmitSampling ("emission_texture_sampling" active for the call, set by begin_call with kSceneEmissionTextures): the
+// same instances take one texture sample per light with a sampleable emission layer at light-sampled Lambert vertices
+// (sample_emit), and weight that light's cone rays against it.
 enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
-                             kSceneTextures = 16u, kSceneEmissionTextures = 32u };
+                             kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u };
 // Either texture set: the calls that have one run the instances that look textures up (pick_queue, fast_auto_variant).
 constexpr uint32_t kSceneAnyTextures = kSceneTextures | kSceneEmissionTextures;
 
