@@ -155,6 +155,45 @@ int tpt_set_textures(tpt_context* ctx, const float* rgba, int width, int height,
  * TPT_MODE_REFGPU_FAST is refused. */
 int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, int height, int layers,
                               const int* sphereLayers, int numSpheres, int onDevice);
+/* Homogeneous participating media inside glass spheres for the fast mode: tinted or milky glass, smoke, jade.
+ *   media5    numSpheres records of 5 floats in HOST memory, {sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g}: record i is
+ *             the medium inside sphere i. sigma_a is the absorption coefficient per colour channel and sigma_s the grey
+ *             scattering coefficient, both per world unit; g is the Henyey-Greenstein asymmetry (g > 0 scatters forward).
+ *             A record whose sigma_a and sigma_s are all zero is "no medium". Sphere ids at or past numSpheres or the
+ *             scene's count, and the padding spheres of the sweep, have none. NULL or numSpheres 0 removes all media.
+ * A medium acts only inside a sphere whose material is glass; on any other sphere it is kept but has no effect (a later
+ * tpt_set_scene may make that sphere glass). Estimator: a path ray whose segment of length t ended on the inside face
+ * (dot(d, normal) > 0) of a glass sphere with a medium, before the depth cap is tested and before any emission is added,
+ *   1. with sigma_s > 0 draws u and takes t_s = -ln(1 - u) / sigma_s (finite: u <= 1 - 2^-24); with sigma_s = 0 draws
+ *      nothing (t_s = +inf);
+ *   2. t_s < t: scatters at o + d t_s. Past the depth cap the path ends and adds nothing (a medium emits nothing);
+ *      otherwise the throughput takes exp(-sigma_a t_s) per channel, the direction becomes a Henyey-Greenstein sample
+ *      around d from two more draws xi1 (cos theta) and xi2 (phi = 2 pi xi2), the depth grows by one, and the next hit
+ *      adds its emission. The hit itself is not shaded. The continuation is an ordinary path ray, traced and counted.
+ *      cos theta = (1 + g^2 - s^2) / (2 g), s = (1 - g^2) / (1 - g + 2 g xi1), clamped to [-1, 1], when |g| >= 1e-3;
+ *      1 - 2 xi1 otherwise;
+ *   3. t_s >= t: the throughput takes exp(-sigma_a t) and the hit is shaded as without media.
+ * Absorption is applied continuously and scattering sampled exactly, so the estimator is unbiased with RGB sigma_a and
+ * no ratio weights. A path none of whose segments ends on the inside face of a glass sphere with sigma_s > 0 draws the
+ * same random numbers as without media; a medium with sigma_s = 0 draws none. No light sampling at medium vertices.
+ * Limits: the medium of a segment is that of the sphere whose inside face it ends on (a segment inside a glass sphere
+ * that ends on the outside of a sphere nested in it runs in vacuum); scatter events count against the depth cap, so
+ * dense media lose energy to it.
+ * Refused, with tpt_last_error text naming the sphere and the field ("tpt_set_media: sphere 3 has sigma_s = -1"):
+ * numSpheres < 0, a non-finite sigma or one with its sign bit set (-0 included), a g that is NaN or has |g| >= 1. A
+ * refused call leaves the media as they were.
+ * Lifetime and ordering: the media belong to the context; tpt_set_scene keeps them and applies them to the new scene's
+ * ids, and before any scene they are stored for the first one. The call re-packs the current scene with a media section
+ * and uploads it as tpt_set_scene does (tpt_last_scene_upload_bytes reports that upload): it never blocks on the GPU,
+ * calls issued before it keep the media they were issued with, even while in flight, and calls issued after it see the
+ * new ones. A scene none of whose spheres has a medium keeps the bytes of its blob and every call its default kernel.
+ * Only TPT_MODE_FAST uses media. While the current scene has one, every fast call (tpt_draw, tpt_trace_rays,
+ * tpt_trace_irradiance, tpt_draw_samples, tpt_trace_samples) runs the slab queue's reference-form instances that carry
+ * the textures: tpt_draw's auto variant is 3, 9 runs the 6-CTA instance, an explicit "fast_variant" 0, 1, 2, 4, 5, 6, 7
+ * or 8 is refused, and tpt_draw in TPT_MODE_EXACT, TPT_MODE_REFGPU and TPT_MODE_REFGPU_FAST is refused. Media combine
+ * with textures, "environment_sampling" and "emission_texture_sampling". tpt_draw_aovs and tpt_trace_aovs, which record
+ * first hits, do not change. */
+int tpt_set_media(tpt_context* ctx, const float* media5, int numSpheres);
 /* Camera only (UpdateTest rebuilds it every frame from the aspect ratio, Test.cpp:341). */
 int tpt_set_camera(tpt_context* ctx, const void* camera88);
 

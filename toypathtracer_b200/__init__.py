@@ -89,6 +89,7 @@ def _load_lib():
     L.tpt_set_environment.argtypes = [vp, vp, ci, ci, ci]; L.tpt_set_environment.restype = ci
     L.tpt_set_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_textures.restype = ci
     L.tpt_set_emission_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_emission_textures.restype = ci
+    L.tpt_set_media.argtypes = [vp, vp, ci]; L.tpt_set_media.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -454,6 +455,36 @@ class Context:
         self._check(getattr(self._L, cname)(self._h, ctypes.c_void_p(addr), shape[2], shape[1], shape[0],
                                             layers.ctypes.data if layers.size else None, int(layers.size),
                                             1 if on_dev else 0), cname)
+
+    def set_media(self, media):
+        """tpt_set_media: homogeneous media inside glass spheres for the fast mode. `media` is an (N, 5) float32 numpy
+        array or CPU torch tensor, row i {sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g} the medium inside sphere i (all
+        sigmas zero: none; spheres past N have none), or None to remove all media. A medium acts only inside glass.
+        Refused here, as by the library: other shapes and dtypes, a non-finite sigma or one with its sign bit set (-0
+        included), a g that is NaN or has |g| >= 1. See include/tpt_b200.h for the estimator and which calls use it."""
+        if media is None:
+            self._check(self._L.tpt_set_media(self._h, None, 0), "tpt_set_media")
+            return
+        if hasattr(media, "data_ptr"):
+            if media.is_cuda:
+                raise TptError("set_media: media must be in host memory (a numpy array or a CPU tensor)")
+            media = media.numpy()
+        if not isinstance(media, np.ndarray):
+            raise TptError("set_media: media must be a numpy array or a CPU torch tensor")
+        if media.ndim != 2 or media.shape[1] != 5:
+            raise TptError(f"set_media: media must have shape (N, 5), not {tuple(media.shape)}")
+        if media.dtype != np.float32:
+            raise TptError(f"set_media: media must be float32, not {media.dtype}")
+        fields = ("sigma_a.r", "sigma_a.g", "sigma_a.b", "sigma_s", "g")
+        for i, row in enumerate(media):
+            for f in range(4):
+                if not np.isfinite(row[f]) or np.signbit(row[f]):
+                    raise TptError(f"set_media: sphere {i} has {fields[f]} = {float(row[f]):g}")
+            if not abs(float(row[4])) < 1.0:
+                raise TptError(f"set_media: sphere {i} has g = {float(row[4]):g}")
+        media = np.ascontiguousarray(media)
+        self._check(self._L.tpt_set_media(self._h, media.ctypes.data if media.size else None, int(media.shape[0])),
+                    "tpt_set_media")
 
     def set_camera(self, camera: np.ndarray):
         camera = np.ascontiguousarray(camera)

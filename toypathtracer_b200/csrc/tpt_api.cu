@@ -87,6 +87,14 @@ struct tpt_context
     int envSampling = 0;                          // "environment_sampling"
     TextureSlots tex, emit;
     int emitSampling = 0;                         // "emission_texture_sampling"
+    // tpt_set_media's records (5 floats per sphere id), which also belong to the context: every pack of a scene puts them
+    // in its blob, so tpt_set_media re-packs the current scene from its inputs, kept here with the flags it was packed with.
+    std::vector<float> media;
+    std::vector<Sphere20> sceneSpheres;
+    std::vector<Material36> sceneMats;
+    std::vector<int> sceneEmissives;
+    bool sceneEmissivesGiven = false;
+    uint32_t scenePackFlags = 0;
 
     // options
     int fastVariant = -1;     // -1 = auto (fast_auto_variant)
@@ -337,30 +345,25 @@ void tpt_destroy(tpt_context* ctx)
 
 const char* tpt_last_error(tpt_context* ctx) { return ctx ? ctx->lastError.c_str() : "null context"; }
 
-int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials36, int count,
-                  const void* camera88, const int* emissives, int emissiveCount)
+} // extern "C"
+
+// The scene upload of tpt_set_scene and tpt_set_media: packs a scene (its inputs as tpt_set_scene takes them, the flags
+// it is packed with and mediaSpheres media records) and makes the blob the scene the calls issued from now on read.
+// Identical bytes are not uploaded again; otherwise the blob goes into the slot the calls in flight are not reading, on
+// the upload stream, and the host never blocks on the GPU. On failure the context's scene is the one it was.
+static int upload_scene(tpt_context* ctx, const char* fn, const Sphere20* spheres, const Material36* mats, int count,
+                        const int* emissives, int emissiveCount, uint32_t packFlags, const float* media5, int mediaSpheres)
 {
-    if (!ctx) return (int)cudaErrorInvalidValue;
-    if (!spheres20 || !materials36 || !camera88 || count <= 0) return fail_msg(ctx, "tpt_set_scene: bad arguments");
-    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
-    // the caller's emissive list indexes spheres/materials (Test.cpp:96-100): refuse what would read out of bounds
-    if (emissives)
-    {
-        if (emissiveCount < 0 || emissiveCount > count) return fail_msg(ctx, "tpt_set_scene: emissiveCount out of range");
-        for (int i = 0; i < emissiveCount; ++i)
-            if (emissives[i] < 0 || emissives[i] >= count) return fail_msg(ctx, "tpt_set_scene: emissive id out of range");
-    }
     std::vector<unsigned char> blob;
     SceneBlobLayout L;
     int nLights = 0;
-    pack_scene_blob((const Sphere20*)spheres20, (const Material36*)materials36, count, emissives, emissiveCount, blob, L, nLights,
-                    ctx->sceneFlags);
+    pack_scene_blob(spheres, mats, count, emissives, emissiveCount, blob, L, nLights, packFlags, media5, mediaSpheres);
     ParamPairs pairs;
     build_param_pairs(blob, L, count, pairs);
     const bool halfOk = build_half_pairs(blob, L, count, pairs);
     // geometry + light table must fit in shared memory next to the kernels' static shared arrays
     const uint32_t kMaxStage = 200 * 1024;
-    if (L.geomBytes > kMaxStage) return fail_msg(ctx, "tpt_set_scene: too many spheres for shared-memory staging");
+    if (L.geomBytes > kMaxStage) return fail_msgf(ctx, "%s: too many spheres for shared-memory staging", fn);
     // A reference shell calls UpdateTest + upload every frame although the scene only changes under kFlagAnimate
     // (Test.cpp:304-308): identical bytes are not uploaded again.
     const bool same = ctx->haveScene && ctx->scene.count == count && ctx->scene.layout.flags == L.flags && blob == ctx->lastBlob;
@@ -412,12 +415,68 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
     ctx->scene.kformOk = true;
     for (int i = 0; i < count; ++i)
     {
-        const Sphere20& s = ((const Sphere20*)spheres20)[i];
+        const Sphere20& s = spheres[i];
         const double c2 = (double)s.center[0] * s.center[0] + (double)s.center[1] * s.center[1] + (double)s.center[2] * s.center[2];
         if (c2 > 128.0 + 2.0 * (double)s.radius * s.radius) ctx->scene.kformOk = false;
     }
-    memcpy(&ctx->cam, camera88, sizeof(Camera88));
     ctx->haveScene = true;
+    return 0;
+}
+
+extern "C" {
+
+int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials36, int count,
+                  const void* camera88, const int* emissives, int emissiveCount)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (!spheres20 || !materials36 || !camera88 || count <= 0) return fail_msg(ctx, "tpt_set_scene: bad arguments");
+    CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+    // the caller's emissive list indexes spheres/materials (Test.cpp:96-100): refuse what would read out of bounds
+    if (emissives)
+    {
+        if (emissiveCount < 0 || emissiveCount > count) return fail_msg(ctx, "tpt_set_scene: emissiveCount out of range");
+        for (int i = 0; i < emissiveCount; ++i)
+            if (emissives[i] < 0 || emissives[i] >= count) return fail_msg(ctx, "tpt_set_scene: emissive id out of range");
+    }
+    if (int r = upload_scene(ctx, "tpt_set_scene", (const Sphere20*)spheres20, (const Material36*)materials36, count, emissives,
+                             emissiveCount, ctx->sceneFlags, ctx->media.empty() ? nullptr : ctx->media.data(),
+                             (int)(ctx->media.size() / 5)))
+        return r;
+    // the inputs tpt_set_media re-packs
+    ctx->sceneSpheres.assign((const Sphere20*)spheres20, (const Sphere20*)spheres20 + count);
+    ctx->sceneMats.assign((const Material36*)materials36, (const Material36*)materials36 + count);
+    ctx->sceneEmissivesGiven = emissives != nullptr;
+    if (emissives) ctx->sceneEmissives.assign(emissives, emissives + emissiveCount);
+    else ctx->sceneEmissives.clear();
+    ctx->scenePackFlags = ctx->sceneFlags;
+    memcpy(&ctx->cam, camera88, sizeof(Camera88));
+    return 0;
+}
+
+int tpt_set_media(tpt_context* ctx, const float* media5, int numSpheres)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    if (numSpheres < 0) return fail_msgf(ctx, "tpt_set_media: numSpheres = %d is negative", numSpheres);
+    if (!media5) numSpheres = 0;
+    static const char* const kField[5] = {"sigma_a.r", "sigma_a.g", "sigma_a.b", "sigma_s", "g"};
+    for (int i = 0; i < numSpheres; ++i)
+    {
+        const float* m = media5 + 5 * (size_t)i;
+        for (int f = 0; f < 4; ++f)
+            if (!env_channel_ok(m[f])) return fail_msgf(ctx, "tpt_set_media: sphere %d has %s = %g", i, kField[f], (double)m[f]);
+        if (!(fabsf(m[4]) < 1.0f)) return fail_msgf(ctx, "tpt_set_media: sphere %d has g = %g", i, (double)m[4]);
+    }
+    std::vector<float> media(media5, media5 + 5 * (size_t)numSpheres);
+    if (ctx->haveScene)
+    {
+        CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+        if (int r = upload_scene(ctx, "tpt_set_media", ctx->sceneSpheres.data(), ctx->sceneMats.data(),
+                                 (int)ctx->sceneSpheres.size(), ctx->sceneEmissivesGiven ? ctx->sceneEmissives.data() : nullptr,
+                                 (int)ctx->sceneEmissives.size(), ctx->scenePackFlags, media.empty() ? nullptr : media.data(),
+                                 numSpheres))
+            return r;
+    }
+    ctx->media.swap(media);
     return 0;
 }
 
@@ -942,13 +1001,17 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
                               "%s(ctx, NULL, 0, 0, 0, NULL, 0, 0) for exact and reference-GPU draws)",
                          albedo ? "textures" : "emission textures", albedo ? "tpt_set_textures" : "tpt_set_emission_textures");
     }
+    if (mode != TPT_MODE_FAST && (ctx->scene.layout.flags & kSceneMedia))
+        return fail_msg(ctx, "tpt_draw: the scene has media, and only TPT_MODE_FAST draws use them (clear them with "
+                             "tpt_set_media(ctx, NULL, 0) for exact and reference-GPU draws)");
     // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
     if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment and look up textures
+    // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment, look up textures and
+    // trace media
     const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
     const bool textured = (scene.layout.flags & kSceneAnyTextures) != 0;
     if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
@@ -962,6 +1025,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
                          albedo ? "textures" : "emission textures", albedo ? "tpt_set_textures" : "tpt_set_emission_textures",
                          ctx->fastVariant);
     }
+    if ((scene.layout.flags & kSceneMedia) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
+        return fail_msgf(ctx, "tpt_draw: the scene has media (tpt_set_media), and fast_variant %d does not trace them: use -1 "
+                              "(auto), 3 or 9", ctx->fastVariant);
 
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);
@@ -972,7 +1038,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     // being traced — no staging image, no device-to-host copy after the kernel.
     bool zeroCopy = false;
     cudaPointerAttributes attr{};
-    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && !envSampling && !textured &&
+    if (!bufferOnDevice && mode == TPT_MODE_FAST && ctx->hostZeroCopy && !(scene.layout.flags & kSceneRefForm) &&
         (ctx->fastVariant < 0 || fast_variant_info(ctx->fastVariant).writesFinalPixels))
     {
         zeroCopy = prevWeight == 0.0f && numFrames <= kMaxFramesPerDraw && cudaPointerGetAttributes(&attr, backbuffer) == cudaSuccess &&

@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "tpt_types.h"
+#include "tpt_scene_pack.h"
 
 namespace tpt {
 
@@ -101,6 +102,7 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     v.matA = (const Q4*)pick(L.offMatA);
     v.matB = (const Q4*)pick(L.offMatB);
     v.matRi = (const float*)pick(L.offMatRi);
+    v.media = (const Q4*)pick(media_offset(L.offMatRi, count));
     v.count = count;
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = nLights;

@@ -874,17 +874,25 @@ __device__ __forceinline__ float light_cone_cos(const LightRec& Lr, V3 o, V3& sw
     return M<false>::sqrt_(1.0f - Lr.radius * Lr.radius * inv * inv);
 }
 
+// The branch-free orthonormal basis (su, sv) around the unit vector w of Duff et al. 2017 (sample_light_cone's cone,
+// hg_sample's scattering cone).
+__device__ __forceinline__ void duff_basis(V3 w, V3& su, V3& sv)
+{
+    const float sgn = copysignf(1.0f, w.z);
+    const float oa = __fdividef(-1.0f, sgn + w.z);       // |sgn + w.z| in [1, 2]: MUFU.RCP + FMUL instead of the IEEE sequence
+    const float ob = w.x * w.y * oa;
+    su = v3(1.0f + sgn * w.x * w.x * oa, sgn * ob, -sgn * w.x);
+    sv = v3(ob, sgn + w.y * w.y * oa, -w.y);
+}
+
 __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l)
 {
     V3 sw;
     const float cosAMax = light_cone_cos(Lr, o, sw);
     // any orthonormal (su, sv) around sw gives the same cone-sample distribution (phi is uniform): use the
     // branch-free basis of Duff et al. 2017 instead of normalize(cross(up, sw)), cross(sw, su) (Test.cpp:108-109)
-    const float sgn = copysignf(1.0f, sw.z);
-    const float oa = __fdividef(-1.0f, sgn + sw.z);      // |sgn + sw.z| in [1, 2]: MUFU.RCP + FMUL instead of the IEEE sequence
-    const float ob = sw.x * sw.y * oa;
-    V3 su = v3(1.0f + sgn * sw.x * sw.x * oa, sgn * ob, -sgn * sw.x);
-    V3 sv = v3(ob, sgn + sw.y * sw.y * oa, -sw.y);
+    V3 su, sv;
+    duff_basis(sw, su, sv);
     float eps1 = RandomFloat01(rng), eps2 = RandomFloat01(rng);
     float cosA = 1.0f - eps1 + eps1 * cosAMax;
     float sinA = M<false>::sqrt_(1.0f - cosA * cosA);
@@ -896,6 +904,61 @@ __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 n
     float dl = dot(l, nl);
     float m = (0.0f < dl) ? dl : 0.0f;
     return m * omega * (1.0f / TPT_PI);
+}
+
+// ---- homogeneous media inside glass spheres (tpt_set_media, kSceneMedia; DESIGN §3.14)
+// A Henyey-Greenstein direction around the unit direction d with asymmetry g (g > 0 forward) from the draws xi1 (cos theta)
+// and xi2 (phi).
+__device__ __forceinline__ V3 hg_sample(V3 d, float g, float xi1, float xi2)
+{
+    float cosT = 1.0f - 2.0f * xi1;
+    if (fabsf(g) >= 1e-3f)
+    {
+        const float s = __fdividef(1.0f - g * g, 1.0f - g + 2.0f * g * xi1);
+        cosT = fminf(fmaxf(__fdividef(1.0f + g * g - s * s, 2.0f * g), -1.0f), 1.0f);
+    }
+    const float sinT = M<false>::sqrt_(fmaxf(1.0f - cosT * cosT, 0.0f));
+    float sp, cp;
+    __sincosf(2.0f * TPT_PI * xi2, &sp, &cp);
+    V3 su, sv;
+    duff_basis(d, su, sv);
+    return su * (sinT * cp) + sv * (sinT * sp) + d * cosT;
+}
+
+// exp(-sigma t) per channel, at most 1 (the factor only ever lowers the throughput).
+__device__ __forceinline__ V3 transmittance(const Q4& m, float t)
+{
+    return v3(fminf(__expf(-m.x * t), 1.0f), fminf(__expf(-m.y * t), 1.0f), fminf(__expf(-m.z * t), 1.0f));
+}
+
+// The medium of sphere `mid` on a path segment of length t that ended on the inside face of that glass sphere: with
+// sigma_s > 0 one free-flight distance t_s = -ln(1 - u) / sigma_s is drawn. Returns true when the path scattered before t
+// (the hit is not shaded): past the depth cap it ends with nothing added (*finished), otherwise the throughput takes
+// exp(-sigma_a t_s) and the path goes on from the scatter point along an HG direction (two more draws) as a path ray
+// whose next hit adds its emission. Otherwise the throughput takes exp(-sigma_a t) and the caller shades the hit.
+// Media entry [count] and the entries of spheres without a medium are zero: no draw, and a factor of exactly 1.
+__device__ __forceinline__ bool medium_step(const SceneView& sc, QPath& st, int mid, float t, bool& finished)
+{
+    const Q4 m = sc.media[mid];
+    if (m.w > 0.0f)
+    {
+        const float ts = __fdividef(-__logf(1.0f - RandomFloat01(st.rng)), m.w);
+        if (ts < t)
+        {
+            if (st.depth >= TPT_MAX_DEPTH) { finished = true; return true; }
+            const float g = reinterpret_cast<const float*>(sc.media + sc.count + 1)[mid];
+            st.thr = st.thr * transmittance(m, ts);
+            st.o = st.o + st.d * ts;
+            const float xi1 = RandomFloat01(st.rng);
+            const float xi2 = RandomFloat01(st.rng);
+            st.d = hg_sample(st.d, g, xi1, xi2);
+            st.doMaterialE = true;
+            ++st.depth;
+            return true;
+        }
+    }
+    st.thr = st.thr * transmittance(m, t);
+    return false;
 }
 
 // Metal bounce direction (Test.cpp:137-150); the path goes on when dot(result, normal) > 0. With roughness == 0 the
@@ -1194,7 +1257,8 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // TEX: where the call's kSceneTextures is set, Lambert and Metal hits take the textured albedo for the material's albedo,
 // and where its kSceneEmissionTextures is set, every hit takes the textured emission for the material's emission and a
 // light's shadow ray that reaches it the light's emission x its layer's lookup at the normal where the ray meets it (the
-// slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while either is set).
+// slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while either is set), and
+// where its kSceneMedia is set, a path ray that ends on the inside face of a glass sphere runs medium_step first.
 template <int LS, int ENVM = 1, bool NEXT = true, bool TEX = false, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
@@ -1236,7 +1300,14 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     // every emission this hit adds below is mat.emissive: with emission textures, the textured one
                     if (sc.flags & kSceneEmissionTextures) mat.emissive = sphere_texture(sc.emit, id, mat.emissive, normal);
                 }
-                if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
+                // a path segment that ran inside a glass sphere with a medium: absorption along it, or a scatter event
+                // inside it instead of this hit (medium_step)
+                bool scattered = false;
+                if constexpr (TEX)
+                    if ((sc.flags & kSceneMedia) && mtype == kDielectric && dot(st.d, normal) > 0.0f)
+                        scattered = medium_step(sc, st, mid, t, finished);
+                if (scattered) {}
+                else if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
                 else if (LS == kLsOff && mtype == kLambert)
                 {
                     // Test.cpp:86-92 without the light loop; the emission is always added (Test.cpp:209-215 compiled out)
@@ -2339,8 +2410,8 @@ static QueuePick pick_queue(const SceneDev& sc, int variant, long long regionPix
 {
     QueuePick q;
     q.kform = fast_queue_kform(sc);
-    // the environment-sampling and texture instances sweep in the reference form (env_mode, tex_mode)
-    const bool refInstances = (sc.layout.flags & (kSceneEnvSampling | kSceneAnyTextures)) != 0;
+    // the environment-sampling, texture and media instances sweep in the reference form (env_mode, tex_mode)
+    const bool refInstances = (sc.layout.flags & kSceneRefForm) != 0;
     if (refInstances) q.kform = 0;
     // the pair array of a scene of at most 64 padded spheres goes in the kernel parameter (form 4), except for variant 4,
     // with "fast_kform" 3 and for tpt_draw_samples' pixel lists (not measured with form 4; they keep form 2). The same
@@ -2657,16 +2728,16 @@ static bool wave_fits(const SceneDev& sc, long long regionPix, long long S)
     return wave_paths(regionPix, S) <= 0x7fffffffLL && sc.nLights < kKindFree;
 }
 
-// The slab queue (3), always while the environment is sampled or textures are set (tpt_draw then never stores into
-// mapped host memory),
+// The slab queue (3), always while the environment is sampled, textures are set or the scene has a medium (tpt_draw then
+// never stores into mapped host memory),
 // except: a draw into mapped host memory runs the group queue (8), which stores its finished pixels
 // itself; and where the sweep dwarfs everything else (>= 1024 spheres) and the slab queue cannot run a packed-pair sweep
 // (pair array does not fit, or "fast_kform" < 2), the block wavefront that sorts its paths by material before Scatter()
 // is faster (4096 spheres, Mray/s: queue packed 443, wavefront 333, queue scalar 312).
 int fast_auto_variant(const SceneDev& sc, long long regionPix, int spp, int numFrames, bool zeroCopy)
 {
-    if (sc.layout.flags & (kSceneEnvSampling | kSceneAnyTextures)) return 3;   // the slab queue alone samples the environment
-                                                                             // and looks up textures
+    if (sc.layout.flags & kSceneRefForm) return 3;   // the slab queue alone samples the environment, looks up textures and
+                                                    // has media
     if (zeroCopy) return 8;
     const long long S = (long long)spp * (numFrames < kMaxFramesPerDraw ? numFrames : kMaxFramesPerDraw);   // first launch
     return sc.count >= 1024 && fast_queue_kform(sc) < 2 && wave_fits(sc, regionPix, S) ? 7 : 3;

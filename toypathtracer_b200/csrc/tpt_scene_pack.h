@@ -10,7 +10,19 @@
 
 namespace tpt {
 
-inline uint32_t align16(uint32_t x) { return (x + 15u) & ~15u; }
+#ifdef __CUDACC__
+#define TPT_PACK_HD __host__ __device__
+#else
+#define TPT_PACK_HD
+#endif
+
+TPT_PACK_HD inline uint32_t align16(uint32_t x) { return (x + 15u) & ~15u; }
+
+// The media section (tpt_set_media, kSceneMedia) of a blob of `count` spheres follows matRi: (count + 1) Q4
+// {sigma_a.rgb, sigma_s}, then (count + 1) floats g, each part padded to 16 B; entry [count] is zero. Its offset, for the
+// pack and for the kernels' views.
+TPT_PACK_HD inline uint32_t media_offset(uint32_t offMatRi, int count) { return offMatRi + align16((uint32_t)(count + 1) * 4u); }
+inline uint32_t media_bytes(int count) { return align16((uint32_t)(count + 1) * 16u) + align16((uint32_t)(count + 1) * 4u); }
 
 inline SceneBlobLayout scene_blob_layout(int count, int nLights)
 {
@@ -32,11 +44,20 @@ inline SceneBlobLayout scene_blob_layout(int count, int nLights)
     return L;
 }
 
+// A medium record of tpt_set_media {sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g}: "no medium" when both sigmas are zero.
+inline bool has_medium(const float* m5) { return m5[0] != 0.0f || m5[1] != 0.0f || m5[2] != 0.0f || m5[3] != 0.0f; }
+
 // emissives == nullptr: derive the list like UpdateTest (Test.cpp:333-338).
+// media5: mediaSpheres records of tpt_set_media (null: none). The blob gets the media section, and kSceneMedia, only when a
+// sphere below `count` has a medium; otherwise its bytes are those of the scene without media.
 inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int count,
                             const int* emissives, int emissiveCount,
-                            std::vector<unsigned char>& blob, SceneBlobLayout& L, int& nLights, uint32_t sceneFlags = 0)
+                            std::vector<unsigned char>& blob, SceneBlobLayout& L, int& nLights, uint32_t sceneFlags = 0,
+                            const float* media5 = nullptr, int mediaSpheres = 0)
 {
+    const int nMedia = media5 ? (mediaSpheres < count ? mediaSpheres : count) : 0;
+    bool anyMedium = false;
+    for (int i = 0; i < nMedia; ++i) anyMedium = anyMedium || has_medium(media5 + 5 * i);
     std::vector<int> em;
     if (emissives) em.assign(emissives, emissives + emissiveCount);
     else
@@ -44,7 +65,12 @@ inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int
             if (mats[i].emissive[0] > 0 || mats[i].emissive[1] > 0 || mats[i].emissive[2] > 0) em.push_back(i);
     nLights = (int)em.size();
     L = scene_blob_layout(count, nLights);
-    L.flags = sceneFlags;
+    L.flags = sceneFlags & ~(uint32_t)kSceneMedia;
+    if (anyMedium)
+    {
+        L.flags |= kSceneMedia;
+        L.totalBytes += media_bytes(count);    // geomBytes stays: the section is material data
+    }
     int simdCount = (count + 3) / 4 * 4;
     blob.assign(L.totalBytes, 0);
     Q4* sph = (Q4*)(blob.data() + L.offSph);
@@ -77,6 +103,17 @@ inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int
         matRi[i] = m.ri;
     }
     // entry [count]: all-zero (Lambert, black) — what the reference's out-of-bounds material read amounts to
+    if (anyMedium)
+    {
+        Q4* media = (Q4*)(blob.data() + media_offset(L.offMatRi, count));
+        float* g = (float*)(media + count + 1);
+        for (int i = 0; i < nMedia; ++i)
+        {
+            const float* m = media5 + 5 * i;
+            media[i].x = m[0]; media[i].y = m[1]; media[i].z = m[2]; media[i].w = m[3];
+            g[i] = m[4];
+        }
+    }
     for (int j = 0; j < nLights; ++j)
     {
         int i = em[j];
@@ -171,6 +208,7 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.matA = (const Q4*)(base + L.offMatA);
     v.matB = (const Q4*)(base + L.offMatB);
     v.matRi = (const float*)(base + L.offMatRi);
+    v.media = (const Q4*)(base + media_offset(L.offMatRi, count));
     v.count = count;
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = sampled_lights(L.flags, nLights);

@@ -58,6 +58,7 @@ struct SceneView
     const Q4* matA;
     const Q4* matB;
     const float* matRi;
+    const Q4* media;      // kSceneMedia: {sigma_a.rgb, sigma_s}[count + 1], then g[count + 1] (media_offset, tpt_scene_pack.h)
     const LightRec* lights;
     int count, simdCount, nLights;
     uint32_t flags;       // kScene* bits
@@ -106,10 +107,16 @@ struct SceneBlobLayout
 // kSceneEmitSampling ("emission_texture_sampling" active for the call, set by begin_call with kSceneEmissionTextures): the
 // same instances take one texture sample per light with a sampleable emission layer at light-sampled Lambert vertices
 // (sample_emit), and weight that light's cone rays against it.
+// kSceneMedia (tpt_set_media, set by the pack when some sphere of the scene has a medium): the blob carries the media
+// section behind matRi, and the same instances absorb and scatter along path segments that end on the inside face of a
+// glass sphere with a medium (medium_step).
 enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
-                             kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u };
+                             kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u, kSceneMedia = 128u };
 // Either texture set: the calls that have one run the instances that look textures up (pick_queue, fast_auto_variant).
 constexpr uint32_t kSceneAnyTextures = kSceneTextures | kSceneEmissionTextures;
+// What only the slab queue's reference-form instances (sweep form 0, path_step's ENVM 2 and TEX) compute: a call with any of
+// these runs them (pick_queue, fast_auto_variant, tpt_draw's variant checks).
+constexpr uint32_t kSceneRefForm = kSceneEnvSampling | kSceneAnyTextures | kSceneMedia;
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.
