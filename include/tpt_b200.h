@@ -178,7 +178,8 @@ int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, in
  * same random numbers as without media; a medium with sigma_s = 0 draws none. No light sampling at medium vertices.
  * Limits: the medium of a segment is that of the sphere whose inside face it ends on (a segment inside a glass sphere
  * that ends on the outside of a sphere nested in it runs in vacuum); scatter events count against the depth cap, so
- * dense media lose energy to it.
+ * dense media lose energy to it at the default cap of 10: the option "max_depth" (tpt_set_option) raises it, with Russian
+ * roulette past depth 10.
  * Refused, with tpt_last_error text naming the sphere and the field ("tpt_set_media: sphere 3 has sigma_s = -1"):
  * numSpheres < 0, a non-finite sigma or one with its sign bit set (-0 included), a g that is NaN or has |g| >= 1. A
  * refused call leaves the media as they were.
@@ -278,7 +279,24 @@ int tpt_set_spp(tpt_context* ctx, int spp);
  * option is on, as tpt_set_environment builds the map's: the same weights (sin theta x the 3 x 3 maximum of mean RGB), alias
  * tables and realised probabilities; they cost 8 * width * height * layers + 8 * height * layers bytes per device copy,
  * plus 4 bytes of padding behind an odd sphere table. Kernels and routing are emission textures': the slab queue's
- * reference-form 6-CTA and 768-thread instances). */
+ * reference-form 6-CTA and 768-thread instances),
+ * "max_depth" (1..256, default 10, the reference's compile-time cap; out of range it is refused with "max_depth: 1..256"
+ * and keeps its value: the fast estimator's path depth cap. Read by each call when it is issued, like
+ * "environment_sampling", not a scene flag: setting it uploads nothing, and calls already issued keep the value they were
+ * issued with. Depth counts Lambert bounces, Metal and glass continuations and medium scatter events. A path ray's hit at
+ * depth >= max_depth adds its emission and ends the path, and a medium scatter event there ends it with nothing added.
+ * Russian roulette, only when max_depth > 10: at every path ray's hit at depth >= 10, before the medium's draw, the cap
+ * test and any emission, the path draws u from its own stream; with q = min(1, max(thr.r, thr.g, thr.b)) of its
+ * throughput, u >= q ends it with nothing added, and otherwise the throughput becomes thr / q and the hit is shaded as
+ * without the roll. Shadow rays and misses take no roll. So a path that ends before depth 10 draws the same numbers as
+ * with the default, max_depth <= 10 draws nothing extra, and the roll is unbiased: a call with max_depth n converges to
+ * the image with cap n. max_depth 10 is the default call exactly (kernels, streams, ray counts and bits). Applies to
+ * tpt_draw in TPT_MODE_FAST, tpt_trace_rays, tpt_trace_irradiance (a point keeps a camera path's budget, from depth 0),
+ * tpt_draw_samples and tpt_trace_samples; tpt_draw_aovs and tpt_trace_aovs, which record first hits, do not change.
+ * While it is not 10 every such call runs the slab queue's reference-form 6-CTA and 768-thread instances: tpt_draw's auto
+ * variant is 3, 9 runs the 6-CTA instance, an explicit "fast_variant" 0, 1, 2, 4, 5, 6, 7 or 8 is refused, and tpt_draw
+ * in TPT_MODE_EXACT, TPT_MODE_REFGPU and TPT_MODE_REFGPU_FAST is refused (those keep the reference's 10 for parity; set
+ * it back to 10 for them). It combines with media, textures, "environment_sampling" and "emission_texture_sampling"). */
 int tpt_set_option(tpt_context* ctx, const char* key, int value);
 
 /* Replaces DrawTest() (Test.cpp:344-367) for frames [frameCount, frameCount+numFrames) — numFrames*spp samples

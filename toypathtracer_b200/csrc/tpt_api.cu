@@ -87,6 +87,7 @@ struct tpt_context
     int envSampling = 0;                          // "environment_sampling"
     TextureSlots tex, emit;
     int emitSampling = 0;                         // "emission_texture_sampling"
+    int maxDepth = kRefMaxDepth;                  // "max_depth"
     // tpt_set_media's records (5 floats per sphere id), which also belong to the context: every pack of a scene puts them
     // in its blob, so tpt_set_media re-packs the current scene from its inputs, kept here with the flags it was packed with.
     std::vector<float> media;
@@ -508,6 +509,7 @@ int tpt_set_option(tpt_context* ctx, const char* key, int value)
     if (!strcmp(key, "mitsuba_compare")) { ctx->sceneFlags = value ? (ctx->sceneFlags | kSceneMitsuba) : (ctx->sceneFlags & ~(uint32_t)kSceneMitsuba); return 0; }
     if (!strcmp(key, "environment_sampling")) { ctx->envSampling = value ? 1 : 0; return 0; }
     if (!strcmp(key, "emission_texture_sampling")) { ctx->emitSampling = value ? 1 : 0; return 0; }
+    if (!strcmp(key, "max_depth")) { if (value < 1 || value > kMaxPathDepth) return fail_msg(ctx, "max_depth: 1..256"); ctx->maxDepth = value; return 0; }
     if (!strcmp(key, "light_sampling")) { ctx->sceneFlags = value ? (ctx->sceneFlags & ~(uint32_t)kSceneNoLightSampling) : (ctx->sceneFlags | kSceneNoLightSampling); return 0; }
     if (!strcmp(key, "host_progress")) { ctx->hostProgress = value ? 1 : 0; return 0; }
     if (!strcmp(key, "host_zero_copy")) { ctx->hostZeroCopy = value ? 1 : 0; return 0; }
@@ -624,6 +626,8 @@ static int begin_call(tpt_context* ctx, void* cudaStreamArg, cudaStream_t* strea
     // "emission_texture_sampling", like "environment_sampling": read per call, not a scene flag
     if (ctx->emitSampling && ctx->emit.slots.have && ctx->emit.sampleable && !(scene->layout.flags & kSceneNoLightSampling))
         scene->layout.flags |= kSceneEmitSampling;
+    // "max_depth", read per call as well: only this call's copy of the layout carries it, never the blob or ctx->scene
+    scene->layout.flags |= depth_flags(ctx->maxDepth);
     scene->kformOk = scene->kformOk && ctx->fastKForm != 0;
     scene->kformMode = ctx->fastKForm;
     scene->pairs.half = scene->halfOk && scene->kformOk && ctx->fastKForm == 2;
@@ -1004,14 +1008,17 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode != TPT_MODE_FAST && (ctx->scene.layout.flags & kSceneMedia))
         return fail_msg(ctx, "tpt_draw: the scene has media, and only TPT_MODE_FAST draws use them (clear them with "
                              "tpt_set_media(ctx, NULL, 0) for exact and reference-GPU draws)");
+    if (mode != TPT_MODE_FAST && ctx->maxDepth != kRefMaxDepth)
+        return fail_msgf(ctx, "tpt_draw: \"max_depth\" is %d, and only TPT_MODE_FAST draws use it (set it back to 10 for "
+                              "exact and reference-GPU draws)", ctx->maxDepth);
     // an empty shard (more ranks than rows, TraceRowJob(start, start)): nothing to trace, nothing to copy
     if (numRows == 0) return empty_call(ctx, outRayCount, outRaysPerFrame, numFrames);
     if (row0 + (long long)(numRows - 1) * rowStep >= height) return fail_msg(ctx, "tpt_draw: rows outside the image");
     cudaStream_t stream;
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
-    // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment, look up textures and
-    // trace media
+    // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment, look up textures,
+    // trace media and take the call's depth cap
     const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
     const bool textured = (scene.layout.flags & kSceneAnyTextures) != 0;
     if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
@@ -1028,6 +1035,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if ((scene.layout.flags & kSceneMedia) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
         return fail_msgf(ctx, "tpt_draw: the scene has media (tpt_set_media), and fast_variant %d does not trace them: use -1 "
                               "(auto), 3 or 9", ctx->fastVariant);
+    if ((scene.layout.flags & kSceneDepth) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
+        return fail_msgf(ctx, "tpt_draw: \"max_depth\" is %d, and fast_variant %d keeps the depth cap at 10: use -1 (auto), 3 "
+                              "or 9", ctx->maxDepth, ctx->fastVariant);
 
     const RowRegion rows = {width, row0, numRows, rowStep, packed};
     const size_t bufBytes = (packed ? (size_t)numRows : (size_t)height) * width * 4 * sizeof(float);

@@ -107,6 +107,7 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = nLights;
     v.flags = L.flags;
+    v.maxDepth = scene_max_depth(L.flags);
     v.sphShared = smem_u32(smemBase + L.offSph);   // geometry is always inside the staged prefix
     v.envLo = L.envLo;
     v.envHi = L.envHi;

@@ -933,9 +933,9 @@ __device__ __forceinline__ V3 transmittance(const Q4& m, float t)
 
 // The medium of sphere `mid` on a path segment of length t that ended on the inside face of that glass sphere: with
 // sigma_s > 0 one free-flight distance t_s = -ln(1 - u) / sigma_s is drawn. Returns true when the path scattered before t
-// (the hit is not shaded): past the depth cap it ends with nothing added (*finished), otherwise the throughput takes
-// exp(-sigma_a t_s) and the path goes on from the scatter point along an HG direction (two more draws) as a path ray
-// whose next hit adds its emission. Otherwise the throughput takes exp(-sigma_a t) and the caller shades the hit.
+// (the hit is not shaded): past the call's depth cap (sc.maxDepth) it ends with nothing added (*finished), otherwise the
+// throughput takes exp(-sigma_a t_s) and the path goes on from the scatter point along an HG direction (two more draws)
+// as a path ray whose next hit adds its emission. Otherwise the throughput takes exp(-sigma_a t) and the caller shades the hit.
 // Media entry [count] and the entries of spheres without a medium are zero: no draw, and a factor of exactly 1.
 __device__ __forceinline__ bool medium_step(const SceneView& sc, QPath& st, int mid, float t, bool& finished)
 {
@@ -945,7 +945,7 @@ __device__ __forceinline__ bool medium_step(const SceneView& sc, QPath& st, int 
         const float ts = __fdividef(-__logf(1.0f - RandomFloat01(st.rng)), m.w);
         if (ts < t)
         {
-            if (st.depth >= TPT_MAX_DEPTH) { finished = true; return true; }
+            if (st.depth >= sc.maxDepth) { finished = true; return true; }
             const float g = reinterpret_cast<const float*>(sc.media + sc.count + 1)[mid];
             st.thr = st.thr * transmittance(m, ts);
             st.o = st.o + st.d * ts;
@@ -958,6 +958,19 @@ __device__ __forceinline__ bool medium_step(const SceneView& sc, QPath& st, int 
         }
     }
     st.thr = st.thr * transmittance(m, t);
+    return false;
+}
+
+// ---- "max_depth" past the reference's cap (kSceneDepth; DESIGN §3.15)
+// Russian roulette at a path ray's hit once the path is at depth TPT_MAX_DEPTH or deeper, in calls whose cap is larger:
+// one draw u, and with q = min(1, max channel of the throughput) the path ends with nothing added when u >= q (returns
+// true); otherwise its throughput is divided by q, which keeps the estimator of the capped path unbiased.
+__device__ __forceinline__ bool roulette(QPath& st)
+{
+    const float u = RandomFloat01(st.rng);
+    const float q = fminf(fmaxf(fmaxf(st.thr.x, st.thr.y), st.thr.z), 1.0f);
+    if (!(u < q)) return true;
+    if (q < 1.0f) st.thr = st.thr * __fdividef(1.0f, q);   // q >= u >= 0 and q > 0 here
     return false;
 }
 
@@ -1258,7 +1271,8 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // and where its kSceneEmissionTextures is set, every hit takes the textured emission for the material's emission and a
 // light's shadow ray that reaches it the light's emission x its layer's lookup at the normal where the ray meets it (the
 // slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while either is set), and
-// where its kSceneMedia is set, a path ray that ends on the inside face of a glass sphere runs medium_step first.
+// where its kSceneMedia is set, a path ray that ends on the inside face of a glass sphere runs medium_step first. TEX also
+// takes the call's depth cap (sc.maxDepth, "max_depth") for the reference's, with roulette past it where it is larger.
 template <int LS, int ENVM = 1, bool NEXT = true, bool TEX = false, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
@@ -1300,14 +1314,20 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                     // every emission this hit adds below is mat.emissive: with emission textures, the textured one
                     if (sc.flags & kSceneEmissionTextures) mat.emissive = sphere_texture(sc.emit, id, mat.emissive, normal);
                 }
-                // a path segment that ran inside a glass sphere with a medium: absorption along it, or a scatter event
-                // inside it instead of this hit (medium_step)
-                bool scattered = false;
+                // the hit is not shaded when, past the reference's depth in a call whose "max_depth" is larger, Russian
+                // roulette ends the path first (roulette), or when the path segment ran inside a glass sphere with a
+                // medium and scattered inside it (medium_step; otherwise the medium absorbs along it)
+                bool unshaded = false;
                 if constexpr (TEX)
-                    if ((sc.flags & kSceneMedia) && mtype == kDielectric && dot(st.d, normal) > 0.0f)
-                        scattered = medium_step(sc, st, mid, t, finished);
-                if (scattered) {}
-                else if (st.depth >= TPT_MAX_DEPTH) { st.col = st.col + st.thr * mat.emissive; finished = true; }
+                {
+                    if (sc.maxDepth > TPT_MAX_DEPTH && st.depth >= TPT_MAX_DEPTH && roulette(st)) unshaded = finished = true;
+                    else if ((sc.flags & kSceneMedia) && mtype == kDielectric && dot(st.d, normal) > 0.0f)
+                        unshaded = medium_step(sc, st, mid, t, finished);
+                }
+                // the depth cap: the reference's in every instance but TEX's, which take the call's
+                const int maxDepth = TEX ? sc.maxDepth : TPT_MAX_DEPTH;
+                if (unshaded) {}
+                else if (st.depth >= maxDepth) { st.col = st.col + st.thr * mat.emissive; finished = true; }
                 else if (LS == kLsOff && mtype == kLambert)
                 {
                     // Test.cpp:86-92 without the light loop; the emission is always added (Test.cpp:209-215 compiled out)

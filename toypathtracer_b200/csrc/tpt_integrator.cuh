@@ -27,6 +27,7 @@ namespace tpt {
 #define TPT_MIN_T 0.001f
 #define TPT_MAX_T 1.0e7f
 #define TPT_MAX_DEPTH 10
+static_assert(TPT_MAX_DEPTH == kRefMaxDepth, "\"max_depth\" defaults to the reference's cap");
 
 // ---- float3 (Maths.h:23-115 SSE semantics, scalar form proven bit-identical in SURVEY §9.2) ----------------
 struct V3 { float x, y, z; };

@@ -213,6 +213,7 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = sampled_lights(L.flags, nLights);
     v.flags = L.flags;
+    v.maxDepth = scene_max_depth(L.flags);
     v.sphShared = 0;
     v.envLo = v.envHi = 0;     // host views never look up an environment
     v.envW = v.envH = 0;

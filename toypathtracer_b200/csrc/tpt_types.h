@@ -62,6 +62,7 @@ struct SceneView
     const LightRec* lights;
     int count, simdCount, nLights;
     uint32_t flags;       // kScene* bits
+    int maxDepth;         // the call's "max_depth" (scene_max_depth of flags): read only where TEX (path_step)
     uint32_t sphShared;   // device: 32-bit shared-memory address of sph[] (always staged), for ld.shared.v4
     uint32_t envLo, envHi; // kSceneEnvironment: address of the envW x envH RGBA texels of the lat-long environment (row 0 =
     int envW, envH;        // zenith, global memory) in two halves, as SceneBlobLayout carries it; its sampling tables follow
@@ -110,13 +111,38 @@ struct SceneBlobLayout
 // kSceneMedia (tpt_set_media, set by the pack when some sphere of the scene has a medium): the blob carries the media
 // section behind matRi, and the same instances absorb and scatter along path segments that end on the inside face of a
 // glass sphere with a medium (medium_step).
+// kSceneDepth ("max_depth" other than the reference's 10 for the call, set by begin_call): the value travels in bits
+// kSceneDepthShift.. of the call's flags (depth_flags, scene_max_depth), and the same instances end paths at that depth
+// instead, with Russian roulette past depth 10 when it is larger (path_step).
 enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
-                             kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u, kSceneMedia = 128u };
+                             kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u, kSceneMedia = 128u,
+                             kSceneDepth = 256u };
 // Either texture set: the calls that have one run the instances that look textures up (pick_queue, fast_auto_variant).
 constexpr uint32_t kSceneAnyTextures = kSceneTextures | kSceneEmissionTextures;
 // What only the slab queue's reference-form instances (sweep form 0, path_step's ENVM 2 and TEX) compute: a call with any of
 // these runs them (pick_queue, fast_auto_variant, tpt_draw's variant checks).
-constexpr uint32_t kSceneRefForm = kSceneEnvSampling | kSceneAnyTextures | kSceneMedia;
+constexpr uint32_t kSceneRefForm = kSceneEnvSampling | kSceneAnyTextures | kSceneMedia | kSceneDepth;
+
+// "max_depth": the reference's compile-time cap (TPT_MAX_DEPTH, tpt_integrator.cuh) is the default and the depth from
+// which Russian roulette runs; the option takes 1..kMaxPathDepth. A per-call value, never part of the scene's blob or the
+// layout the upload compares: it exists only in the copy of the layout a call passes to its kernels.
+constexpr int kRefMaxDepth = 10;
+constexpr int kMaxPathDepth = 256;
+constexpr int kSceneDepthShift = 16;
+constexpr uint32_t kSceneDepthMask = 0x1ffu;   // 9 bits: 1..256
+// The flag bits of a call with max_depth n: none for the default.
+inline constexpr uint32_t depth_flags(int n)
+{
+    return n == kRefMaxDepth ? 0u : kSceneDepth | ((uint32_t)n & kSceneDepthMask) << kSceneDepthShift;
+}
+// The max_depth of a call's flags.
+#ifdef __CUDACC__
+__host__ __device__
+#endif
+inline constexpr int scene_max_depth(uint32_t flags)
+{
+    return (flags & kSceneDepth) ? (int)(flags >> kSceneDepthShift & kSceneDepthMask) : kRefMaxDepth;
+}
 
 // Number of lights the integrators sample: the scene's emissive list with light sampling on, none with it off. The blob
 // keeps the light table either way, so toggling the switch uploads the same bytes.
