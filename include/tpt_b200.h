@@ -195,6 +195,50 @@ int tpt_set_emission_textures(tpt_context* ctx, const float* rgba, int width, in
  * with textures, "environment_sampling" and "emission_texture_sampling". tpt_draw_aovs and tpt_trace_aovs, which record
  * first hits, do not change. */
 int tpt_set_media(tpt_context* ctx, const float* media5, int numSpheres);
+/* Homogeneous fog in the air between the spheres for the fast mode, lit by the lights: beams, glows around lamps, haze.
+ *   fog9      9 floats in HOST memory, {c.x, c.y, c.z, R, sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g}: the fog fills the
+ *             ball B = {c, R} minus the scene's spheres. sigma_a is the absorption coefficient per colour channel and
+ *             sigma_s the grey scattering coefficient, both per world unit; g is the Henyey-Greenstein asymmetry. NULL, or
+ *             a record whose sigmas are all zero, removes the fog.
+ * Which segments are in air: a ray segment [o, o + t d] runs in air when it ends on the outside face of a sphere
+ * (dot(d, normal) <= 0) or leaves the scene (t = TPT_MAX_T); this holds for path rays and every kind of shadow ray. A
+ * segment that ends on an inside face runs in that sphere (tpt_set_media's rule). The fog length of a segment in air is
+ * L = |[0, t] ∩ [t_in, t_out]|, the part of it inside B.
+ * Estimator: a path ray's segment in air, after the "max_depth" roulette on a hit and before the depth cap is tested and
+ * any emission or sky is added (a miss takes no roll),
+ *   1. with L > 0 and sigma_s > 0 draws u and takes t_s = -ln(1 - u) / sigma_s, measured along the fog part of the
+ *      segment; with sigma_s = 0 it draws nothing and the throughput takes exp(-sigma_a L);
+ *   2. t_s < L: the path scatters at o + d (max(t_in, 0) + t_s) and the throughput takes exp(-sigma_a t_s). Past the
+ *      depth cap the path ends and adds nothing; otherwise the depth grows by one, once per event. With light sampling
+ *      off two draws xi1, xi2 give the direction hg_sample(d, g, xi1, xi2) (tpt_set_media's HG sample) and the next hit
+ *      adds its emission. With it on, the vertex works like a Lambert vertex with the phase function
+ *      p(cos) = (1 - g^2) / (4 pi (1 + g^2 - 2 g cos)^(3/2)) (exactly 1 / (4 pi) for |g| < 1e-3) for cos / pi: first the
+ *      HG direction is drawn (xi1, xi2) and kept; then every light in order (none is excluded) takes one cone sample
+ *      (2 draws) and its shadow ray, which, when it reaches light j, adds thr E_j omega p(dot(d, l)) T_shadow; then the
+ *      path bounces along the kept direction, and emission after the bounce follows the rule after a Lambert vertex.
+ *      Fog vertices take no "environment_sampling" sample (their bounce's miss keeps full weight) and no
+ *      "emission_texture_sampling" sample (their cone rays keep full weight and still take the emission texture's
+ *      lookup where they meet the light);
+ *   3. t_s >= L: the throughput takes exp(-sigma_a L) and the hit or miss is handled as without fog.
+ * The rays that leave a fog scatter point (its cone rays and its continuation) take hits from distance 0 rather than
+ * TPT_MIN_T: the point lies in air but may lie within TPT_MIN_T of a surface, which they must not skip.
+ * Every shadow ray in air (Lambert and fog-vertex cones, environment samples that miss, emission-texture samples) takes
+ * T_shadow = exp(-(sigma_a + sigma_s) L) per channel and draws nothing. A path that never crosses B with sigma_s > 0 draws
+ * the same random numbers as without fog.
+ * Limit: a segment inside a glass sphere that ends on the outside of a sphere nested in it counts as air.
+ * Refused, with tpt_last_error text naming the field ("tpt_set_fog: radius = -1"): a non-finite centre; a radius that is
+ * not finite or not > 0; a sigma that is non-finite or has its sign bit set (-0 included); a g that is NaN or has
+ * |g| >= 1. A refused call leaves the fog as it was.
+ * Lifetime and ordering are tpt_set_media's: the fog belongs to the context, tpt_set_scene keeps it, a fog set before any
+ * scene is stored for the first one, and the call re-packs the current scene with a fog section and uploads it as
+ * tpt_set_scene does (identical bytes are not uploaded again; tpt_last_scene_upload_bytes reports the upload). It never
+ * blocks on the GPU, and calls issued before it keep the fog they were issued with, even while in flight.
+ * Only TPT_MODE_FAST uses fog. While it is set, every fast call (tpt_draw, tpt_trace_rays, tpt_trace_irradiance,
+ * tpt_draw_samples, tpt_trace_samples) runs the slab queue's reference-form instances that carry the textures: an
+ * explicit "fast_variant" other than -1, 3 or 9 is refused, and so is tpt_draw in TPT_MODE_EXACT, TPT_MODE_REFGPU and
+ * TPT_MODE_REFGPU_FAST. Fog combines with media, textures, "max_depth", "environment_sampling" and
+ * "emission_texture_sampling". tpt_draw_aovs and tpt_trace_aovs, which record first hits, do not change. */
+int tpt_set_fog(tpt_context* ctx, const float* fog9);
 /* Camera only (UpdateTest rebuilds it every frame from the aspect ratio, Test.cpp:341). */
 int tpt_set_camera(tpt_context* ctx, const void* camera88);
 

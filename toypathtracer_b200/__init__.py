@@ -90,6 +90,7 @@ def _load_lib():
     L.tpt_set_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_textures.restype = ci
     L.tpt_set_emission_textures.argtypes = [vp, vp, ci, ci, ci, vp, ci, ci]; L.tpt_set_emission_textures.restype = ci
     L.tpt_set_media.argtypes = [vp, vp, ci]; L.tpt_set_media.restype = ci
+    L.tpt_set_fog.argtypes = [vp, vp]; L.tpt_set_fog.restype = ci
     cull = ctypes.c_ulonglong
     L.tpt_mem_alloc.argtypes = [vp, cull, ctypes.POINTER(vp)]; L.tpt_mem_alloc.restype = ci
     L.tpt_mem_free.argtypes = [vp, vp]; L.tpt_mem_free.restype = ci
@@ -485,6 +486,43 @@ class Context:
         media = np.ascontiguousarray(media)
         self._check(self._L.tpt_set_media(self._h, media.ctypes.data if media.size else None, int(media.shape[0])),
                     "tpt_set_media")
+
+    def set_fog(self, centre, radius=None, sigma_a=None, sigma_s=None, g=0.0):
+        """tpt_set_fog: homogeneous fog in the air between the spheres for the fast mode, lit by the lights. The fog fills
+        the ball {centre, radius} minus the spheres; sigma_a is the absorption coefficient (a number, or one per colour
+        channel), sigma_s the grey scattering coefficient and g the Henyey-Greenstein asymmetry. set_fog(None) removes it,
+        as does a fog whose sigmas are all zero. Refused here, as by the library and with its field names: a non-finite
+        centre, a radius that is not finite or not > 0, a sigma that is non-finite or has its sign bit set (-0 included), a
+        g that is NaN or has |g| >= 1. See include/tpt_b200.h for the estimator and which calls use it."""
+        if centre is None:
+            self._check(self._L.tpt_set_fog(self._h, None), "tpt_set_fog")
+            return
+        try:
+            c = np.asarray(centre, np.float64).reshape(-1)
+            sa = np.asarray(sigma_a, np.float64).reshape(-1)
+            rec = [float(radius), float(sigma_s), float(g)]
+        except (TypeError, ValueError):
+            raise TptError("set_fog: centre must be 3 numbers, and radius, sigma_a, sigma_s and g numbers") from None
+        if c.size != 3:
+            raise TptError(f"set_fog: centre must be 3 numbers, not {c.size}")
+        if sa.size == 1:
+            sa = np.repeat(sa, 3)
+        if sa.size != 3:
+            raise TptError(f"set_fog: sigma_a must be a number or 3 numbers, not {sa.size}")
+        with np.errstate(over="ignore"):
+            fog = np.array([*c, rec[0], *sa, rec[1], rec[2]], np.float32)
+        names = ("centre.x", "centre.y", "centre.z", "radius", "sigma_a.r", "sigma_a.g", "sigma_a.b", "sigma_s", "g")
+        for f in range(3):
+            if not np.isfinite(fog[f]):
+                raise TptError(f"set_fog: {names[f]} = {float(fog[f]):g}")
+        if not (np.isfinite(fog[3]) and fog[3] > 0):
+            raise TptError(f"set_fog: radius = {float(fog[3]):g}")
+        for f in range(4, 8):
+            if not np.isfinite(fog[f]) or np.signbit(fog[f]):
+                raise TptError(f"set_fog: {names[f]} = {float(fog[f]):g}")
+        if not abs(float(fog[8])) < 1.0:
+            raise TptError(f"set_fog: g = {float(fog[8]):g}")
+        self._check(self._L.tpt_set_fog(self._h, fog.ctypes.data), "tpt_set_fog")
 
     def set_camera(self, camera: np.ndarray):
         camera = np.ascontiguousarray(camera)

@@ -7,6 +7,7 @@
 #include "tpt_integrator.cuh"
 #include "tpt_env_tables.h"
 #include <cuda.h>      // types only: cuStreamWaitValue32 is resolved at run time (cudaGetDriverEntryPoint), libcuda is not linked
+#include <cmath>
 #include <string>
 #include <vector>
 #include <string.h>
@@ -91,6 +92,8 @@ struct tpt_context
     // tpt_set_media's records (5 floats per sphere id), which also belong to the context: every pack of a scene puts them
     // in its blob, so tpt_set_media re-packs the current scene from its inputs, kept here with the flags it was packed with.
     std::vector<float> media;
+    // tpt_set_fog's record (9 floats; empty: none), which the packs put in the blob the same way.
+    std::vector<float> fog;
     std::vector<Sphere20> sceneSpheres;
     std::vector<Material36> sceneMats;
     std::vector<int> sceneEmissives;
@@ -348,17 +351,19 @@ const char* tpt_last_error(tpt_context* ctx) { return ctx ? ctx->lastError.c_str
 
 } // extern "C"
 
-// The scene upload of tpt_set_scene and tpt_set_media: packs a scene (its inputs as tpt_set_scene takes them, the flags
-// it is packed with and mediaSpheres media records) and makes the blob the scene the calls issued from now on read.
+// The scene upload of tpt_set_scene, tpt_set_media and tpt_set_fog: packs a scene (its inputs as tpt_set_scene takes them,
+// the flags it is packed with, mediaSpheres media records and the fog record fog9, null for none) and makes the blob the
+// scene the calls issued from now on read.
 // Identical bytes are not uploaded again; otherwise the blob goes into the slot the calls in flight are not reading, on
 // the upload stream, and the host never blocks on the GPU. On failure the context's scene is the one it was.
 static int upload_scene(tpt_context* ctx, const char* fn, const Sphere20* spheres, const Material36* mats, int count,
-                        const int* emissives, int emissiveCount, uint32_t packFlags, const float* media5, int mediaSpheres)
+                        const int* emissives, int emissiveCount, uint32_t packFlags, const float* media5, int mediaSpheres,
+                        const float* fog9)
 {
     std::vector<unsigned char> blob;
     SceneBlobLayout L;
     int nLights = 0;
-    pack_scene_blob(spheres, mats, count, emissives, emissiveCount, blob, L, nLights, packFlags, media5, mediaSpheres);
+    pack_scene_blob(spheres, mats, count, emissives, emissiveCount, blob, L, nLights, packFlags, media5, mediaSpheres, fog9);
     ParamPairs pairs;
     build_param_pairs(blob, L, count, pairs);
     const bool halfOk = build_half_pairs(blob, L, count, pairs);
@@ -441,7 +446,7 @@ int tpt_set_scene(tpt_context* ctx, const void* spheres20, const void* materials
     }
     if (int r = upload_scene(ctx, "tpt_set_scene", (const Sphere20*)spheres20, (const Material36*)materials36, count, emissives,
                              emissiveCount, ctx->sceneFlags, ctx->media.empty() ? nullptr : ctx->media.data(),
-                             (int)(ctx->media.size() / 5)))
+                             (int)(ctx->media.size() / 5), ctx->fog.empty() ? nullptr : ctx->fog.data()))
         return r;
     // the inputs tpt_set_media re-packs
     ctx->sceneSpheres.assign((const Sphere20*)spheres20, (const Sphere20*)spheres20 + count);
@@ -474,10 +479,41 @@ int tpt_set_media(tpt_context* ctx, const float* media5, int numSpheres)
         if (int r = upload_scene(ctx, "tpt_set_media", ctx->sceneSpheres.data(), ctx->sceneMats.data(),
                                  (int)ctx->sceneSpheres.size(), ctx->sceneEmissivesGiven ? ctx->sceneEmissives.data() : nullptr,
                                  (int)ctx->sceneEmissives.size(), ctx->scenePackFlags, media.empty() ? nullptr : media.data(),
-                                 numSpheres))
+                                 numSpheres, ctx->fog.empty() ? nullptr : ctx->fog.data()))
             return r;
     }
     ctx->media.swap(media);
+    return 0;
+}
+
+int tpt_set_fog(tpt_context* ctx, const float* fog9)
+{
+    if (!ctx) return (int)cudaErrorInvalidValue;
+    static const char* const kField[9] = {"centre.x", "centre.y", "centre.z", "radius", "sigma_a.r", "sigma_a.g", "sigma_a.b",
+                                          "sigma_s", "g"};
+    if (fog9)
+    {
+        for (int f = 0; f < 3; ++f)
+            if (!std::isfinite(fog9[f])) return fail_msgf(ctx, "tpt_set_fog: %s = %g", kField[f], (double)fog9[f]);
+        if (!(std::isfinite(fog9[3]) && fog9[3] > 0.0f)) return fail_msgf(ctx, "tpt_set_fog: radius = %g", (double)fog9[3]);
+        for (int f = 4; f < 8; ++f)
+            if (!env_channel_ok(fog9[f])) return fail_msgf(ctx, "tpt_set_fog: %s = %g", kField[f], (double)fog9[f]);
+        if (!(fabsf(fog9[8]) < 1.0f)) return fail_msgf(ctx, "tpt_set_fog: g = %g", (double)fog9[8]);
+    }
+    // a record whose sigmas are all zero is no fog: stored as none, so the blob keeps the plain scene's bytes
+    std::vector<float> fog;
+    if (has_fog(fog9)) fog.assign(fog9, fog9 + 9);
+    if (ctx->haveScene)
+    {
+        CK(cudaSetDevice(ctx->device), "cudaSetDevice");
+        if (int r = upload_scene(ctx, "tpt_set_fog", ctx->sceneSpheres.data(), ctx->sceneMats.data(),
+                                 (int)ctx->sceneSpheres.size(), ctx->sceneEmissivesGiven ? ctx->sceneEmissives.data() : nullptr,
+                                 (int)ctx->sceneEmissives.size(), ctx->scenePackFlags,
+                                 ctx->media.empty() ? nullptr : ctx->media.data(), (int)(ctx->media.size() / 5),
+                                 fog.empty() ? nullptr : fog.data()))
+            return r;
+    }
+    ctx->fog.swap(fog);
     return 0;
 }
 
@@ -1008,6 +1044,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     if (mode != TPT_MODE_FAST && (ctx->scene.layout.flags & kSceneMedia))
         return fail_msg(ctx, "tpt_draw: the scene has media, and only TPT_MODE_FAST draws use them (clear them with "
                              "tpt_set_media(ctx, NULL, 0) for exact and reference-GPU draws)");
+    if (mode != TPT_MODE_FAST && (ctx->scene.layout.flags & kSceneFog))
+        return fail_msg(ctx, "tpt_draw: the scene has fog, and only TPT_MODE_FAST draws use it (clear it with "
+                             "tpt_set_fog(ctx, NULL) for exact and reference-GPU draws)");
     if (mode != TPT_MODE_FAST && ctx->maxDepth != kRefMaxDepth)
         return fail_msgf(ctx, "tpt_draw: \"max_depth\" is %d, and only TPT_MODE_FAST draws use it (set it back to 10 for "
                               "exact and reference-GPU draws)", ctx->maxDepth);
@@ -1018,7 +1057,7 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     SceneDev scene;
     if (int r = begin_call(ctx, cudaStreamArg, &stream, &scene)) return r;
     // only the slab queue's reference-form 6-CTA and 768-thread instances sample the environment, look up textures,
-    // trace media and take the call's depth cap
+    // trace media and fog and take the call's depth cap
     const bool envSampling = (scene.layout.flags & kSceneEnvSampling) != 0;
     const bool textured = (scene.layout.flags & kSceneAnyTextures) != 0;
     if (envSampling && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
@@ -1034,6 +1073,9 @@ int tpt_draw(tpt_context* ctx, int frameCount, int numFrames, int width, int hei
     }
     if ((scene.layout.flags & kSceneMedia) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
         return fail_msgf(ctx, "tpt_draw: the scene has media (tpt_set_media), and fast_variant %d does not trace them: use -1 "
+                              "(auto), 3 or 9", ctx->fastVariant);
+    if ((scene.layout.flags & kSceneFog) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
+        return fail_msgf(ctx, "tpt_draw: the scene has fog (tpt_set_fog), and fast_variant %d does not trace it: use -1 "
                               "(auto), 3 or 9", ctx->fastVariant);
     if ((scene.layout.flags & kSceneDepth) && ctx->fastVariant >= 0 && !fast_variant_info(ctx->fastVariant).referenceQueue)
         return fail_msgf(ctx, "tpt_draw: \"max_depth\" is %d, and fast_variant %d keeps the depth cap at 10: use -1 (auto), 3 "

@@ -103,6 +103,7 @@ __device__ __forceinline__ SceneView make_view(const unsigned char* smemBase, co
     v.matB = (const Q4*)pick(L.offMatB);
     v.matRi = (const float*)pick(L.offMatRi);
     v.media = (const Q4*)pick(media_offset(L.offMatRi, count));
+    v.fog = (const Q4*)pick(fog_offset(L.offMatRi, count, L.flags));
     v.count = count;
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = nLights;

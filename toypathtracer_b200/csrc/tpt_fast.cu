@@ -885,7 +885,10 @@ __device__ __forceinline__ void duff_basis(V3 w, V3& su, V3& sv)
     sv = v3(ob, sgn + w.y * w.y * oa, -w.y);
 }
 
-__device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l)
+// TEX with fogG (a fog scatter vertex, lambert_next): the weight is omega x the fog's phase function at cos = l . nl (nl
+// holds the incoming direction there; fogG points at the fog's {g, ...}) instead.
+template <bool TEX = false>
+__device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 nl, uint32_t& rng, V3& l, const Q4* fogG = nullptr)
 {
     V3 sw;
     const float cosAMax = light_cone_cos(Lr, o, sw);
@@ -901,6 +904,8 @@ __device__ __forceinline__ float sample_light_cone(const LightRec Lr, V3 o, V3 n
     __sincosf(phi, &sp, &cp);
     l = su * (cp * sinA) + sv * (sp * sinA) + sw * cosA;
     float omega = 2.0f * TPT_PI * (1.0f - cosAMax);
+    if constexpr (TEX)
+        if (fogG) return omega * hg_phase(dot(l, nl), fogG->x);
     float dl = dot(l, nl);
     float m = (0.0f < dl) ? dl : 0.0f;
     return m * omega * (1.0f / TPT_PI);
@@ -958,6 +963,83 @@ __device__ __forceinline__ bool medium_step(const SceneView& sc, QPath& st, int 
         }
     }
     st.thr = st.thr * transmittance(m, t);
+    return false;
+}
+
+// ---- fog between the spheres (tpt_set_fog, kSceneFog; DESIGN §3.16)
+// QPath::mid of a fog scatter vertex on its way through lambert_next. A Lambert vertex's mid is its sphere (0..count) or,
+// from tpt_trace_irradiance, the caller's id, which begin_vertex keeps at -1 or above in the instances that trace fog: no
+// light is excluded (next_light), and the mark cannot be a caller's.
+constexpr int kMidFog = -2;
+// QPath::kind of the path ray that leaves a fog scatter vertex. It and the vertex's cone rays start at distance 0 rather
+// than TPT_MIN_T: the scatter point lies in air, but it may lie within TPT_MIN_T of a surface, which such a ray would
+// skip (into glass at an angle past the critical one, where total internal reflection then keeps the path until the
+// cap). path_step sets it back to 0 once the ray is traced.
+constexpr int kKindFogPath = INT_MAX;
+
+// The fog length L of the segment o + s d, s in [0, t], and where it starts, max(t_in, 0), in tin (fog_chord).
+__device__ __forceinline__ float fog_length(const SceneView& sc, V3 o, V3 d, float t, float& tin)
+{
+    const Q4 b = sc.fog[0];
+    return fog_chord(o.x, o.y, o.z, d.x, d.y, d.z, t, b.x, b.y, b.z, b.w, &tin);
+}
+
+// A shadow ray's factor over its segment of length t in air: exp(-(sigma_a + sigma_s) L) per channel, no draw.
+__device__ __forceinline__ V3 fog_transmittance(const SceneView& sc, V3 o, V3 d, float t)
+{
+    float tin;
+    const float L = fog_length(sc, o, d, t, tin);
+    const Q4 m = sc.fog[1];
+    return transmittance(Q4{m.x + m.w, m.y + m.w, m.z + m.w, 0.0f}, L);
+}
+
+// The fog on a path ray's segment of length t in air (it ended on the outside face of a sphere, or left the scene with
+// t = TPT_MAX_T): with a fog length L > 0 and sigma_s > 0 one free-flight distance t_s = -ln(1 - u) / sigma_s is drawn
+// along the fog part. Returns true when the path scattered at o + d (max(t_in, 0) + t_s), t_s < L (the hit or miss is
+// not shaded): past the call's depth cap it ends with nothing added (*finished); otherwise the throughput takes
+// exp(-sigma_a t_s) and two more draws give a Henyey-Greenstein direction. Without light sampling the path goes on along
+// it as a path ray whose next hit adds its emission (depth + 1). With it, the vertex is set up like a Lambert vertex for
+// lambert_next (wantLight): nextDir the HG direction, thrAlb the throughput, nl the incoming direction, mid kMidFog and
+// doMaterialE false (no environment sample); lambert_next samples every light and then bounces (depth + 1). Otherwise
+// the throughput takes exp(-sigma_a L) and the caller shades the hit or the miss.
+template <int LS>
+__device__ __forceinline__ bool fog_step(const SceneView& sc, QPath& st, float t, bool& finished, bool& wantLight)
+{
+    float tin;
+    const float L = fog_length(sc, st.o, st.d, t, tin);
+    if (!(L > 0.0f)) return false;
+    const Q4 m = sc.fog[1];
+    if (m.w > 0.0f)
+    {
+        const float ts = __fdividef(-__logf(1.0f - RandomFloat01(st.rng)), m.w);
+        if (ts < L)
+        {
+            if (st.depth >= sc.maxDepth) { finished = true; return true; }
+            st.thr = st.thr * transmittance(m, ts);
+            st.o = st.o + st.d * (tin + ts);
+            const float xi1 = RandomFloat01(st.rng);
+            const float xi2 = RandomFloat01(st.rng);
+            const V3 dir = hg_sample(st.d, sc.fog[2].x, xi1, xi2);
+            if (LS == kLsOff)
+            {
+                st.d = dir;
+                st.doMaterialE = true;
+                st.kind = kKindFogPath;
+                ++st.depth;
+            }
+            else
+            {
+                st.nextDir = dir;
+                st.thrAlb = st.thr;
+                st.nl = st.d;
+                st.mid = kMidFog;
+                st.doMaterialE = false;
+                wantLight = true;
+            }
+            return true;
+        }
+    }
+    st.thr = st.thr * transmittance(m, L);
     return false;
 }
 
@@ -1223,11 +1305,13 @@ __device__ __forceinline__ bool sample_emit(const SceneView& sc, const LightRec&
 // bounce, which keeps its pdf_b in pend for its miss (fast_sky_mis), or -1 where the vertex took no sample.
 // TEX with kSceneEmitSampling: after the cone ray of light coneOf (>= 0), that light's texture sample (sample_emit) and its
 // shadow ray, which comes back with lightFrom = coneOf + 1 and coneOf -1.
+// TEX at a fog scatter vertex (mid kMidFog, fog_step): every light's cone weighted by the phase function, no texture or
+// environment sample, then the bounce.
 template <int LS, int ENVM = 1, bool TEX = false>
 __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int lightFrom, int coneOf = -1)
 {
     if constexpr (TEX)
-        if (coneOf >= 0 && (sc.flags & kSceneEmitSampling) && sample_emit(sc, sc.lights[coneOf], st))
+        if (coneOf >= 0 && (sc.flags & kSceneEmitSampling) && st.mid != kMidFog && sample_emit(sc, sc.lights[coneOf], st))
         {
             st.kind = kKindEmit - coneOf;
             return;
@@ -1235,7 +1319,10 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
     const int j = LS == kLsOff ? sc.nLights : next_light(sc, lightFrom, st.mid);
     if (j < sc.nLights)
     {
-        st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
+        if constexpr (TEX)
+            st.pend = sample_light_cone<true>(sc.lights[j], st.o, st.nl, st.rng, st.d, st.mid == kMidFog ? sc.fog + 2 : nullptr);
+        else
+            st.pend = sample_light_cone(sc.lights[j], st.o, st.nl, st.rng, st.d);
         st.kind = 1 + j;
     }
     else
@@ -1252,7 +1339,8 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
         }
         st.d = st.nextDir;
         st.thr = st.thrAlb;
-        st.kind = 0;
+        if constexpr (TEX) st.kind = st.mid == kMidFog ? kKindFogPath : 0;
+        else st.kind = 0;
         if constexpr (ENVM == 2) st.pend = envSampled ? fmaxf(dot(st.nextDir, st.nl), 0.0f) * (1.0f / TPT_PI) : -1.0f;
         st.doMaterialE = LS == kLsRuntime && emission_after_lambert(sc);
         ++st.depth;
@@ -1273,13 +1361,19 @@ __device__ __forceinline__ void lambert_next(const SceneView& sc, QPath& st, int
 // slab queue's instances with ENVM 2 and their light-sampling-off twins; pick_queue runs them while either is set), and
 // where its kSceneMedia is set, a path ray that ends on the inside face of a glass sphere runs medium_step first. TEX also
 // takes the call's depth cap (sc.maxDepth, "max_depth") for the reference's, with roulette past it where it is larger.
+// Where its kSceneFog is set, a path ray in air (a miss, or a hit on an outside face) runs fog_step first, and a shadow
+// ray in air takes the fog's transmittance (fog_transmittance).
 template <int LS, int ENVM = 1, bool NEXT = true, bool TEX = false, class Hitter>
 __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsigned& rc, const Hitter& hitter)
 {
     // ---- intersect
     float t = TPT_MAX_T;
     int id = -1;
-    if (st.active) { id = hitter.hit(sc, st.o, st.d, TPT_MIN_T, TPT_MAX_T, t); ++rc; }
+    // TEX: the rays that leave a fog scatter point (its path ray, and its cone rays: kind > 0 at mid kMidFog) start at 0
+    float tMin = TPT_MIN_T;
+    if constexpr (TEX)
+        if (st.kind == kKindFogPath || (st.kind > 0 && st.mid == kMidFog)) tMin = 0.0f;
+    if (st.active) { id = hitter.hit(sc, st.o, st.d, tMin, TPT_MAX_T, t); ++rc; }
 
     // ---- shade
     bool wantLight = false;
@@ -1288,9 +1382,15 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
     bool finished = false;
     if (st.active)
     {
-        if (LS == kLsOff || st.kind == 0)
+        if (LS == kLsOff || st.kind == 0 || (TEX && st.kind == kKindFogPath))
         {
-            if (id < 0)
+            if constexpr (TEX) st.kind = 0;
+            // a miss runs in air to TPT_MAX_T: the fog may scatter the path before it leaves
+            bool fogged = false;
+            if constexpr (TEX)
+                if (id < 0 && (sc.flags & kSceneFog)) fogged = fog_step<LS>(sc, st, TPT_MAX_T, finished, wantLight);
+            if (fogged) {}
+            else if (id < 0)
             {
                 if constexpr (ENVM == 2) st.col = st.col + st.thr * fast_sky_mis(sc, st);
                 else if constexpr (ENVM == 1) st.col = st.col + st.thr * fast_sky(st.d, sc);
@@ -1316,13 +1416,16 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                 }
                 // the hit is not shaded when, past the reference's depth in a call whose "max_depth" is larger, Russian
                 // roulette ends the path first (roulette), or when the path segment ran inside a glass sphere with a
-                // medium and scattered inside it (medium_step; otherwise the medium absorbs along it)
+                // medium and scattered inside it (medium_step; otherwise the medium absorbs along it), or ran in air and
+                // scattered in the fog (fog_step; otherwise the fog absorbs along it)
                 bool unshaded = false;
                 if constexpr (TEX)
                 {
                     if (sc.maxDepth > TPT_MAX_DEPTH && st.depth >= TPT_MAX_DEPTH && roulette(st)) unshaded = finished = true;
                     else if ((sc.flags & kSceneMedia) && mtype == kDielectric && dot(st.d, normal) > 0.0f)
                         unshaded = medium_step(sc, st, mid, t, finished);
+                    else if ((sc.flags & kSceneFog) && !(dot(st.d, normal) > 0.0f))
+                        unshaded = fog_step<LS>(sc, st, t, finished, wantLight);
                 }
                 // the depth cap: the reference's in every instance but TEX's, which take the call's
                 const int maxDepth = TEX ? sc.maxDepth : TPT_MAX_DEPTH;
@@ -1380,7 +1483,13 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
         else if (ENVM == 2 && st.kind == kKindEnv)
         {
             // the environment sample's shadow ray (sample_env); after it, the bounce
-            if (id < 0) st.col = st.col + (st.thrAlb * env_radiance(sc, st.d)) * st.pend;
+            if (id < 0)
+            {
+                V3 e = env_radiance(sc, st.d);
+                if constexpr (TEX)
+                    if (sc.flags & kSceneFog) e = e * fog_transmittance(sc, st.o, st.d, TPT_MAX_T);
+                st.col = st.col + (st.thrAlb * e) * st.pend;
+            }
             wantLight = true; lightFrom = sc.nLights + 1;
         }
         else
@@ -1403,7 +1512,7 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                         {
                             const V3 x = st.o + st.d * t;
                             const V3 n = (x - v3(Lj.cx, Lj.cy, Lj.cz)) * sc.invRadius[id];
-                            if (!texRay && (sc.flags & kSceneEmitSampling))
+                            if (!texRay && (sc.flags & kSceneEmitSampling) && st.mid != kMidFog)
                             {
                                 float P;
                                 e = sphere_texture_layer<true>(sc.emit, layer, e, n, &P);
@@ -1413,6 +1522,10 @@ __device__ __forceinline__ bool path_step(const SceneView& sc, QPath& st, unsign
                                 e = sphere_texture_layer(sc.emit, layer, e, n);
                         }
                     }
+                // a shadow ray that meets its light's outside face ran in air: the fog's transmittance along it
+                if constexpr (TEX)
+                    if ((sc.flags & kSceneFog) && !(dot(st.d, st.o + st.d * t - v3(Lj.cx, Lj.cy, Lj.cz)) > 0.0f))
+                        e = e * fog_transmittance(sc, st.o, st.d, t);
                 st.col = st.col + (st.thrAlb * e) * pend;
             }
             wantLight = true; lightFrom = j + 1;
@@ -1433,7 +1546,7 @@ __device__ __forceinline__ void begin_vertex(const SceneView& sc, QPath& st, int
     st.nl = st.d;
     st.nextDir = M<false>::normalize(st.d + RandomUnitVector<false>(st.rng));
     st.thrAlb = v3(1, 1, 1);
-    st.mid = mid;
+    st.mid = TEX ? max(mid, -1) : mid;     // (TEX: a negative id never matches a light, and kMidFog marks fog vertices)
     lambert_next<LS, ENVM, TEX>(sc, st, 0);     // (begin_path left doMaterialE true: the point takes an environment sample)
 }
 

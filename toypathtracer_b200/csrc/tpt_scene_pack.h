@@ -4,6 +4,7 @@
 // multiple of 4 with "impossible" spheres (Cpp/Source/Maths.h:370-388).
 #pragma once
 #include "tpt_types.h"
+#include "tpt_fog.h"
 #include <vector>
 #include <string.h>
 #include <math.h>
@@ -22,7 +23,12 @@ TPT_PACK_HD inline uint32_t align16(uint32_t x) { return (x + 15u) & ~15u; }
 // {sigma_a.rgb, sigma_s}, then (count + 1) floats g, each part padded to 16 B; entry [count] is zero. Its offset, for the
 // pack and for the kernels' views.
 TPT_PACK_HD inline uint32_t media_offset(uint32_t offMatRi, int count) { return offMatRi + align16((uint32_t)(count + 1) * 4u); }
-inline uint32_t media_bytes(int count) { return align16((uint32_t)(count + 1) * 16u) + align16((uint32_t)(count + 1) * 4u); }
+TPT_PACK_HD inline uint32_t media_bytes(int count) { return align16((uint32_t)(count + 1) * 16u) + align16((uint32_t)(count + 1) * 4u); }
+// The fog section (tpt_set_fog, kSceneFog), kFogBytes, follows the media section where the blob has one, else matRi.
+TPT_PACK_HD inline uint32_t fog_offset(uint32_t offMatRi, int count, uint32_t flags)
+{
+    return media_offset(offMatRi, count) + ((flags & kSceneMedia) ? media_bytes(count) : 0u);
+}
 
 inline SceneBlobLayout scene_blob_layout(int count, int nLights)
 {
@@ -46,14 +52,19 @@ inline SceneBlobLayout scene_blob_layout(int count, int nLights)
 
 // A medium record of tpt_set_media {sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g}: "no medium" when both sigmas are zero.
 inline bool has_medium(const float* m5) { return m5[0] != 0.0f || m5[1] != 0.0f || m5[2] != 0.0f || m5[3] != 0.0f; }
+// A fog record of tpt_set_fog {c.x, c.y, c.z, R, sigma_a.r, sigma_a.g, sigma_a.b, sigma_s, g}: "no fog" when its sigmas
+// are all zero.
+inline bool has_fog(const float* f9) { return f9 && has_medium(f9 + 4); }
 
 // emissives == nullptr: derive the list like UpdateTest (Test.cpp:333-338).
 // media5: mediaSpheres records of tpt_set_media (null: none). The blob gets the media section, and kSceneMedia, only when a
 // sphere below `count` has a medium; otherwise its bytes are those of the scene without media.
+// fog9: tpt_set_fog's record (null: none). The blob gets the fog section, and kSceneFog, only when it has a non-zero
+// sigma; otherwise its bytes are those of the scene without fog.
 inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int count,
                             const int* emissives, int emissiveCount,
                             std::vector<unsigned char>& blob, SceneBlobLayout& L, int& nLights, uint32_t sceneFlags = 0,
-                            const float* media5 = nullptr, int mediaSpheres = 0)
+                            const float* media5 = nullptr, int mediaSpheres = 0, const float* fog9 = nullptr)
 {
     const int nMedia = media5 ? (mediaSpheres < count ? mediaSpheres : count) : 0;
     bool anyMedium = false;
@@ -65,11 +76,17 @@ inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int
             if (mats[i].emissive[0] > 0 || mats[i].emissive[1] > 0 || mats[i].emissive[2] > 0) em.push_back(i);
     nLights = (int)em.size();
     L = scene_blob_layout(count, nLights);
-    L.flags = sceneFlags & ~(uint32_t)kSceneMedia;
+    L.flags = sceneFlags & ~(uint32_t)(kSceneMedia | kSceneFog);
     if (anyMedium)
     {
         L.flags |= kSceneMedia;
         L.totalBytes += media_bytes(count);    // geomBytes stays: the section is material data
+    }
+    const bool fog = has_fog(fog9);
+    if (fog)
+    {
+        L.flags |= kSceneFog;
+        L.totalBytes += kFogBytes;
     }
     int simdCount = (count + 3) / 4 * 4;
     blob.assign(L.totalBytes, 0);
@@ -113,6 +130,11 @@ inline void pack_scene_blob(const Sphere20* spheres, const Material36* mats, int
             media[i].x = m[0]; media[i].y = m[1]; media[i].z = m[2]; media[i].w = m[3];
             g[i] = m[4];
         }
+    }
+    if (fog)
+    {
+        float* f = (float*)(blob.data() + fog_offset(L.offMatRi, count, L.flags));
+        for (int k = 0; k < 9; ++k) f[k] = fog9[k];
     }
     for (int j = 0; j < nLights; ++j)
     {
@@ -209,6 +231,7 @@ inline SceneView scene_view_from_blob(const unsigned char* base, const SceneBlob
     v.matB = (const Q4*)(base + L.offMatB);
     v.matRi = (const float*)(base + L.offMatRi);
     v.media = (const Q4*)(base + media_offset(L.offMatRi, count));
+    v.fog = (const Q4*)(base + fog_offset(L.offMatRi, count, L.flags));
     v.count = count;
     v.simdCount = (count + 3) / 4 * 4;
     v.nLights = sampled_lights(L.flags, nLights);

@@ -59,6 +59,7 @@ struct SceneView
     const Q4* matB;
     const float* matRi;
     const Q4* media;      // kSceneMedia: {sigma_a.rgb, sigma_s}[count + 1], then g[count + 1] (media_offset, tpt_scene_pack.h)
+    const Q4* fog;        // kSceneFog: {c.xyz, R}, {sigma_a.rgb, sigma_s}, {g, 0, 0, 0} (fog_offset, tpt_scene_pack.h)
     const LightRec* lights;
     int count, simdCount, nLights;
     uint32_t flags;       // kScene* bits
@@ -114,14 +115,17 @@ struct SceneBlobLayout
 // kSceneDepth ("max_depth" other than the reference's 10 for the call, set by begin_call): the value travels in bits
 // kSceneDepthShift.. of the call's flags (depth_flags, scene_max_depth), and the same instances end paths at that depth
 // instead, with Russian roulette past depth 10 when it is larger (path_step).
+// kSceneFog (tpt_set_fog, set by the pack when the context's fog has a non-zero sigma): the blob carries the fog section
+// behind the media section, and the same instances absorb and scatter along path segments in air inside the fog's ball,
+// sample the lights at fog scatter vertices and attenuate shadow rays in air (fog_step, fog_transmittance).
 enum SceneFlags : uint32_t { kSceneMitsuba = 1u, kSceneNoLightSampling = 2u, kSceneEnvironment = 4u, kSceneEnvSampling = 8u,
                              kSceneTextures = 16u, kSceneEmissionTextures = 32u, kSceneEmitSampling = 64u, kSceneMedia = 128u,
-                             kSceneDepth = 256u };
+                             kSceneDepth = 256u, kSceneFog = 512u };
 // Either texture set: the calls that have one run the instances that look textures up (pick_queue, fast_auto_variant).
 constexpr uint32_t kSceneAnyTextures = kSceneTextures | kSceneEmissionTextures;
 // What only the slab queue's reference-form instances (sweep form 0, path_step's ENVM 2 and TEX) compute: a call with any of
 // these runs them (pick_queue, fast_auto_variant, tpt_draw's variant checks).
-constexpr uint32_t kSceneRefForm = kSceneEnvSampling | kSceneAnyTextures | kSceneMedia | kSceneDepth;
+constexpr uint32_t kSceneRefForm = kSceneEnvSampling | kSceneAnyTextures | kSceneMedia | kSceneDepth | kSceneFog;
 
 // "max_depth": the reference's compile-time cap (TPT_MAX_DEPTH, tpt_integrator.cuh) is the default and the depth from
 // which Russian roulette runs; the option takes 1..kMaxPathDepth. A per-call value, never part of the scene's blob or the
